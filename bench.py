@@ -11,7 +11,7 @@ data-path collective (weak scaling: every rank evaluates its own 1M rows per ste
 
 Timing: W warm-up steps, then exactly K steps bracketed by barrier + synchronize, CUDA events on
 the launching stream, MAX over ranks.  Inputs are resident in HBM; four distinct q batches
-(4 x 56 MB) are rotated and every step writes 464 MB, so nothing is served from the 126 MB L2.
+(4 x 56 MB) are rotated and every step writes 464 MB, so nothing is served from the 50 MB L2.
 
 Extra objects in the JSON line (see DESIGN.md "Measurement"):
   roofline      algorithmic bytes (520 B/eval, SURVEY 8d) / average kernel time vs MEASURED_PEAKS hbm_gbs
@@ -25,7 +25,7 @@ Extra objects in the JSON line (see DESIGN.md "Measurement"):
                 ik_lm_panda_f32_100k_* (configs[3], both protocols of SURVEY 8d), fkj_ur10_f32_1M (configs[4]
                 per-GPU shard; at N > 1 it runs on every rank with seed 3 + rank: fkj_ur10_f32_sharded)
   gather        (N > 1) NCCL reassembly of the UR10 result shards, outside the metric: one all-gather of the
-                packed (T|J) buffer and a gather to rank 0, achieved GB/s into a rank against 900 GB/s
+                packed (T|J) buffer and a gather to rank 0, achieved GB/s into a rank against 450 GB/s
   clocks        SM clocks / throttle reasons sampled through NVML during the timed region
   gpu_launches  kernels this library launched inside the timed region
 """
@@ -48,7 +48,7 @@ N_JOINTS = 7
 BYTES_PER_EVAL = (7 + 16 + 42) * 8  # SURVEY 8d: q + T + J0, fp64
 METRIC = "Panda 7-DOF fkine+jacob0 evals/sec @ batch 1M"
 WORKLOAD = "panda_ets_fkine_jacob0_f64_batch1M"
-NVLINK_GBS = 900.0  # nominal NVLink 5 bandwidth per direction per GPU (B200_PROFILING.md)
+NVLINK_GBS = 450.0  # nominal NVLink 4 bandwidth per direction per GPU (H100 SXM data sheet: 900 GB/s both directions)
 PARITY_ROWS = 4096
 IK_PARITY_ROWS = 1024
 IK_PROTOCOLS = {  # SURVEY 8d config 4: the notebook protocol and the API default
@@ -65,7 +65,7 @@ def make_config(world):
     """The workload description, identical for both arms (the driver compares them)."""
     return {"workload": WORKLOAD, "rows_per_gpu": ROWS_PER_GPU, "global_batch": ROWS_PER_GPU * world,
             "parallelism": f"rows sharded over {world} rank(s), no data-path collective",
-            "l2": "4 distinct 56 MB q batches rotated + 464 MB written per step (> 126 MB L2)"}
+            "l2": "4 distinct 56 MB q batches rotated + 464 MB written per step (> 50 MB L2)"}
 
 
 # ------------------------------------------------------------------ parity-sample inputs (shared by both legs)
@@ -225,7 +225,7 @@ class ClockSampler(threading.Thread):
         return out
 
 
-# ------------------------------------------------------------------ the B200 arm
+# ------------------------------------------------------------------ the CUDA arm
 def load_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
@@ -233,18 +233,7 @@ def load_peaks():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md: 6.65 TB/s)"
-
-
-def load_traffic(key=WORKLOAD):
-    """dram bytes per launch from the committed ncu --set full capture of that kernel, if any."""
-    p = os.path.join(ROOT, "profiles", "traffic.json")
-    if os.path.exists(p):
-        try:
-            return json.load(open(p)).get(key)
-        except Exception:
-            return None
-    return None
+    return 3350.0, "fallback (H100 SXM data sheet: 3.35 TB/s)"
 
 
 def err_stats(got, ref, atol):
@@ -255,6 +244,20 @@ def err_stats(got, ref, atol):
     d = np.abs(got - ref)
     big = np.abs(ref) >= 1e-6
     return float(d.max()), float((d[big] / np.abs(ref[big])).max()) if big.any() else 0.0
+
+
+DUMP_ROWS = 65_536  # 30 MB of T and J; a whole 1M-row step would be 464 MB
+
+
+def dump_outputs(out_dir, T, J):
+    """T and J of the last timed step at a fixed, seeded sample of rows (ascending), as float64 .npy files."""
+    import torch
+
+    rows = np.sort(np.random.default_rng(7).choice(T.shape[0], DUMP_ROWS, replace=False))
+    idx = torch.from_numpy(rows).to(T.device)
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "fkine_T.npy"), T.index_select(0, idx).cpu().numpy())
+    np.save(os.path.join(out_dir, "jacob0_J.npy"), J.index_select(0, idx).cpu().numpy())
 
 
 def run_b200(args):
@@ -347,6 +350,8 @@ def run_b200(args):
     n0 = rtb.launch_count()
     ms_step = time_steps(step, args.steps, W)
     launches = rtb.launch_count() - n0 - W
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, T, J)
     value = ROWS_PER_GPU * world / (ms_step * 1e-3)
     clocks = sampler.summary(windows[-1:])
     per = time_steps(step, min(args.steps, 200), 0, per_step=True)  # distribution, outside `value`
@@ -370,10 +375,9 @@ def run_b200(args):
     headline_parity = parity_fkj(ets, "panda_fkj", make_q(4242, PARITY_ROWS, 7), np.float64, 1e-10, 1e-12)
 
     # ================================================================ the other BASELINE configs
-    def roof(bytes_per_row, rows, ms, bound="hbm", note=None, traffic_key=None):
+    def roof(bytes_per_row, rows, ms, bound="hbm", note=None):
         a = bytes_per_row * rows / (ms * 1e-3) / 1e9
         r = {"bound": bound, "achieved": a, "peak": peak, "unit": "GB/s", "frac": a / peak,
-             "traffic": load_traffic(traffic_key) if traffic_key else None,
              "algorithmic_bytes_per_launch": bytes_per_row * rows}
         if note:
             r["note"] = note
@@ -425,7 +429,7 @@ def run_b200(args):
             g_ms = time_steps(g0, 5, 2)
             del parts
             # the same reassembly WITHOUT a collective: every rank's kernel writes its shard straight into rank 0's memory
-            # (peer pointer from torch symmetric memory; the pose rows go out as 256-bit stores, the Jacobian tiles as TMA
+            # (peer pointer from torch symmetric memory; the pose rows go out as 128-bit stores, the Jacobian tiles as TMA
             # bulk copies -- over NVLink instead of to local HBM).  Root ingress is the bound: (world - 1) shards.
             fused = None
             try:
@@ -449,7 +453,7 @@ def run_b200(args):
                 ref = [torch.empty_like(TJ) for _ in range(world)] if rank == 0 else None
                 dist.gather(TJ, ref, dst=0)
                 same = bool(torch.equal(sbuf.view(world, -1), torch.stack(ref))) if rank == 0 else None
-                fused = {"ms": f_ms, "GBps_into_root": recv / (f_ms * 1e-3) / 1e9, "frac_of_900GBps": recv / (f_ms * 1e-3) / 1e9 / NVLINK_GBS,
+                fused = {"ms": f_ms, "GBps_into_root": recv / (f_ms * 1e-3) / 1e9, "frac_of_nvlink": recv / (f_ms * 1e-3) / 1e9 / NVLINK_GBS,
                          "identical_to_nccl_gather": same,
                          "how": "k_fkj_fast<float,6> launched with T / J pointing into rank 0's symmetric-memory buffer"}
                 del sbuf
@@ -460,9 +464,9 @@ def run_b200(args):
                         "writing its shard directly into rank 0's memory over NVLink (no collective)",
                 "bytes_per_rank_shard": TJ.numel() * 4, "bytes_received_per_rank": recv,
                 "all_gather_ms": ag_ms, "gather_to_root_ms": g_ms,
-                "GBps": recv / (ag_ms * 1e-3) / 1e9, "frac_of_900GBps": recv / (ag_ms * 1e-3) / 1e9 / NVLINK_GBS,
+                "GBps": recv / (ag_ms * 1e-3) / 1e9, "frac_of_nvlink": recv / (ag_ms * 1e-3) / 1e9 / NVLINK_GBS,
                 "gather_to_root_GBps": recv / (g_ms * 1e-3) / 1e9,
-                "gather_to_root_frac_of_900GBps": recv / (g_ms * 1e-3) / 1e9 / NVLINK_GBS,
+                "gather_to_root_frac_of_nvlink": recv / (g_ms * 1e-3) / 1e9 / NVLINK_GBS,
                 "fused_store_to_root": fused,
                 "kernel_ms": ms, "note": "GB/s = bytes received by one rank / time; the kernel that produced the shard "
                                          "takes kernel_ms, so the reassembly cannot be hidden behind it (SURVEY 8e)",
@@ -496,7 +500,7 @@ def run_b200(args):
             "baseline_config": "configs[2]: Puma560 DHRobot rne (q, qd, qdd) batch 1M fp64",
             "ms": ms, "value": ROWS_PER_GPU / (ms * 1e-3), "unit": "rows/s", "rows": ROWS_PER_GPU, "dtype": "f64",
             "steps": KS, "kernel": rtb.rne_kernel_name(puma) if hasattr(rtb, "rne_kernel_name") else "k_rne<double,6,DH,allrev>",
-            "roofline": roof(24 * 8, ROWS_PER_GPU, ms, note="issue-bound (2-cycle FP64 issue + integer / control): DESIGN 3.4", traffic_key="rne_puma_f64_1M"),
+            "roofline": roof(24 * 8, ROWS_PER_GPU, ms, note="issue-bound (2-cycle FP64 issue + integer / control)"),
             "cpu_baseline": cpu["configs"].get("rne_puma_f64_1M") if cpu else None, "parity": par,
         }
         del rb, tau
@@ -543,8 +547,7 @@ def run_b200(args):
                 "ms": ms, "value": IK_ROWS / (ms * 1e-3), "unit": "solves/s", "rows": IK_ROWS, "dtype": "f32", "steps": 5,
                 "kernel": "k_ik_lm + k_ik_restarts", "launches_per_step": ik_launches,
                 "roofline": roof((16 + 7 + 4) * 4, IK_ROWS, ms, bound="latency",
-                                 note="serial LM iterations per target: latency / issue bound, HBM fraction reported for completeness",
-                                 traffic_key="ik_lm_panda_f32_100k_chan0.1" if name.endswith("chan0.1") else None),
+                                 note="serial LM iterations per target: latency / issue bound, HBM fraction reported for completeness"),
                 "cpu_baseline": cpu["configs"].get(name) if cpu else None, "parity": par,
             }
         del qstar, Tep64, Tep32
@@ -590,7 +593,7 @@ def run_b200(args):
             "config": make_config(world),
             "kernel": "k_fkj_fast<double,7,T,J0> (1 launch per step)",
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                         "traffic": load_traffic(), "peak_source": peak_src,
+                         "peak_source": peak_src,
                          "algorithmic_bytes_per_launch": BYTES_PER_EVAL * ROWS_PER_GPU},
             "step_ms": step_ms,
             "cpu_baseline": hb,
@@ -625,6 +628,9 @@ def main():
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--headline-only", action="store_true", help="skip the secondary configs and the gather")
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR",
+                    help=f"after the timed steps, write T and J of the last one (a seeded sample of {DUMP_ROWS} rows, "
+                         "rank 0) to DIR/fkine_T.npy and DIR/jacob0_J.npy")
     ap.add_argument("--no-fused-gather", action="store_true", help="skip the symmetric-memory store-to-root experiment (N>1)")
     args = ap.parse_args()
     if args.impl == "reference":

@@ -1,5 +1,5 @@
 /*
- * b2kin.h -- C ABI of libb2kin.so: batched serial-chain kinematics / dynamics on B200 (sm_100a).
+ * b2kin.h -- C ABI of libb2kin.so: batched serial-chain kinematics / dynamics on H100 (sm_90a).
  *
  * This is the drop-in boundary for the reference's native fast path
  * (petercorke/robotics-toolbox-python, src/roboticstoolbox/core/).  Each entry point names
@@ -184,7 +184,7 @@ int b2k_rne(b2k_rne_t rne, int dtype, const void *q, const void *qd, const void 
             const double *grav, const double *fext, void *tau, void *stream);
 
 /* Robot-specialised kernels.  For all-revolute arms b2k_rne (and the dynamics entry points below) run a kernel that is
- * generated for THIS robot's link table and compiled for sm_100a at first use (NVRTC): terms whose link parameter is zero
+ * generated for THIS robot's link table and compiled for sm_90a at first use (NVRTC): terms whose link parameter is zero
  * are never emitted, alpha = k pi/2 turns rotations into permutations, constants are folded (csrc/b2k_rne_gen.cpp,
  * b2k_rne_spec.cu).  Results equal the generic kernel's to rounding.  Environment: B2K_RNE_SPEC=0 disables it, =2 makes a
  * failure to specialise an error; B2K_NVRTC_PATH names libnvrtc.so.12 when it is not on the loader path.

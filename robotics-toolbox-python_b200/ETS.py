@@ -308,7 +308,7 @@ class ETS:
         b0 = np.eye(4) if base is None else base
         if not ETS.frames_single_walk:
             # one pose launch per frame over the prefix chains into frame-major memory (each launch re-reads q and
-            # re-walks its prefix); kept selectable for measurement, see DESIGN 3.6
+            # re-walks its prefix); kept selectable for measurement
             frames = B.empty((len(chains) + 1, N, 4, 4), dt, like=qd)
             t = B.require_cuda()
             b0 = np.eye(4) if base is None else base

@@ -1,8 +1,8 @@
-"""b2kin -- Blackwell-native batched robot kinematics & dynamics.
+"""b2kin -- H100-native batched robot kinematics & dynamics.
 
 A drop-in for ONE hot path of petercorke/robotics-toolbox-python: serial-chain forward
 kinematics, geometric Jacobians, DH recursive Newton-Euler and Levenberg-Marquardt IK over an
-(N, n) batch of joint configurations, computed by hand-written sm_100a CUDA kernels behind the
+(N, n) batch of joint configurations, computed by hand-written sm_90a CUDA kernels behind the
 C ABI in include/b2kin.h.  The classes keep the reference's names (ET, ETS, DHRobot, Robot,
 IKSolution, IK_LM, models.*).  The directory name is not a Python identifier; import it as
 

@@ -52,12 +52,12 @@ int b2k_num_sms(int *device_out)
     static std::mutex mu;
     static std::map<int, int> cache;
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess) return 148;
+    if (cudaGetDevice(&dev) != cudaSuccess) return 132;
     if (device_out) *device_out = dev;
     std::lock_guard<std::mutex> lk(mu);
     auto it = cache.find(dev);
     if (it != cache.end()) return it->second;
-    int sms = 148;
+    int sms = 132;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     cache[dev] = sms;
     return sms;

@@ -1,4 +1,4 @@
-// b2k_common.cuh -- shared types between the host-side chain compiler and the sm_100a kernels.
+// b2k_common.cuh -- shared types between the host-side chain compiler and the sm_90a kernels.
 #pragma once
 
 #include <cuda_runtime.h>
@@ -253,7 +253,7 @@ template <> __device__ __forceinline__ void store16<float>(float *p, const float
 }
 // element index of an (N, n) array -> (row, axis).  n is a run-time value: the 64-bit division the plain expression
 // compiles to is a ~100-instruction software routine per element (it, not the 168 B / row of stores, bounded k_jtraj and
-// k_mtraj at 60 us per 1M x 7 samples); arrays below 2^32 elements take the 32-bit division.
+// k_mtraj); arrays below 2^32 elements take the 32-bit division.
 __device__ __forceinline__ void split_elem(long long e, int n, long long total, long long &row, int &j)
 {
     if (total <= 0xffffffffLL) {

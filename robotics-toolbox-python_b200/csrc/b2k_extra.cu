@@ -11,8 +11,8 @@
 // l, l + 32, ... of the row.  Which four J entries an output needs depends only on its position in the row, i.e. on
 // (lane, iteration): the shared-memory offsets are worked out ONCE per thread and kept in registers, so a row costs
 // 8 LDS + 4 flops + one vector store per pair and no index arithmetic (the previous form decoded (a, r, b) and
-// branched per element: ~40 instructions per output, issue-bound at 0.84 ms for 1M Panda rows; one thread per output
-// element with J through L1 was slower still, 1.21 ms).  The next row's J values are fetched while this one is written.
+// branched per element: ~40 instructions per output, issue-bound; one thread per output
+// element with J through L1 was slower still).  The next row's J values are fetched while this one is written.
 template <typename real> struct Pair2;
 template <> struct Pair2<double> { typedef double2 type; };
 template <> struct Pair2<float> { typedef float2 type; };
@@ -80,7 +80,7 @@ __global__ void __launch_bounds__(256) k_hessian(const real *__restrict__ J, lon
 
 // The same Hessian for output arrays that are 16-byte aligned (every torch allocation): a LANE per row, the row's J in
 // registers, every output a compile-time choice of four registers -- no shared-memory operand reads at all (the kernel
-// above spends 8 LDS.64 per output pair, 3.2 bank cycles each: shared-memory bandwidth, not HBM, bounds it at 0.61 ms).
+// above spends 8 LDS.64 per output pair, 3.2 bank cycles each: shared-memory bandwidth, not HBM, bounds it).
 // A block of 4 warps owns a tile of 32 rows; warp w produces the 16-byte units w, w + 4, ... of every row and stores
 // them into a shared-memory image of the tile's output block, which leaves through the TMA engine
 // (cp.async.bulk shared -> global: no LDS / STG instructions).  The row pitch of the image is an odd number of units,
@@ -192,7 +192,7 @@ __global__ void __launch_bounds__(128) k_hessian_tile(const real *__restrict__ J
 // ---- lane-per-row kernels over Jacobian rows: 64-thread blocks, each warp stages its tile of 32 rows (6N reals each)
 // through shared memory so that the global loads / stores are coalesced, and a lane then owns one row in registers.
 // (Reading the rows straight from global memory -- 32 lanes x a 6N-real stride per load instruction -- measured
-// 0.14-0.2 of the HBM rate on 1M Panda rows; profiles/r02_kernels_extra.jsonl.)
+// a small fraction of the HBM rate.)
 #define B2K_XT 64 /* threads per block of the staged kernels: 2 warps x 32 x 60 doubles = 30 KB at n = 10 */
 template <typename real>
 __device__ __forceinline__ void xt_copy(real *dst, const real *src, int count, int lane)
@@ -232,8 +232,7 @@ __global__ void __launch_bounds__(B2K_XT) k_yoshikawa_all(const real *__restrict
 
 // Jd = sum_i H[i] qd[i]  (Robot.jacob0_dot, Robot.py:964-1099: np.tensordot(H, qd, (0, 0))) without materialising H:
 // Jd[r, b] = sum_a qd[a] * H[a, r, b], H from J as in k_hessian (methods.cpp:16-32).  One lane per row, J and qd in
-// registers, the tile doubling as the output stage.  (The first version was a warp per row over shared memory:
-// 0.57 ms for 1M Panda rows, 0.19 of HBM.)
+// registers, the tile doubling as the output stage.  (The first version, a warp per row over shared memory, was slower.)
 template <typename real, int N>
 __global__ void __launch_bounds__(B2K_XT) k_jacob_dot_lane(const real *__restrict__ J, const real *__restrict__ qd, long long nrows,
                                                            real *__restrict__ Jd)
@@ -323,13 +322,13 @@ __global__ void __launch_bounds__(128) k_yoshikawa(const real *__restrict__ J, l
 // pivot search, which would need run-time row indices -- i.e. local memory) gives m = sqrt(det A) = prod L_jj and the
 // columns G[:, k] = A^-1 J[:, k]; then  sum_{a,b} (J H_i^T)[a,b] A^-1[a,b] = sum_{b,k} H_i[b,k] G[b,k]  (A^-1 is
 // symmetric), which needs the Hessian terms once per (i, b, k) instead of once per (i, a, b, k): ~1 800 operations per
-// row instead of ~14 000.  Measured, 1M Panda rows fp64: 4.19 ms with the general kernel below (na read at run time,
-// Gauss-Jordan with pivoting, every array in local memory).
+// row instead of ~14 000.  The general kernel below (na read at run time, Gauss-Jordan with pivoting, every array in
+// local memory) is far slower.
 template <typename real, int N>
 __global__ void __launch_bounds__(128) k_jacobm_all(const real *__restrict__ J, long long nrows, real *__restrict__ Jm)
 {
     // (rows are read straight from global memory here: with ~250 live registers the staged form -- 64-thread blocks,
-    // 10 KB of shared memory per warp -- measured 0.167 ms against 0.125 ms for 1M Panda rows)
+    // 10 KB of shared memory per warp -- measured slower)
     const long long row = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (row >= nrows) return;
     const real *jr = J + row * (6 * N);
@@ -454,7 +453,7 @@ __global__ void __launch_bounds__(128) k_jacobm(const real *__restrict__ J, long
 // values -- accurate to rounding even next to a singularity, where squaring into the Gram matrix would lose half the digits.
 // All six axes selected: the shape of the working matrix (P x D = max(6,N) x min(6,N)) is known at compile time, every
 // index is a constant, the 6N values live in registers (the general kernel below keeps them in local memory because its
-// shape is read from the axes mask: 1.35 ms against the 0.06 ms the traffic needs, 1M Panda rows).
+// shape is read from the axes mask, far from what the traffic needs).
 template <typename real, int N>
 __global__ void __launch_bounds__(128) k_singular_all(const real *__restrict__ J, long long nrows, int kind, real *__restrict__ m)
 {

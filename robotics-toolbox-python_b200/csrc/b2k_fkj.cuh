@@ -1,4 +1,4 @@
-// b2k_fkj.cuh -- forward kinematics + geometric Jacobian kernels for sm_100a.
+// b2k_fkj.cuh -- forward kinematics + geometric Jacobian kernels for sm_90a.
 //
 // Mapping (DESIGN.md "Kernel K12"): a warp owns a TILE of 32 joint configurations.  Lane l
 // walks the serial chain of row (tile*32 + l) entirely in registers -- pose as four 3-vectors
@@ -8,8 +8,8 @@
 // its T / J blocks between HBM and registers through a per-warp shared-memory stage so that
 // every global access is a fully coalesced warp transaction:
 //     q tile  (32 x ldq)  : 16-byte cp.async (LDGSTS) straight into smem; one row per lane read back
-//     T tile  (32 x 16)   : one pose row per lane, 256-bit stores straight from registers
-//                           (a row is 128 B / 64 B contiguous: full sectors without staging)
+//     T tile  (32 x 16)   : lean kernels stage it like J and drain it coalesced; the general kernels store one
+//                           pose row per lane with 128-bit stores straight from registers
 //     J tile  (32 x 6n)   : registers -> 16-byte vector STS into a stage that is the exact image of
 //                           the output block -> ONE TMA bulk copy (cp.async.bulk, SASS UBLKCP)
 // Two forms of every walk: the general kernels (k_fkj_forward / k_fkj_backward: any row stride, jindex
@@ -248,7 +248,7 @@ __device__ __forceinline__ void je_col_pri(const Pose<real> &U, real sg, real *c
 //   1 "DH-like": every joint is an unflipped Rz and every inter-joint constant has the Rx form
 //     [[1,0,0],[0,a,b],[0,c,d]] (+ translation) -- standard / modified DH robots and the Panda ETS.
 //     Straight-line code: no switches (the compiler if-converts small uniform switches into
-//     select chains, ncu profiles/r01_fkj_v2.md), all n sincos evaluated as one interleaved batch.
+//     select chains), all n sincos evaluated as one interleaved batch.
 //   0 generic: any axis / flip / constant, runtime (uniform) switches.
 //   TRIG = 1 (the IK loop, whose iterates leave [-pi, pi] in some lanes of most warps): fp32 angles are reduced once
 //   and go to the special-function unit whatever their size, so a warp never runs two sincos paths back to back.
@@ -487,28 +487,21 @@ __device__ __forceinline__ void pose_to_row(const Pose<real> &T, real *row)
 }
 
 // The pose block needs no transposition through shared memory: a row is 16 contiguous reals
-// (128 B in fp64, 64 B in fp32), so each lane stores its own row with full-sector vector stores
-// straight from registers.
+// (128 B in fp64, 64 B in fp32), so each lane stores its own row with 128-bit vector stores (the
+// widest sm_90 has; two per 32-byte sector) straight from registers.
 template <typename real>
 __device__ __forceinline__ void store_pose_row(const Pose<real> &T, real *grow)
 {
     real row[16];
     pose_to_row(T, row);
     if constexpr (sizeof(real) == 8) {
-        double4 *g = reinterpret_cast<double4 *>(grow);
+        double2 *g = reinterpret_cast<double2 *>(grow);
 #pragma unroll
-        for (int u = 0; u < 4; u++) { // 256-bit stores (sm_100): one full 32-byte sector per instruction per lane
-            asm volatile("st.global.v4.f64 [%0], {%1, %2, %3, %4};" ::"l"(g + u), "d"(row[4 * u]), "d"(row[4 * u + 1]),
-                         "d"(row[4 * u + 2]), "d"(row[4 * u + 3]) : "memory");
-        }
+        for (int u = 0; u < 8; u++) g[u] = make_double2(row[2 * u], row[2 * u + 1]);
     } else {
         float4 *g = reinterpret_cast<float4 *>(grow);
 #pragma unroll
-        for (int u = 0; u < 2; u++) {
-            asm volatile("st.global.v8.f32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(g + 2 * u), "f"(row[8 * u]),
-                         "f"(row[8 * u + 1]), "f"(row[8 * u + 2]), "f"(row[8 * u + 3]), "f"(row[8 * u + 4]),
-                         "f"(row[8 * u + 5]), "f"(row[8 * u + 6]), "f"(row[8 * u + 7]) : "memory");
-        }
+        for (int u = 0; u < 4; u++) g[u] = make_float4(row[4 * u], row[4 * u + 1], row[4 * u + 2], row[4 * u + 3]);
     }
 }
 
@@ -549,7 +542,7 @@ __device__ __forceinline__ void load_q_tile(real *sq, const real *__restrict__ g
 }
 
 // Under a saturated write stream a DRAM read waits far longer than one tile's worth of work
-// (ncu: the warps' top stall was the cp.async wait, profiles/r01_fkj_v4.md), so the q block of a
+// (ncu: the warps' top stall was the cp.async wait), so the q block of a
 // tile further ahead is pulled into L2 with fire-and-forget prefetches; the cp.async that later
 // stages it into shared memory is then an L2 hit.  Costs one instruction, no registers, no smem.
 template <typename real>
@@ -714,7 +707,7 @@ __device__ __forceinline__ void backward_walk_dh(const ChainP<real, N> &P, const
 
 // ------------------------------------------------------------------ forward walk, lean form for the common call
 // k_fkj_forward above is general: any row stride / jindex permutation / alignment, ragged tiles, several tiles per
-// warp, measurement skeletons.  ncu on the pose-only fp32 kernel (profiles/r01_fkine_f32.txt) showed what that
+// warp, measurement skeletons.  ncu on the pose-only fp32 kernel showed what that
 // generality costs on a one-shot grid, where every warp pays the prologue for a single tile: ~300 of 714 issued
 // instructions per tile were integer / control (IMAD, ISETP, LOP3, BRA, BSSY ...), and the kernel was issue-bound.
 // This kernel is the same walk with everything about the call fixed at compile time: DH-like chain (PROF 1),
@@ -724,9 +717,27 @@ template <typename real, int N>
 struct FkjFast {
     static constexpr int QBYTES = 32 * N * (int)sizeof(real);          // multiple of 128
     static constexpr int QUNITS = QBYTES / 16;
-    static constexpr int WB_POSE = QBYTES;                                  // per-warp shared memory, pose only
-    static constexpr int WB_JAC = QBYTES + TileStage<real, 6 * N>::BYTES;   // with the Jacobian stage
+    // per-warp shared memory: the q tile, then ONE output stage that the pose tile and the Jacobian tile take in turn
+    static constexpr int PBYTES = TileStage<real, 16>::BYTES, JBYTES = TileStage<real, 6 * N>::BYTES;
+    __host__ __device__ static constexpr int wb(bool wt, bool wj) { return QBYTES + ((wj && JBYTES > PBYTES) ? JBYTES : (wt ? PBYTES : JBYTES)); }
 };
+
+// The pose tile of a lean kernel: each lane puts its row into the stage (odd row stride: conflict-free 16-byte
+// stores), then the warp copies the tile out with coalesced 16-byte stores, 512 contiguous bytes per instruction.
+// sm_90 has no 256-bit store, and per-lane 128-bit stores of the 128 B rows cover half a sector per lane per
+// instruction: 0.144 -> 0.067 ms for the 1M-row Panda fp64 pose on H100.  The padded stage would leave through the TMA
+// engine only as one 128 B bulk copy per row, which measured slightly slower than this drain.
+template <typename real>
+__device__ __forceinline__ void stage_pose_tile(const Pose<real> &T, unsigned char *stage, real *gout, int lane)
+{
+    typedef TileStage<real, 16> PS;
+    real row[16];
+    pose_to_row(T, row);
+    PS::put_row(stage, lane, row);
+    __syncwarp();
+    PS::drain(stage, gout, 32, lane);
+    __syncwarp(); // the stage is free for the Jacobian tile
+}
 
 template <typename real, int N, bool WT, bool WJ>
 __global__ void __launch_bounds__(B2K_THREADS, FkjBounds<real, N, WJ>::MINB)
@@ -735,7 +746,7 @@ k_fkj_fast(const __grid_constant__ ChainP<real, N> P, const real *__restrict__ q
 {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     typedef FkjFast<real, N> F;
-    constexpr int WB = WJ ? F::WB_JAC : F::WB_POSE;
+    constexpr int WB = F::wb(WT, WJ);
     const int lane = threadIdx.x & 31;
     const int warp = threadIdx.x >> 5;
     const int tile = blockIdx.x * B2K_WARPS_PER_BLOCK + warp;
@@ -759,15 +770,14 @@ k_fkj_fast(const __grid_constant__ ChainP<real, N> P, const real *__restrict__ q
     Pose<real> T;
     real zj[WJ ? N : 1][3], pj[WJ ? N : 1][3];
     chain_forward<real, N, WJ, 1>(P, [&](int j, int) { return qrow[j]; }, T, zj, pj);
-    const size_t row = (size_t)tile * 32 + lane;
+    unsigned char *so = wbase + F::QBYTES;
     if (WT) {
         Pose<real> Tb = T;
         if (P.has_base) pose_mul_const_left(Tb, P.B, AK_GEN | AK_TX | AK_TY | AK_TZ);
-        store_pose_row<real>(Tb, Tout + row * 16);
+        stage_pose_tile<real>(Tb, so, Tout + (size_t)tile * (32 * 16), lane);
     }
     if (WJ) {
         typedef TileStage<real, 6 * N> JS;
-        unsigned char *so = wbase + F::QBYTES;
         real jrow[6 * N];
         jacob0_row<real, N, 1>(P, T, zj, pj, jrow);
         JS::put_row(so, lane, jrow);
@@ -793,7 +803,7 @@ k_fkj_back_fast(const __grid_constant__ ChainP<real, N> P, const real *__restric
     const int warp = threadIdx.x >> 5;
     const int tile = blockIdx.x * B2K_WARPS_PER_BLOCK + warp;
     if (tile >= ntiles) return;
-    unsigned char *wbase = smem_raw + warp * F::WB_JAC;
+    unsigned char *wbase = smem_raw + warp * F::wb(WT, true);
     real *sq = reinterpret_cast<real *>(wbase);
     {
         const uint4 *g = reinterpret_cast<const uint4 *>(q + (size_t)tile * (32 * N));
@@ -813,13 +823,13 @@ k_fkj_back_fast(const __grid_constant__ ChainP<real, N> P, const real *__restric
     real jrow[6 * N];
     pose_from_const(U, P.A[N]);
     backward_walk_dh<real, N>(P, eta, U, jrow);
+    unsigned char *so = wbase + F::QBYTES;
     if (WT) {
         Pose<real> Tb = U;
         if (P.has_base) pose_mul_const_left(Tb, P.B, AK_GEN | AK_TX | AK_TY | AK_TZ);
-        store_pose_row<real>(Tb, Tout + ((size_t)tile * 32 + lane) * 16);
+        stage_pose_tile<real>(Tb, so, Tout + (size_t)tile * (32 * 16), lane);
     }
     typedef TileStage<real, 6 * N> JS;
-    unsigned char *so = wbase + F::QBYTES;
     JS::put_row(so, lane, jrow);
     real *gout = Jout + (size_t)tile * (32 * 6 * N);
     if (!JS::drain_async(so, gout, 32, lane)) {
@@ -961,8 +971,8 @@ int fkj_launch_n(const b2k_chain_s *c, int mode, const real *q, long long nrows,
         if (per_sm < 1) return per_sm < 0 ? per_sm : (b2k_set_error("fkj kernel does not fit on an SM (smem %zu B)", smem), B2K_ERR_INVALID);
         // One-shot grid, a few consecutive tiles per warp: the hardware block scheduler hands out
         // row ranges in address order as SMs free up, which keeps the set of DRAM pages being
-        // written compact.  A persistent grid (variant 4) measured 15-20 % lower write bandwidth
-        // on B200 (scripts/exp/exp_mem3.cu: 5.96 vs 6.73 TB/s for this exact store pattern).
+        // written compact.  A persistent grid (variant 4) measured lower write bandwidth for this
+        // store pattern.
         long long tpw = b2k_tiles_per_warp(wj0 || wje);
         if (variant == 4) { // persistent: as many blocks as fit, each warp a contiguous share of the tiles
             long long g = (long long)b2k_num_sms() * per_sm;
@@ -995,11 +1005,11 @@ int fkj_launch_n(const b2k_chain_s *c, int mode, const real *q, long long nrows,
         };
         typedef FkjFast<real, N> F;
         int rc;
-        if (wje) rc = wt ? launch_fast(k_fkj_back_fast<real, N, true>, (size_t)F::WB_JAC * B2K_WARPS_PER_BLOCK)
-                         : launch_fast(k_fkj_back_fast<real, N, false>, (size_t)F::WB_JAC * B2K_WARPS_PER_BLOCK);
-        else if (wt && wj0) rc = launch_fast(k_fkj_fast<real, N, true, true>, (size_t)F::WB_JAC * B2K_WARPS_PER_BLOCK);
-        else if (wt) rc = launch_fast(k_fkj_fast<real, N, true, false>, (size_t)F::WB_POSE * B2K_WARPS_PER_BLOCK);
-        else rc = launch_fast(k_fkj_fast<real, N, false, true>, (size_t)F::WB_JAC * B2K_WARPS_PER_BLOCK);
+        if (wje) rc = wt ? launch_fast(k_fkj_back_fast<real, N, true>, (size_t)F::wb(true, true) * B2K_WARPS_PER_BLOCK)
+                         : launch_fast(k_fkj_back_fast<real, N, false>, (size_t)F::wb(false, true) * B2K_WARPS_PER_BLOCK);
+        else if (wt && wj0) rc = launch_fast(k_fkj_fast<real, N, true, true>, (size_t)F::wb(true, true) * B2K_WARPS_PER_BLOCK);
+        else if (wt) rc = launch_fast(k_fkj_fast<real, N, true, false>, (size_t)F::wb(true, false) * B2K_WARPS_PER_BLOCK);
+        else rc = launch_fast(k_fkj_fast<real, N, false, true>, (size_t)F::wb(false, true) * B2K_WARPS_PER_BLOCK);
         const long long done = (long long)nfull * 32;
         if (rc != B2K_OK || done == nrows) return rc;
         // ragged tail: the last nrows % 32 rows, general kernel on the slices that start at row `done`

@@ -6,7 +6,7 @@
 // step is a handful of __shfl_sync + FMA on those 12 lanes, the n sincos are evaluated by n lanes
 // in parallel, the Jacobian columns are formed by 3n lanes, outputs are written coalesced by the
 // warp.  20 of 32 lanes idle through the serial part, and every instruction serves ONE row
-// instead of 32: measured 6-8x slower than the default kernel (profiles/r01_variants.md).
+// instead of 32: measured several times slower than the default kernel.
 // Supported for "DH-like" chains only (unflipped Rz joints, any constants): it is a measurement
 // aid selected with b2k_set_variant(1), not a product path.
 #include "b2k_fkj.cuh"

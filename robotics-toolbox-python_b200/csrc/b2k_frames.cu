@@ -5,10 +5,10 @@
 // A frame is "the pose right after joint `after` of the chain, times a constant tail" (the constant transforms of the
 // link that follow its joint), or an absolute constant (`after` = -1: the base frame, links ahead of the first joint).
 // One lane walks one configuration, T = base A_0 J_0(q) A_1 J_1(q) ..., entirely in registers; whenever the walk has
-// passed the joint a frame hangs on, the lane forms T * tail and stores the 16 reals of the frame with full-sector
-// vector stores (256 bit) into row-major (N, slots, 4, 4) memory -- a row's frames are contiguous, a warp writes
+// passed the joint a frame hangs on, the lane forms T * tail and stores the 16 reals of the frame with 128-bit
+// vector stores into row-major (N, slots, 4, 4) memory -- a row's frames are contiguous, a warp writes
 // 32 x slots x 128 B (fp64) of consecutive memory.  The earlier form was one pose launch per frame over prefix chains
-// (q re-read and the prefix re-walked per frame, frame-major output): 0.33 ms for the 8 frames of 1M Panda rows.
+// (q re-read and the prefix re-walked per frame, frame-major output).
 // HBM-bound: 16 reals per frame per row out, n reals per row in.
 #include "b2k_fkj.cuh"
 
@@ -102,7 +102,7 @@ extern "C" int b2k_fkine_frames(b2k_chain_t c, int dtype, const void *q, int64_t
     if (base && (base[12] != 0.0 || base[13] != 0.0 || base[14] != 0.0 || base[15] != 1.0)) { b2k_set_error("%s: base is not an SE(3)/affine matrix", fn); return B2K_ERR_INVALID; }
     const unsigned es = dtype == B2K_F64 ? 8u : 4u;
     if ((uintptr_t)q & (es - 1)) { b2k_set_error("%s: q must be %u-byte aligned", fn, es); return B2K_ERR_INVALID; }
-    if ((uintptr_t)out & 31) { b2k_set_error("%s: out must be 32-byte aligned (256-bit stores)", fn); return B2K_ERR_INVALID; }
+    if ((uintptr_t)out & 31) { b2k_set_error("%s: out must be 32-byte aligned", fn); return B2K_ERR_INVALID; }
     if (N == 0) return B2K_OK;
     B2K_ON_DEVICE_OF(q);
     cudaStream_t st = (cudaStream_t)stream;

@@ -1,4 +1,4 @@
-// b2k_ik.cuh -- batched Levenberg-Marquardt inverse kinematics, one fused persistent kernel (sm_100a).
+// b2k_ik.cuh -- batched Levenberg-Marquardt inverse kinematics, one fused persistent kernel (sm_90a).
 //
 // Replaces fknm.IK_LM_c (reference fknm.cpp:394-525 -> _IK_LM_Chan/_Wampler/_Sugihara
 // ik.cpp:157-209 -> _IK_loop ik.cpp:19-75) and, with semantics = B2K_IK_SEM_PYTHON, the Python
@@ -352,7 +352,7 @@ __device__ __forceinline__ bool ik_wrap_and_check(const IkP<real, N> &K, real *q
 // two_phase != 0 a lane does only the FIRST search of a problem; a problem whose first search
 // fails is appended to the hard list (with its iteration contribution) for k_ik_restarts.
 // Resident blocks per SM asked of ptxas: with the normal equations and the Jacobian in registers the fp32 kernels
-// fit 128 registers (4 blocks) without spilling; the fp64 ones would take ~250 (2 blocks) and run 1-4 % faster held to 168 (3 blocks, ~150 B of spills; profiles/r02_ik_seg_sweep.jsonl).  -DB2K_IK_MINB=n overrides both
+// fit 128 registers (4 blocks) without spilling; the fp64 ones would take ~250 (2 blocks) and run 1-4 % faster held to 168 (3 blocks, ~150 B of spills).  -DB2K_IK_MINB=n overrides both
 // (DESIGN 3.5 has the sweep: 4 / 5 / 6 blocks measure the same, 8 spills and is 10 % slower).
 #ifdef B2K_IK_MINB
 template <typename real> constexpr int ik_min_blocks() { return B2K_IK_MINB; }

@@ -1,4 +1,4 @@
-// b2k_rne.cuh -- batched recursive Newton-Euler inverse dynamics for DH / MDH arms (sm_100a).
+// b2k_rne.cuh -- batched recursive Newton-Euler inverse dynamics for DH / MDH arms (sm_90a).
 //
 // Replaces the per-row frne.frne loop of DHRobot.rne (reference DHRobot.py:1442-1451 ->
 // frne.c:106-230 -> newton_euler ne.c:62-492, rot_mat frne.c:310-351).

@@ -2,14 +2,14 @@
 //
 // The generic kernels (b2k_rne.cuh) multiply through every link parameter of the 24-double table
 // whether it is zero or not: for a Puma560 that is 886 FP64 instructions per row, and the kernel is
-// FP64-pipe bound (profiles/r01_rne_v3.txt).  Most of a real arm's table is structure, not numbers:
+// FP64-pipe bound.  Most of a real arm's table is structure, not numbers:
 // alpha in {0, +-pi/2}, a or d zero, centre of mass on an axis, diagonal inertia, no tip wrench, gravity
 // along one base axis, and the first links of the chain carry sparse velocities (w_0 = 0).  This file
 // is the chain compiler for dynamics: it runs the Luh-Walker-Paul recursion (reference ne.c:137-457)
 // SYMBOLICALLY over scalars that are either exactly zero, a known constant or a run-time value, and
 // emits straight-line CUDA C in which a term whose factor is zero never appears, a factor of +-1 is
 // a sign, constants are folded, and every sum of products is a chain of FMAs.  The text is compiled
-// for sm_100a at run time (NVRTC, b2k_rne_spec.cu) into a kernel for THIS robot; the same text
+// for sm_90a at run time (NVRTC, b2k_rne_spec.cu) into a kernel for THIS robot; the same text
 // compiles as plain C++ for the host, which is how tests/ check it against the oracle without a GPU.
 //
 // The dynamics fan-outs of the reference's DynamicsMixin (Dynamics.py: inertia, gravload, itorque,

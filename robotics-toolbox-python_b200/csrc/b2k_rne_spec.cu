@@ -3,7 +3,7 @@
 // b2k_rne_gen.cpp turns one robot's 24-double link table into straight-line CUDA C for the recursion
 // (and for the dynamics fan-outs built on it).  Here that text is wrapped in the tile I/O of the RNE
 // kernels (a warp owns 32 rows: cp.async tiles in, one row per lane, results staged and written by one
-// TMA bulk copy), compiled for sm_100a with NVRTC the first time a (robot, operation, dtype, gravity
+// TMA bulk copy), compiled for sm_90a with NVRTC the first time a (robot, operation, dtype, gravity
 // pattern) is used, loaded through the driver API and launched on the caller's stream.  Both libraries
 // are found with dlopen at run time (libnvrtc.so.12 of the CUDA toolkit, libcuda.so.1 of the driver):
 // libb2kin.so itself links neither.  When either is missing the
@@ -153,7 +153,7 @@ __device__ __forceinline__ void load_tile(real *s, const real *g, int lane)
 // A warp owns TPW consecutive tiles of 32 rows (one-shot grid of full tiles; the ragged tail of a batch goes to the
 // generic kernel).  The input tiles are double-buffered: the cp.async loads of tile t+1 are issued before tile t is
 // computed, so a warp always has a tile's worth of reads in flight -- with one tile per warp and 16-20 resident warps
-// per SM the kernel was latency-bound (ncu: long-scoreboard the top stall, FP64 pipe 62 % busy; profiles/r02_rne64s_v1.txt).
+// per SM the kernel was latency-bound (ncu: long-scoreboard the top stall, FP64 pipe 62 % busy).
 extern "C" __global__ void __launch_bounds__(128, MINB)
 k_rne_spec(const __grid_constant__ SpecP P, const real *__restrict__ in0, const real *__restrict__ in1,
            const real *__restrict__ in2, real *__restrict__ out, long long ntiles)
@@ -524,7 +524,7 @@ Driver *driver()
 struct Program {
     bool ok = false;
     std::string why;          // why not, when !ok
-    std::string cubin;        // sm_100a image
+    std::string cubin;        // sm_90a image
     std::vector<double> consts;
     int nin = 1, nout = 0, nres = 0, nc = 1, tpw = 1;
     const char *entry = "k_rne_spec";
@@ -576,12 +576,11 @@ std::string build_source(const GenFn &gen, int n, int mode, int dtype, Program &
     // tiles per warp (double-buffered inputs when > 1).  fp64: no gain -- the kernel is bound by instruction issue (2-cycle
     // FP64 issue + integer / control), and the second buffer costs registers.  fp32: the whole recursion is ~480 issued
     // instructions per row, short enough for the tile-load latency to show (ncu: long-scoreboard the top stall), and two
-    // tiles per warp with 8 resident blocks measured 24.9 -> 22.2 us on the Puma (profiles/r02_rne_sweep32.jsonl).
-    // Tried and dropped (commit b8738be, profiles/r02_rne_pair_sweep.jsonl, r02_rne_persist_sweep.jsonl): two fp32 rows per
+    // tiles per warp with 8 resident blocks measured faster on the Puma.
+    // Tried and dropped (commit b8738be): two fp32 rows per
     // lane as f32x2 pairs (FFMA2 / FMUL2: 35 % fewer issued instructions, same time -- an FFMA2 still holds the FP32
     // pipe for two cycles and the kernel is not bound by issue at this size) and a persistent grid-stride loop with
-    // double-buffered tiles (fp32 equal, fp64 slower: the second buffer's registers spill).  At 1M rows the one-shot
-    // kernel pays 4-6 us of fill / drain per launch; at 4M rows it streams at 0.82 (fp64) / 0.91 (fp32) of HBM.
+    // double-buffered tiles (fp32 equal, fp64 slower: the second buffer's registers spill).
     const bool light = mode == B2K_GEN_RNE || mode == B2K_GEN_GRAVLOAD || mode == B2K_GEN_ITORQUE;
     int tpw = (dtype == B2K_F32 && light) ? 2 : 1;
     if (const char *e = getenv("B2K_RNE_SPEC_TPW")) tpw = atoi(e) > 0 ? atoi(e) : tpw;
@@ -589,7 +588,7 @@ std::string build_source(const GenFn &gen, int n, int mode, int dtype, Program &
     p.smem = 4 * ((tpw > 1 ? 2 : 1) * p.nin * in_bytes + (size_t)32 * p.nout * es);
     if (p.smem > 220 * 1024) { p.why = "a tile of this operation does not fit the shared memory of an SM (" + std::to_string(p.smem) + " B)"; return std::string(); }
     int minb = (int)((200 * 1024) / (p.smem + 1024));
-    // resident blocks to aim for (profiles/r02_rne_sweep.jsonl, r02_rne_sweep32.jsonl: fp64 96 registers / 5 blocks, fp32 64 registers / 8 blocks)
+    // resident blocks to aim for (swept: fp64 96 registers / 5 blocks, fp32 64 registers / 8 blocks)
     const int want = light ? (es == 8 ? 5 : 8) : (es == 8 ? 2 : 3);
     if (minb > want) minb = want;
     if (minb < 1) minb = 1;
@@ -612,7 +611,7 @@ void compile(const GenFn &gen, int n, const Key &key, Program &p)
     if (fdyn) p.entry = "k_fdyn";
     const std::string src = build_source(gen, n, mode, dtype, p, defs, fdyn ? kFdyn : nullptr);
     if (src.empty()) return;
-    std::vector<std::string> opts = {"--gpu-architecture=sm_100a", "--std=c++17"};
+    std::vector<std::string> opts = {"--gpu-architecture=sm_90a", "--std=c++17"};
     if (getenv("B2K_RNE_SPEC_LINEINFO")) opts.push_back("-lineinfo");
     for (auto &d : defs) opts.push_back(d);
     std::vector<const char *> copts;

@@ -1,7 +1,7 @@
 // b2k_trig.cuh -- sincos for the chain walk.
 //
 // CUDA's sincos() is accurate but costs ~100 issued instructions per call in this kernel
-// (ncu, profiles/r01_fkj_first.md): its 14 polynomial coefficients are materialised as pairs of
+// (ncu): its 14 polynomial coefficients are materialised as pairs of
 // 32-bit immediates and the quadrant fix-up is a chain of 22 FSEL.  This version does the same
 // mathematics -- three-FMA Cody-Waite reduction by pi/2 (exact products thanks to FMA, valid for
 // |x| < 105615 like CUDA's own fast path), fdlibm's degree-13/14 minimax kernels on

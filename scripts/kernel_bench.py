@@ -2,7 +2,7 @@
 """Device-timed micro-benchmarks of every hot-path kernel (one JSON line per case).
 
 Each case: W warm-up launches, then K launches bracketed by CUDA events on the launching stream;
-inputs rotate over enough distinct batches to exceed the 126 MB L2.  `frac` is algorithmic bytes
+inputs rotate over enough distinct batches to exceed the 50 MB L2.  `frac` is algorithmic bytes
 (SURVEY 8d) / time / MEASURED_PEAKS hbm_gbs.  Usage:  python scripts/kernel_bench.py [--rows 1000000] [--only substr]
 """
 import argparse
@@ -28,7 +28,7 @@ args = ap.parse_args()
 try:
     PEAK = float(json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"])
 except Exception:
-    PEAK = 6650.0
+    PEAK = 3350.0  # H100 SXM data sheet
 dev = torch.device("cuda", 0)
 torch.cuda.set_device(0)
 if args.variant:

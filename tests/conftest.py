@@ -1,7 +1,7 @@
 """pytest configuration: registers the `gpu` marker and puts the repo root on sys.path.
 
 `-m "not gpu"` runs everywhere (oracle vs golden vectors, host logic, C-ABI symbols);
-`-m gpu` needs a B200 and calls the CUDA kernels through the C-ABI.
+`-m gpu` needs an H100 and calls the CUDA kernels through the C-ABI.
 """
 import os
 import sys
@@ -16,7 +16,7 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
 
 
 @pytest.fixture(scope="session")

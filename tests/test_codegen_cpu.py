@@ -2,7 +2,7 @@
 emits is plain C in terms of `real`, so the same text the library hands to NVRTC is compiled here for the host
 (g++) and compared with the oracle -- the C restatement of the reference's ne.c -- on seeded inputs, for every
 operation the generator serves (rne + the five dynamics fan-outs), standard and modified DH, the benchmark robots
-and random arms with random sparsity.  Also: the generated text compiles for sm_100a through the library's own
+and random arms with random sparsity.  Also: the generated text compiles for sm_90a through the library's own
 NVRTC path (no device needed for that), and what it leaves out (zero terms) is reported."""
 import ctypes as C
 import os
@@ -168,7 +168,7 @@ def test_specialisation_drops_the_structural_zeros_of_the_puma():
 
 @pytest.mark.skipif(not any(os.path.exists(p) for p in ("/usr/local/cuda/lib64/libnvrtc.so.12", "/usr/local/cuda/lib64/libnvrtc.so")),
                     reason="NVRTC not installed")
-def test_generated_kernels_compile_for_sm_100a_through_the_library():
+def test_generated_kernels_compile_for_sm_90a_through_the_library():
     """The library's own NVRTC path (needs no device): every operation x dtype builds for Puma560 and Panda MDH."""
     lib = rtb._lib.lib()
     g = np.array([0.0, 0.0, 9.81])
