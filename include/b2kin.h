@@ -270,6 +270,32 @@ int b2k_tree_fdyn(b2k_tree_t tree, int dtype, const void *q0, const void *qd0, i
                  double rtol, double atol, double max_step, double first_step, double dt, int grid, int M, void *out_t,
                  void *out_q, void *out_qd, int32_t *out_count, int32_t *out_status, void *stream);
 
+/* ---------------------------------------------------------------- operational-space dynamics
+ * The arithmetic of DynamicsMixin.inertia_x, coriolis_x, gravload_x and accel_x (robot/Dynamics.py, between gravload and
+ * itorque: per row np.linalg.inv / pinv of the analytical Jacobian and numpy triple products, in a Python loop), as an
+ * epilogue over what the joint-space entry points produced.  All arrays are (N, ...) device arrays of dtype, row-major:
+ *   Ja (N,6,n) analytical Jacobian (b2k_jacob0_analytical)   Ji_in (N,n,6) a given inverse (then Ja is not inverted)
+ *   M, C (N,n,n) inertia / Coriolis matrix    Jd (N,6,n) time derivative of Ja    G (N,n) gravity load
+ *   Mx_in (N,6,6) a given Mx (Cx then needs no M)    xd (N,6) task-space velocity    w (N,6) wrench
+ * inverse B2K_OPS_INV: Ji = inv(Ja), n must be 6, partial pivoting as LAPACK getrf; a row with an exactly zero pivot gets
+ * NaN in every output that depends on Ji (numpy raises LinAlgError for it).  B2K_OPS_PINV: Ji = pinv(Ja) by one-sided
+ * Jacobi SVD, singular values <= 1e-15 s_max dropped as numpy.linalg.pinv does.  One launch writes any non-NULL output:
+ *   Ji  (N,n,6)                                                         needs Ja or Ji_in
+ *   Mx  (N,6,6) = Ji^T M Ji                      (inertia_x)            needs M
+ *   Cx  (N,6,6) = Ji^T C Ji - Mx Jd Ji           (coriolis_x)           needs C, Jd and M or Mx_in
+ *   Gx  (N,6)   = Ji^T G                         (gravload_x)           needs G
+ *   qd  (N,n)   = Ji xd                          (accel_x, first stage) needs xd
+ *   tau (N,n)   = Ja^T w                         (accel_x, first stage) needs Ja and w
+ * b2k_opspace_xdd is the last stage of accel_x: xdd (N,6) = Ja qdd + Jd qd, with qdd from b2k_rne_accel / b2k_tree_dyn
+ * and Jd taken at qd.  Arguments are validated before any CUDA call. */
+#define B2K_OPS_INV 0
+#define B2K_OPS_PINV 1
+int b2k_opspace(int dtype, int n, int inverse, const void *Ja, const void *Ji_in, const void *M, const void *C, const void *Jd,
+                const void *G, const void *Mx_in, const void *xd, const void *w, int64_t N, void *Ji, void *Mx, void *Cx, void *Gx,
+                void *qd, void *tau, void *stream);
+int b2k_opspace_xdd(int dtype, int n, const void *Ja, const void *qdd, const void *Jd, const void *qd, int64_t N, void *xdd,
+                    void *stream);
+
 /* ---------------------------------------------------------------- pure functions of the Jacobian
  * b2k_hessian replaces fknm.ETS_hessian0 / ETS_hessiane (fknm.cpp:583-783 -> _ETS_hessian
  * methods.cpp:16-32): H (N,n,6,n) from J (N,6,n); pass jacob0 for hessian0, jacobe for hessiane.

@@ -15,6 +15,7 @@ import numpy as np
 
 from . import _buffers as B
 from . import _lib
+from . import _opspace
 from ._se3 import SE3
 from .DHLink import DHLink
 from .ET import ET
@@ -416,3 +417,20 @@ class DHRobot:
         """Forward dynamics qdd = M(q)^-1 (torque - rne(q, qd, 0)), joint friction included
         (reference Dynamics.accel, Dynamics.py:424-510)."""
         return self._dyn("b2k_rne_accel", [q, qd, torque], (self.n,), gravity=gravity, use_gravity=True, dtype=dtype)
+
+    # ---- operational-space dynamics (reference DynamicsMixin, Dynamics.py between gravload and itorque): _opspace.py
+    def inertia_x(self, q, pinv=False, representation="rpy/xyz", Ji=None, dtype=None):
+        """Operational-space inertia Mx = Ji^T M Ji, (6,6) or (N,6,6); Ji = inv / pinv of jacob0_analytical."""
+        return _opspace.inertia_x(self, q, pinv=pinv, representation=representation, Ji=Ji, dtype=dtype)
+
+    def coriolis_x(self, q, qd, pinv=False, representation="rpy/xyz", J=None, Ji=None, Jd=None, C=None, Mx=None, dtype=None):
+        """Operational-space Coriolis matrix Cx = Ji^T C Ji - Mx Jad Ji, (6,6) or (N,6,6)."""
+        return _opspace.coriolis_x(self, q, qd, pinv=pinv, representation=representation, J=J, Ji=Ji, Jd=Jd, C=C, Mx=Mx, dtype=dtype)
+
+    def gravload_x(self, q, gravity=None, pinv=False, representation="rpy/xyz", Ji=None, dtype=None):
+        """Operational-space gravity load Gx = Ji^T G, (6,) or (N,6)."""
+        return _opspace.gravload_x(self, q, gravity=gravity, pinv=pinv, representation=representation, Ji=Ji, dtype=dtype)
+
+    def accel_x(self, q, xd, wrench, gravity=None, pinv=False, representation="rpy/xyz", dtype=None):
+        """Operational-space forward dynamics: task acceleration (6,) or (N,6) under the end-effector wrench."""
+        return _opspace.accel_x(self, q, xd, wrench, gravity=gravity, pinv=pinv, representation=representation, dtype=dtype)

@@ -12,6 +12,7 @@ import numpy as np
 
 from . import _buffers as B
 from . import _lib
+from . import _opspace
 from ._se3 import SE3
 from .DHLink import _inertia
 from .ET import ET
@@ -533,6 +534,35 @@ class Robot:
         """Forward dynamics qdd = M(q)^-1 (torque - rne(q, qd, 0)) (Dynamics.py:424-503: n + 1 rne calls and a numpy
         solve per row there)."""
         return self._tree_dyn("accel", (q, qd, torque), ("q", "qd", "torque"), (self.n,), gravity=gravity, dtype=dtype)
+
+    # ---- operational-space dynamics (reference DynamicsMixin, Dynamics.py between gravload and itorque): _opspace.py
+    def _opspace_robot(self):
+        """The tree kernels list torque columns in joint-group order, the Jacobian lists joints in chain order: the two
+        only meet when both are q order and the chain to the end-effector moves every joint."""
+        if list(self.tree_description()["jindex"]) != list(range(self.n)):
+            raise ValueError("operational-space dynamics needs the joint groups in q order (jindex 0..n-1)")
+        if list(self.ets().jindices) != list(range(self.n)):
+            raise ValueError("operational-space dynamics needs the Jacobian to the end-effector to cover all n joints in q order")
+        return self
+
+    def inertia_x(self, q, pinv=False, representation="rpy/xyz", Ji=None, dtype=None):
+        """Operational-space inertia Mx = Ji^T M Ji, (6,6) or (N,6,6); Ji = inv / pinv of jacob0_analytical."""
+        return _opspace.inertia_x(self._opspace_robot(), q, pinv=pinv, representation=representation, Ji=Ji, dtype=dtype)
+
+    def coriolis_x(self, q, qd, pinv=False, representation="rpy/xyz", J=None, Ji=None, Jd=None, C=None, Mx=None, dtype=None):
+        """Operational-space Coriolis matrix Cx = Ji^T C Ji - Mx Jad Ji, (6,6) or (N,6,6)."""
+        return _opspace.coriolis_x(self._opspace_robot(), q, qd, pinv=pinv, representation=representation, J=J, Ji=Ji, Jd=Jd, C=C,
+                                   Mx=Mx, dtype=dtype)
+
+    def gravload_x(self, q, gravity=None, pinv=False, representation="rpy/xyz", Ji=None, dtype=None):
+        """Operational-space gravity load Gx = Ji^T G, (6,) or (N,6)."""
+        return _opspace.gravload_x(self._opspace_robot(), q, gravity=gravity, pinv=pinv, representation=representation, Ji=Ji,
+                                   dtype=dtype)
+
+    def accel_x(self, q, xd, wrench, gravity=None, pinv=False, representation="rpy/xyz", dtype=None):
+        """Operational-space forward dynamics: task acceleration (6,) or (N,6) under the end-effector wrench."""
+        return _opspace.accel_x(self._opspace_robot(), q, xd, wrench, gravity=gravity, pinv=pinv, representation=representation,
+                                dtype=dtype)
 
     def fdyn(self, T, q0, Q=None, Q_args=None, qd0=None, solver="RK45", solver_args=None, dt=None, progress=False, gravity=None,
              max_steps: int = 4096, dtype=None):

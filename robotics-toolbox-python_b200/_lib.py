@@ -21,6 +21,7 @@ MAX_QWIDTH = 16
 LM_METHODS = {"chan": 0, "wampler": 1, "sugihara": 2}
 SEM_CPP, SEM_PYTHON = 0, 1
 IK_NR, IK_GN = 3, 4  # method codes of b2k_ik_lm beyond the three LM damping rules
+OPS_INV, OPS_PINV = 0, 1  # inverse kinds of b2k_opspace
 
 _lib = None
 
@@ -71,6 +72,8 @@ _PROTOS = {
     "b2k_angle_axis": (C.c_int, [C.c_int, vp, vp, i64, i64, vp, vp]),
     "b2k_p_servo": (C.c_int, [C.c_int, vp, vp, i64, i64, dp, C.c_double, vp, vp, vp]),
     "b2k_jacob0_analytical": (C.c_int, [C.c_int, C.c_int, vp, vp, i64, C.c_int, vp, vp]),
+    "b2k_opspace": (C.c_int, [C.c_int, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp, vp, vp, vp, i64, vp, vp, vp, vp, vp, vp, vp]),
+    "b2k_opspace_xdd": (C.c_int, [C.c_int, C.c_int, vp, vp, vp, vp, i64, vp, vp]),
     "b2k_p_servo_rpy": (C.c_int, [C.c_int, vp, vp, i64, i64, dp, C.c_double, vp, vp, vp]),
     "b2k_ctraj": (C.c_int, [C.c_int, dp, dp, vp, i64, vp, vp]),
     "b2k_mstraj": (C.c_int, [C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int64), C.POINTER(C.c_int64), ip, dp, dp, dp, dp, i64, vp, vp]),

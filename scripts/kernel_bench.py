@@ -260,6 +260,40 @@ if want("extra_"):
             print(json.dumps({"case": name, "error": f"{type(e).__name__}: {e}"[:300]}), flush=True)
     del Qx, QDx, Jx, Tx, Ty
 
+# Operational-space dynamics (b2k_opspace): the epilogue alone over staged joint-space inputs -- inverse (Puma560) and
+# Jacobi pseudo-inverse (PandaMDH, n = 7) -- and the whole coriolis_x pipeline through the public call.  Bytes per row =
+# the arrays the epilogue must read and write.
+if want("opspace_"):
+    NO = args.rows
+    rngo = np.random.default_rng(6)
+    Lo = rtb._lib.lib()
+    sto = torch.cuda.current_stream().cuda_stream
+    for tag, rob, kind in (("puma_inv", rtb.models.Puma560(), rtb._lib.OPS_INV), ("pandamdh_pinv", rtb.models.PandaMDH(), rtb._lib.OPS_PINV)):
+        n = rob.n
+        qo = torch.from_numpy(rngo.uniform(-2, 2, (NO, n))).to(dev)
+        qdo = torch.from_numpy(rngo.normal(size=(NO, n))).to(dev)
+        Ja, M, Cm, G = rob.jacob0_analytical(qo), rob.inertia(qo), rob.coriolis(qo, qdo), rob.gravload(qo)
+        Jd = rob.jacob0_dot(qo, qdo, representation="rpy/xyz")
+        Mx, Cx = (torch.empty((NO, 6, 6), dtype=torch.float64, device=dev) for _ in range(2))
+        Gx = torch.empty((NO, 6), dtype=torch.float64, device=dev)
+        p = lambda t: None if t is None else t.data_ptr()  # noqa: E731
+        for case, ins, outs in ((f"opspace_mx_{tag}_f64", (Ja, M, None, None, None), (Mx, None, None)),
+                                (f"opspace_mx_cx_gx_{tag}_f64", (Ja, M, Cm, Jd, G), (Mx, Cx, Gx))):
+            if not want(case):
+                continue
+            a = [p(t) for t in ins]
+            o = [p(t) for t in outs]
+            bpr = (sum(t[0].numel() for t in ins if t is not None) + sum(t[0].numel() for t in outs if t is not None)) * 8
+            report(case, timeit(lambda i: rtb._lib.check(Lo.b2k_opspace(rtb._lib.F64, n, kind, a[0], None, a[1], a[2], a[3], a[4], None,
+                                                                        None, None, NO, None, o[0], o[1], o[2], None, None, sto)), 1),
+                   NO, bpr, {"api": "C ABI, inputs staged on the device"})
+        case = f"opspace_coriolis_x_pipeline_{tag}_f64"
+        if want(case):
+            pinv = kind == rtb._lib.OPS_PINV
+            report(case, timeit(lambda i: rob.coriolis_x(qo, qdo, pinv=pinv), 1), NO, (2 * n + 36) * 8,
+                   {"api": "public Python call on device-resident q, qd: jacob0_analytical, jacob0_dot, coriolis, inertia, b2k_opspace"})
+        del qo, qdo, Ja, M, Cm, G, Jd, Mx, Cx, Gx
+
 # IK (config 4): reachable targets, chan
 if want("ik_"):
     panda = rtb.models.Panda().ets()
