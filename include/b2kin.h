@@ -296,6 +296,22 @@ int b2k_opspace(int dtype, int n, int inverse, const void *Ja, const void *Ji_in
 int b2k_opspace_xdd(int dtype, int n, const void *Ja, const void *qdd, const void *Jd, const void *qd, int64_t N, void *xdd,
                     void *stream);
 
+/* ---------------------------------------------------------------- closed-form inverse kinematics
+ * b2k_ikine_6s replaces DHRobot.ikine_6s (robot/DHRobot.py), which Puma560.ikine_a calls: the analytic joint solution of a
+ * wrist-partitioned standard-DH 6R arm with the Puma link pattern, one pose per row, no iteration.
+ *   dh   host (6,4) rows of (d, a, alpha, offset).  The pattern, each condition to 1e-9: alpha = (+pi/2, 0, -pi/2, s pi/2,
+ *        -s pi/2, any) with s = +1 or -1, a1 = a4 = a5 = 0, d5 = 0, a2 != 0.  Anything else is B2K_ERR_INVALID.
+ *   base, tool  host 4x4 row-major, NULL = identity
+ *   T    (N,4,4) device poses of dtype
+ *   conf host array of nconf (1..8) configuration codes: bit 0 set = shoulder right ("r", else "l"), bit 1 set = elbow
+ *        down ("d", else "u"), bit 2 set = wrist flipped ("f", else "n")
+ *   q    (N,nconf,6) joint angles wrapped into [-pi, pi), the solution for conf[k] in slot k; NaN where out of reach
+ *   ok   (N,nconf) int32: 1 = solved, 0 = the pose is out of reach for that configuration
+ * Joint limits are not applied (the reference does not apply them either).  One launch; arguments are validated before
+ * any CUDA call, and N = 0 returns without touching the device. */
+int b2k_ikine_6s(int dtype, const double *dh, const double *base, const double *tool, const void *T, int64_t N, int nconf,
+                 const int32_t *conf, void *q, int32_t *ok, void *stream);
+
 /* ---------------------------------------------------------------- pure functions of the Jacobian
  * b2k_hessian replaces fknm.ETS_hessian0 / ETS_hessiane (fknm.cpp:583-783 -> _ETS_hessian
  * methods.cpp:16-32): H (N,n,6,n) from J (N,6,n); pass jacob0 for hessian0, jacobe for hessiane.

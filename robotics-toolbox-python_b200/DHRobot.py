@@ -4,7 +4,7 @@ through the batched RNE kernel.
 Mirrors the hot-path part of the reference's ``DHRobot`` (reference
 src/roboticstoolbox/robot/DHRobot.py): ``ets()`` 878-918, ``fkine`` 920-979, ``jacobe`` 1066-1140,
 ``jacob0`` 1142-1198, ``rne`` 1373-1456 with its parameter packing ``_init_rne`` 1340-1361 and
-dirty tracking (DHLink.py:24-51), ``ikine_LM`` 2454-2474.
+dirty tracking (DHLink.py:24-51), ``ikine_LM`` 2454-2474, and the closed-form ``ikine_6s`` as ``ikine_a``.
 """
 from __future__ import annotations
 
@@ -20,6 +20,7 @@ from ._se3 import SE3
 from .DHLink import DHLink
 from .ET import ET
 from .ETS import ETS, _mat44
+from .IK import IKSolution
 
 
 class DHRobot:
@@ -180,6 +181,99 @@ class DHRobot:
 
         q1, q2 = self.ikine_LM(T1, **kwargs), self.ikine_LM(T2, **kwargs)
         return _jtraj(q1.q, q2.q, t, device=device)
+
+    # ---- closed-form inverse kinematics (reference DHRobot.ikine_6s, which Puma560.ikine_a calls): csrc/b2k_ik6s.cu
+    _IKINE_A_LETTERS = ("lr", "ud", "nf")
+
+    @staticmethod
+    def config_validate(config: str, allowables) -> str:
+        """The reference's configuration-string rules: one letter of each pair in ``allowables`` (for example
+        ("lr", "ud", "nf")), the first of a pair where the string has neither; both letters of a pair, or a letter of no
+        pair, raise ValueError.  Returns the letters in the order of ``allowables``."""
+        if not isinstance(config, str):
+            raise TypeError("config must be a string")
+        known = "".join(allowables)
+        for ch in config:
+            if ch not in known:
+                raise ValueError(f"bad config specifier {ch!r}: the letters are {', '.join(allowables)}")
+        out = ""
+        for pair in allowables:
+            given = set(pair) & set(config)
+            if len(given) > 1:
+                raise ValueError(f"config {config!r} gives more than one of {pair!r}")
+            out += given.pop() if given else pair[0]
+        return out
+
+    def _ikine_a_table(self) -> np.ndarray:
+        """(6,4) rows of (d, a, alpha, offset) for b2k_ikine_6s, after the checks its table cannot express"""
+        if self.n != 6:
+            raise ValueError(f"ikine_a: the closed form serves 6-joint arms; this robot has {self.n} joints")
+        if self.mdh:
+            raise ValueError("ikine_a: the closed form serves standard DH; this robot uses modified DH")
+        for j, l in enumerate(self.links):
+            if not l.isrevolute:
+                raise ValueError(f"ikine_a: joint {j + 1} is prismatic; the closed form needs revolute joints")
+            if l.flip:
+                raise ValueError(f"ikine_a: joint {j + 1} is flipped; the closed form needs unflipped joints")
+        return np.ascontiguousarray([[l.d, l.a, l.alpha, l.offset] for l in self.links], dtype=np.float64)
+
+    def ikine_a(self, T, config="lun", dtype=None) -> IKSolution:
+        """Analytic inverse kinematics of a Puma-type 6R arm (reference DHRobot.ikine_6s / Puma560.ikine_a): the exact
+        joint solution for a shoulder (l / r), elbow (u / d) and wrist (n / f) configuration, with no iteration.
+
+        The robot must be a standard-DH, all-revolute 6-joint arm with alpha = (pi/2, 0, -pi/2, +-pi/2, -+pi/2, any),
+        a1 = a4 = a5 = 0, d5 = 0 and a2 != 0; any other robot raises ValueError naming what breaks the pattern.
+        ``T`` is an SE3, a (4,4) or (N,4,4) array, or a CUDA tensor; ``config`` a string ("lun" default, missing letters
+        filled by :meth:`config_validate`) or a sequence of up to 8 strings, all solved from one read of T in one launch.
+        One pose gives ``IKSolution(q (6,), success, reason="Success" | "Out of reach")``; a batch q (N,6) with NaN
+        rows where the pose is out of reach, success = every row reachable.  A sequence of configurations makes q
+        (k,6) / (N,k,6).  numpy in gives numpy out, a CUDA tensor gives q on its device.  Joint limits are not applied."""
+        configs = [config] if isinstance(config, str) else list(config)
+        if not 1 <= len(configs) <= 8:
+            raise ValueError(f"ikine_a: give 1 to 8 configurations, got {len(configs)}")
+        codes = []
+        for c in configs:
+            v = self.config_validate(c, self._IKINE_A_LETTERS)
+            codes.append(int(v[0] == "r") | int(v[1] == "d") << 1 | int(v[2] == "f") << 2)
+        conf = np.array(codes, dtype=np.int32)
+        dh = self._ikine_a_table()
+        base = None if np.array_equal(self._base, np.eye(4)) else np.ascontiguousarray(self._base)
+        tool = None if np.array_equal(self._tool, np.eye(4)) else np.ascontiguousarray(self._tool)
+        L = _lib.lib()
+        cp = conf.ctypes.data_as(_lib.ip)
+        # the link pattern is checked by the C entry point; N = 0 validates without touching a device
+        _lib.check(L.b2k_ikine_6s(_lib.F64, _lib.dptr(dh), _lib.dptr(base), _lib.dptr(tool), None, 0, len(conf), cp, None,
+                                  None, None))
+        T = getattr(T, "A", T)
+        B.check_numeric(T, "T")
+        if not B.is_tensor(T):
+            T = np.asarray(T)
+        if T.ndim not in (2, 3) or tuple(T.shape[-2:]) != (4, 4):
+            raise ValueError(f"T must be (4,4) or (N,4,4); got {tuple(T.shape)}")
+        single = T.ndim == 2
+        dt = B.pick_dtype(T, dtype)
+        Td = B.to_device(T, dt).reshape(-1, 4, 4).contiguous()
+        N, k = Td.shape[0], len(conf)
+        q = B.empty((N, k, 6), dt, like=Td)
+        ok = B.empty_i32((N, k), like=Td)
+        _lib.check(L.b2k_ikine_6s(B.code(dt), _lib.dptr(dh), _lib.dptr(base), _lib.dptr(tool), B.ptr(Td), N, k, cp, B.ptr(q),
+                                  B.ptr(ok), B.stream_ptr(Td)))
+        reached = B.to_host(ok).astype(bool)
+        if not B.is_tensor(T):
+            q = B.to_host(q)
+        if isinstance(config, str):
+            q, reached = q[:, 0], reached[:, 0]
+        if single:
+            q, reached = q[0], reached[0]
+        missed = int(reached.size - reached.sum())
+        if single and reached.ndim == 0:
+            reason = "Success" if missed == 0 else "Out of reach"
+        elif missed == 0:
+            reason = "Success"
+        else:
+            what = "rows" if isinstance(config, str) else "solutions"
+            reason = f"Out of reach: {missed} of {reached.size} {what}"
+        return IKSolution(q=q, success=missed == 0, reason=reason)
 
     def ik_NR(self, Tep, **kwargs):
         return self.ets().ik_NR(Tep, **kwargs)

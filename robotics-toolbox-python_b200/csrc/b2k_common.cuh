@@ -4,6 +4,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <type_traits>
+
 #include "../../include/b2kin.h"
 
 #define B2K_WARPS_PER_BLOCK 4
@@ -264,5 +266,28 @@ __device__ __forceinline__ void split_elem(long long e, int n, long long total, 
         row = e / n;
         j = (int)(e - row * n);
     }
+}
+
+template <typename real> __device__ __forceinline__ real r_atan2(real y, real x);
+template <> __device__ __forceinline__ double r_atan2<double>(double y, double x) { return atan2(y, x); }
+template <> __device__ __forceinline__ float r_atan2<float>(float y, float x) { return atan2f(y, x); }
+template <typename real> __device__ __forceinline__ real r_eps() { return sizeof(real) == 8 ? (real)2.220446049250313e-16 : (real)1.1920929e-07f; }
+
+// spatialmath's tr2eul: R = Rz(phi) Ry(theta) Rz(psi) -> (phi, theta, psi), theta >= 0; FLIP takes the other solution
+// (phi + pi, theta < 0).  With |R02| and |R12| below 10 eps phi is 0.  Used by jacob0_analytical("eul") and ikine_a.
+// SinCos, when given, is a stateless functor SinCos()(x, s, c) that forms sin and cos of phi (a caller whose angles are
+// small can avoid libm's Payne-Hanek branch); by default libm's sin and cos.
+template <typename real, bool FLIP = false, typename SinCos = void>
+__device__ __forceinline__ void rot_to_eul(const real R[3][3], real g[3])
+{
+    real sp = 0, cp = 1;
+    if (fabs(R[0][2]) < 10 * r_eps<real>() && fabs(R[1][2]) < 10 * r_eps<real>()) g[0] = 0;
+    else {
+        g[0] = FLIP ? r_atan2<real>(-R[1][2], -R[0][2]) : r_atan2<real>(R[1][2], R[0][2]);
+        if constexpr (std::is_void<SinCos>::value) { sp = sin(g[0]); cp = cos(g[0]); }
+        else SinCos()(g[0], sp, cp);
+    }
+    g[1] = r_atan2<real>(cp * R[0][2] + sp * R[1][2], R[2][2]);
+    g[2] = r_atan2<real>(-sp * R[0][0] + cp * R[1][0], -sp * R[0][1] + cp * R[1][1]);
 }
 #endif // __CUDACC__

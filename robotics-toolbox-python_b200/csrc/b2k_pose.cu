@@ -21,11 +21,6 @@
 
 namespace {
 
-template <typename real> __device__ __forceinline__ real r_atan2(real y, real x);
-template <> __device__ __forceinline__ double r_atan2<double>(double y, double x) { return atan2(y, x); }
-template <> __device__ __forceinline__ float r_atan2<float>(float y, float x) { return atan2f(y, x); }
-template <typename real> __device__ __forceinline__ real r_eps() { return sizeof(real) == 8 ? (real)2.220446049250313e-16 : (real)1.1920929e-07f; }
-
 // tr2rpy(order="zyx"): R = Rz(yaw) Ry(pitch) Rx(roll) -> (roll, pitch, yaw); at |R20| = 1 roll := 0
 template <typename real>
 __device__ __forceinline__ void rot_to_rpy_zyx(const real R[3][3], real g[3])
@@ -53,19 +48,6 @@ __device__ __forceinline__ void rot_to_rpy_xyz(const real R[3][3], real g[3])
         g[2] = -r_atan2<real>(R[1][2], R[2][2]);
         g[1] = r_atan2<real>(R[0][2], sqrt(R[0][0] * R[0][0] + R[0][1] * R[0][1]));
     }
-}
-// tr2eul: R = Rz(phi) Ry(theta) Rz(psi)
-template <typename real>
-__device__ __forceinline__ void rot_to_eul(const real R[3][3], real g[3])
-{
-    real sp = 0, cp = 1;
-    if (fabs(R[0][2]) < 10 * r_eps<real>() && fabs(R[1][2]) < 10 * r_eps<real>()) g[0] = 0;
-    else {
-        g[0] = r_atan2<real>(R[1][2], R[0][2]);
-        sp = sin(g[0]); cp = cos(g[0]);
-    }
-    g[1] = r_atan2<real>(cp * R[0][2] + sp * R[1][2], R[2][2]);
-    g[2] = r_atan2<real>(-sp * R[0][0] + cp * R[1][0], -sp * R[0][1] + cp * R[1][1]);
 }
 // trlog: exponential coordinates v = theta * axis
 template <typename real>

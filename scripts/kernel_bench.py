@@ -294,6 +294,45 @@ if want("opspace_"):
                    {"api": "public Python call on device-resident q, qd: jacob0_analytical, jacob0_dot, coriolis, inertia, b2k_opspace"})
         del qo, qdo, Ja, M, Cm, G, Jd, Mx, Cx, Gx
 
+# Closed-form IK (b2k_ikine_6s) of Puma560 on device-resident poses: one configuration, and all eight from one read of T.
+# Bytes per row = T in, q and the ok flags out: (16 + 6) reals + 4 for one, 16 reals + 8 (6 reals + 4) for eight.  The
+# share is against the data sheet's 3.35 TB/s; where it stays low the kernel is bound by FP64 issue (about a dozen
+# transcendental functions per configuration), not by HBM.  The card's name and power limit are read in the same run.
+if want("ikine_a_"):
+    import subprocess
+
+    try:
+        plim = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True,
+                              text=True, timeout=30).stdout.strip()
+    except Exception as e:  # the figure is context, the timing does not depend on it
+        plim = f"unavailable ({type(e).__name__})"
+    card = {"gpu": torch.cuda.get_device_name(0), "power_limit": plim}
+    puma = rtb.models.Puma560()
+    NI = args.rows
+    Tq = torch.from_numpy(rng.uniform(-np.pi, np.pi, (NI, 6))).to(dev)
+    T64 = puma.ets().eval(Tq)
+    Li = rtb._lib.lib()
+    sti = torch.cuda.current_stream().cuda_stream
+    dhi = np.ascontiguousarray([[l.d, l.a, l.alpha, l.offset] for l in puma.links], dtype=np.float64)
+    for dt, tag in ((np.float64, "f64"), (np.float32, "f32")):
+        Ti = T64 if dt == np.float64 else T64.float()
+        sz = np.dtype(dt).itemsize
+        for nc, bpr in ((1, (16 + 6) * sz + 4), (8, 16 * sz + 8 * (6 * sz + 4))):
+            case = f"ikine_a_puma_{nc}conf_{tag}"
+            if not want(case):
+                continue
+            conf = np.arange(nc, dtype=np.int32)
+            qi = torch.empty((NI, nc, 6), dtype=Ti.dtype, device=dev)
+            oki = torch.empty((NI, nc), dtype=torch.int32, device=dev)
+            code = rtb._lib.F64 if dt == np.float64 else rtb._lib.F32
+            ms = timeit(lambda i: rtb._lib.check(Li.b2k_ikine_6s(code, rtb._lib.dptr(dhi), None, None, Ti.data_ptr(), NI, nc,
+                                                                 conf.ctypes.data_as(rtb._lib.ip), qi.data_ptr(), oki.data_ptr(),
+                                                                 sti)), 1)
+            report(case, ms, NI, bpr, dict(card, api="C ABI, poses on the device", frac_of_3350=round(bpr * NI / (ms * 1e-3) / 3.35e12, 4),
+                                           solved=float(oki.float().mean())))
+            del qi, oki
+    del Tq, T64
+
 # IK (config 4): reachable targets, chan
 if want("ik_"):
     panda = rtb.models.Panda().ets()
