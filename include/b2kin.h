@@ -168,6 +168,30 @@ int b2k_ik_lm(b2k_chain_t chain, int dtype, const void *Tep, int64_t N, const vo
               int32_t *success, int32_t *iterations, int32_t *searches, void *residual,
               void *stream);
 
+/* The Python solver loop of b2k_ik_lm (always B2K_IK_SEM_PYTHON) with the null-space terms of the reference's
+ * IK_LM / IK_NR / IK_GN (IKSolver._calc_qnull / _null_Σ, IK.py), for redundant chains (7 <= n <= 10).  Arguments
+ * as b2k_ik_lm, plus:
+ *   kq   joint-limit avoidance gain; > 0 turns the term on (the reference's `if λΣ > 0`)
+ *   km   manipulability gain; > 0 turns the term on
+ *   ps   scalar; pi  host n-vector, the influence distance of each joint's limits
+ * Every step, at the pre-step q and with the unweighted base-frame J:
+ *   q <- q + dq_solver + qnull,  qnull = (I - pinv(J) J) g
+ *   g = [kq > 0] sigma(q) / kq + [km > 0] jacobm(q) / km       (jacobm as b2k_jacobm with all six axes)
+ *   sigma_i = +((q_i - l_i) - pi_i)^2 / (ps - pi_i)^2  if q_i - l_i <= pi_i
+ *           = -((h_i - q_i) - pi_i)^2 / (ps - pi_i)^2  if h_i - q_i <= pi_i (wins when both hold); 0 otherwise
+ * with l, h the chain's joint limits in chain order (a sub-chain of a larger robot uses its own joints, where the
+ * reference indexes its padded q by position).  The projector is formed as g - J^T (J J^T)^-1 J g from the Cholesky
+ * factor of J J^T; where that factor does not exist (J close to losing row rank) the search is abandoned, as a
+ * singular step is.  Rejected before any CUDA call: everything b2k_ik_lm rejects, n < 7 (a full-rank J of n <= 6
+ * joints has no null space: call b2k_ik_lm), non-finite kq, km, ps or pi, neither kq nor km > 0, and ps == pi[i]
+ * with kq > 0 (the reference divides by zero there).
+ */
+int b2k_ikine_null(b2k_chain_t chain, int dtype, const void *Tep, int64_t N, const void *q0,
+                   int ilimit, int slimit, double tol, int reject_jl, const double *we, double lambda,
+                   int method, uint64_t seed, int rng_per_row, double kq, double km, double ps,
+                   const double *pi, void *q_out, int32_t *success, int32_t *iterations,
+                   int32_t *searches, void *residual, void *stream);
+
 /* ---------------------------------------------------------------- inverse dynamics (DH RNE)
  * b2k_rne_create replaces frne.init (frne.c:233-299): n links, mdh = 0 standard / 1 modified
  * DH, L = 24 doubles per link packed as reference DHRobot.py:1340-1358

@@ -643,7 +643,8 @@ class ETS:
         return out[0] if single else out
 
     # ------------------------------------------------------------------ inverse kinematics
-    def _ik(self, Tep, q0, ilimit, slimit, tol, mask, joint_limits, k, method, seed, semantics, rng_per_row, dtype):
+    def _ik(self, Tep, q0, ilimit, slimit, tol, mask, joint_limits, k, method, seed, semantics, rng_per_row, dtype,
+            null=None):
         Tep = getattr(Tep, "A", Tep)
         B.check_numeric(Tep, "Tep")
         host = not B.is_tensor(Tep)
@@ -681,10 +682,18 @@ class ETS:
         E = B.empty((N,), dt, like=Td)
         if seed is None:
             seed = int(np.random.default_rng().integers(0, 2**63 - 1))
-        _lib.check(_lib.lib().b2k_ik_lm(
-            self._chain, B.code(dt), B.ptr(Td), N, B.ptr(q0d), int(ilimit), int(slimit), float(tol),
-            int(bool(joint_limits)), _lib.dptr(we), float(k), meth, int(seed) & (2**64 - 1), semantics,
-            int(bool(rng_per_row)), B.ptr(q), B.ptr(succ), B.ptr(its), B.ptr(srch), B.ptr(E), B.stream_ptr(Td)))
+        if null is None:
+            _lib.check(_lib.lib().b2k_ik_lm(
+                self._chain, B.code(dt), B.ptr(Td), N, B.ptr(q0d), int(ilimit), int(slimit), float(tol),
+                int(bool(joint_limits)), _lib.dptr(we), float(k), meth, int(seed) & (2**64 - 1), semantics,
+                int(bool(rng_per_row)), B.ptr(q), B.ptr(succ), B.ptr(its), B.ptr(srch), B.ptr(E), B.stream_ptr(Td)))
+        else:  # the Python loop with the null-space terms (semantics is SEM_PYTHON)
+            kq, km, ps, pi = null
+            _lib.check(_lib.lib().b2k_ikine_null(
+                self._chain, B.code(dt), B.ptr(Td), N, B.ptr(q0d), int(ilimit), int(slimit), float(tol),
+                int(bool(joint_limits)), _lib.dptr(we), float(k), meth, int(seed) & (2**64 - 1),
+                int(bool(rng_per_row)), float(kq), float(km), float(ps), _lib.dptr(pi), B.ptr(q), B.ptr(succ),
+                B.ptr(its), B.ptr(srch), B.ptr(E), B.stream_ptr(Td)))
         if host:
             q, succ, its, srch, E = (B.to_host(x) for x in (q, succ, its, srch, E))
         return q, succ, its, srch, E, single
@@ -726,11 +735,33 @@ class ETS:
         return self._ik_tuple(self._ik(Tep, q0, ilimit, slimit, tol, mask, joint_limits, 0.0, _lib.IK_GN,
                                        seed, _lib.SEM_CPP, True, dtype))
 
-    def _ikine(self, meth, Tep, q0, ilimit, slimit, tol, mask, joint_limits, seed, k, kq, km, dtype) -> IKSolution:
-        if kq != 0.0 or km != 0.0:
-            raise NotImplementedError("null-space terms (kq, km) are outside the accelerated path (SURVEY 2.1 row 5)")
+    def _null_args(self, kq, km, ps, pi):
+        """(kq, km, ps, pi as an n-vector) for b2k_ikine_null, or None when neither null-space term is on.
+        The terms of the reference's _calc_qnull run only for a gain > 0; on a chain of n <= 6 joints a full-rank J
+        has no null space, and the terms are accepted (their arguments still checked) and ignored (DESIGN (f-7))."""
+        kq, km = float(kq), float(km)
+        if not (kq > 0 or km > 0):
+            return None
+        n = self.n
+        pa = np.asarray(pi, dtype=np.float64)
+        if pa.ndim == 0:
+            pa = np.full(n, float(pa))
+        elif pa.shape != (n,):
+            raise ValueError(f"pi must be a scalar or have {n} elements, got shape {pa.shape}")
+        pa = np.ascontiguousarray(pa)
+        ps = float(ps)
+        if not (np.isfinite(kq) and np.isfinite(km) and np.isfinite(ps) and np.isfinite(pa).all()):
+            raise ValueError("kq, km, ps and pi must be finite")
+        if kq > 0 and (pa == ps).any():
+            raise ValueError(f"ps == pi at joint {int(np.argmax(pa == ps))}: the joint-limit term divides by ps - pi")
+        if n < 7:
+            return None
+        return kq, km, ps, pa
+
+    def _ikine(self, meth, Tep, q0, ilimit, slimit, tol, mask, joint_limits, seed, k, kq, km, dtype, ps=0.0,
+               pi=0.3) -> IKSolution:
         q, s, it, sr, E, single = self._ik(Tep, q0, ilimit, slimit, tol, mask, joint_limits, k, meth, seed,
-                                           _lib.SEM_PYTHON, False, dtype)
+                                           _lib.SEM_PYTHON, False, dtype, null=self._null_args(kq, km, ps, pi))
         if B.is_tensor(q):
             q, s, it, sr, E = (B.to_host(x) for x in (q, s, it, sr, E))
         fail = "iteration and search limit reached"
@@ -747,14 +778,16 @@ class ETS:
                  km: float = 0.0, ps: float = 0.0, pi=0.3, dtype=None, **kwargs) -> IKSolution:
         """Newton-Raphson IK with the semantics of the reference's Python solver class (ETS.ikine_NR,
         ETS.py:2639-2776 -> IK_NR, IK.py:579-762: q += pinv(J) e or inv(J) e -- the same vector)."""
-        return self._ikine(_lib.IK_NR, Tep, q0, ilimit, slimit, tol, mask, joint_limits, seed, 0.0, kq, km, dtype)
+        return self._ikine(_lib.IK_NR, Tep, q0, ilimit, slimit, tol, mask, joint_limits, seed, 0.0, kq, km, dtype,
+                           ps, pi)
 
     def ikine_GN(self, Tep, q0=None, ilimit: int = 30, slimit: int = 100, tol: float = 1e-6, mask=None,
                  joint_limits: bool = True, seed: Optional[int] = None, pinv: bool = False, kq: float = 0.0,
                  km: float = 0.0, ps: float = 0.0, pi=0.3, dtype=None, **kwargs) -> IKSolution:
         """Gauss-Newton IK with the semantics of the reference's Python solver class (ETS.ikine_GN,
         ETS.py:2778-2930 -> IK_GN, IK.py:1020-1219; its step is also q += pinv(J) e, IK.py:1214-1217)."""
-        return self._ikine(_lib.IK_NR, Tep, q0, ilimit, slimit, tol, mask, joint_limits, seed, 0.0, kq, km, dtype)
+        return self._ikine(_lib.IK_NR, Tep, q0, ilimit, slimit, tol, mask, joint_limits, seed, 0.0, kq, km, dtype,
+                           ps, pi)
 
     def ikine_LM(self, Tep, q0=None, ilimit: int = 30, slimit: int = 100, tol: float = 1e-6, mask=None,
                  joint_limits: bool = True, seed: Optional[int] = None, k: float = 1.0, method: str = "chan",
@@ -763,4 +796,4 @@ class ETS:
         (ETS.ikine_LM, ETS.py:2443-2637 -> IK_LM.solve, IK.py:174-367, 912-1017): returns an
         :class:`IKSolution`; for an (N,4,4) trajectory q is (N,n), success is the conjunction,
         iterations / searches are summed and residual is the minimum (IK.py:263-290)."""
-        return self._ikine(method, Tep, q0, ilimit, slimit, tol, mask, joint_limits, seed, k, kq, km, dtype)
+        return self._ikine(method, Tep, q0, ilimit, slimit, tol, mask, joint_limits, seed, k, kq, km, dtype, ps, pi)

@@ -486,6 +486,55 @@ extern "C" int b2k_ik_lm(b2k_chain_t c, int dtype, const void *Tep, int64_t N, c
                              rng_per_row, q_out, success, iterations, searches, residual, st);
 }
 
+int b2k_ik_ns_launch_f32(const b2k_chain_s *, const void *, long long, const void *, int, int, double, int, const double *,
+                         double, int, unsigned long long, int, void *, int *, int *, int *, void *, const IkNullArgs &,
+                         cudaStream_t);
+int b2k_ik_ns_launch_f64(const b2k_chain_s *, const void *, long long, const void *, int, int, double, int, const double *,
+                         double, int, unsigned long long, int, void *, int *, int *, int *, void *, const IkNullArgs &,
+                         cudaStream_t);
+
+extern "C" int b2k_ikine_null(b2k_chain_t c, int dtype, const void *Tep, int64_t N, const void *q0, int ilimit,
+                              int slimit, double tol, int reject_jl, const double *we, double lambda, int method,
+                              uint64_t seed, int rng_per_row, double kq, double km, double ps, const double *pi,
+                              void *q_out, int32_t *success, int32_t *iterations, int32_t *searches, void *residual,
+                              void *stream)
+{
+    const char *fn = "b2k_ikine_null";
+    if (!c) { b2k_set_error("%s: chain handle is NULL", fn); return B2K_ERR_INVALID; }
+    if (dtype != B2K_F32 && dtype != B2K_F64) { b2k_set_error("%s: dtype must be B2K_F32 or B2K_F64", fn); return B2K_ERR_INVALID; }
+    if (N < 0) { b2k_set_error("%s: N is negative", fn); return B2K_ERR_INVALID; }
+    if (!c->distinct_jindex) {
+        b2k_set_error("%s: two joints of the chain share a jindex (coupled joints are outside the solver's model)", fn);
+        return B2K_ERR_INVALID;
+    }
+    if (c->n < 7 || c->n > B2K_MAX_JOINTS) {
+        b2k_set_error("%s: the null-space terms need a redundant chain of 7..%d joints (n = %d)", fn, B2K_MAX_JOINTS, c->n);
+        return B2K_ERR_INVALID;
+    }
+    if (ilimit < 1 || slimit < 1) { b2k_set_error("%s: ilimit and slimit must be >= 1", fn); return B2K_ERR_INVALID; }
+    if (method < B2K_LM_CHAN || method > B2K_IK_GN) { b2k_set_error("%s: bad method %d", fn, method); return B2K_ERR_INVALID; }
+    if (!isfinite(kq) || !isfinite(km)) { b2k_set_error("%s: kq and km must be finite", fn); return B2K_ERR_INVALID; }
+    if (!(kq > 0) && !(km > 0)) { b2k_set_error("%s: at least one of kq and km must be > 0", fn); return B2K_ERR_INVALID; }
+    if (!isfinite(ps)) { b2k_set_error("%s: ps must be finite", fn); return B2K_ERR_INVALID; }
+    if (!pi) { b2k_set_error("%s: pi is NULL", fn); return B2K_ERR_INVALID; }
+    for (int i = 0; i < c->n; i++) {
+        if (!isfinite(pi[i])) { b2k_set_error("%s: pi[%d] is not finite", fn, i); return B2K_ERR_INVALID; }
+        if (kq > 0 && ps == pi[i]) { b2k_set_error("%s: ps == pi[%d] divides by zero in the joint-limit term", fn, i); return B2K_ERR_INVALID; }
+    }
+    int rc;
+    if ((rc = check_out(fn, "Tep", Tep, N)) || (rc = check_out(fn, "q_out", q_out, N)) ||
+        (rc = check_out(fn, "success", success, N)) || (rc = check_out(fn, "iterations", iterations, N)) ||
+        (rc = check_out(fn, "searches", searches, N)) || (rc = check_out(fn, "residual", residual, N)))
+        return rc;
+    if ((method == B2K_IK_NR || method == B2K_IK_GN) && lambda < 0) { b2k_set_error("%s: pinv_damping is negative", fn); return B2K_ERR_INVALID; }
+    if (N == 0) return B2K_OK;
+    B2K_ON_DEVICE_OF(Tep);
+    const IkNullArgs ns{kq, km, ps, pi};
+    auto launch = dtype == B2K_F64 ? b2k_ik_ns_launch_f64 : b2k_ik_ns_launch_f32;
+    return launch(c, Tep, N, q0, ilimit, slimit, tol, reject_jl, we, method == B2K_IK_GN ? 0.0 : lambda, method, seed,
+                  rng_per_row, q_out, success, iterations, searches, residual, ns, (cudaStream_t)stream);
+}
+
 // ------------------------------------------------------------------ dynamics fan-outs
 int b2k_rne_fan_launch_f32(const b2k_rne_s *, int, const void *, const void *, const void *, long long, const double *, void *, cudaStream_t);
 int b2k_rne_fan_launch_f64(const b2k_rne_s *, int, const void *, const void *, const void *, long long, const double *, void *, cudaStream_t);

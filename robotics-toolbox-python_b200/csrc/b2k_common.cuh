@@ -100,6 +100,12 @@ struct b2k_chain_s {
     int distinct_jindex; // no two joints read the same column of q
 };
 
+// null-space gains and influence band of b2k_ikine_null, as the host passes them (validated there; b2k_ik.cuh)
+struct IkNullArgs {
+    double kq, km, ps;
+    const double *pi; // host, n
+};
+
 struct b2k_rne_s {
     int n, mdh;
     double L[B2K_MAX_JOINTS][24];

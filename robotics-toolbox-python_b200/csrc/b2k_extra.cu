@@ -322,7 +322,8 @@ __global__ void __launch_bounds__(128) k_yoshikawa(const real *__restrict__ J, l
 // pivot search, which would need run-time row indices -- i.e. local memory) gives m = sqrt(det A) = prod L_jj and the
 // columns G[:, k] = A^-1 J[:, k]; then  sum_{a,b} (J H_i^T)[a,b] A^-1[a,b] = sum_{b,k} H_i[b,k] G[b,k]  (A^-1 is
 // symmetric), which needs the Hessian terms once per (i, b, k) instead of once per (i, a, b, k): ~1 800 operations per
-// row instead of ~14 000.  The general kernel below (na read at run time, Gauss-Jordan with pivoting, every array in
+// row instead of ~14 000.  The Gram factor and the Hessian terms come from b2k_gram_chol6 / b2k_hess_term (b2k_ik.cuh),
+// which the IK null-space term shares.  The general kernel below (na read at run time, Gauss-Jordan with pivoting, every array in
 // local memory) is far slower.
 template <typename real, int N>
 __global__ void __launch_bounds__(128) k_jacobm_all(const real *__restrict__ J, long long nrows, real *__restrict__ Jm)
@@ -335,21 +336,9 @@ __global__ void __launch_bounds__(128) k_jacobm_all(const real *__restrict__ J, 
     real j[6 * N];
 #pragma unroll
     for (int e = 0; e < 6 * N; e++) j[e] = jr[e];
-    real A[21];
-#pragma unroll
-    for (int a = 0; a < 6; a++)
-#pragma unroll
-        for (int b = 0; b <= a; b++) {
-            real s = 0;
-#pragma unroll
-            for (int k = 0; k < N; k++) s = fma(j[a * N + k], j[b * N + k], s);
-            A[a * (a + 1) / 2 + b] = s;
-        }
-    ik_chol_factor<real, 6>(A); // a singular Gram matrix ends in inf / nan, as numpy's inv does in the reference
-    real m = 1;
-#pragma unroll
-    for (int a = 0; a < 6; a++) m *= A[a * (a + 1) / 2 + a]; // the diagonal holds 1 / L_aa
-    m = (real)1 / m;
+    auto jx = [&](int a, int k) { return j[a * N + k]; };
+    real A[21], m;
+    b2k_gram_chol6<real, N>(jx, A, m); // a singular Gram matrix ends in inf / nan, as numpy's inv does in the reference
     real G[6 * N];
 #pragma unroll
     for (int k = 0; k < N; k++) {
@@ -364,18 +353,10 @@ __global__ void __launch_bounds__(128) k_jacobm_all(const real *__restrict__ J, 
     for (int i = 0; i < N; i++) {
         real acc = 0;
 #pragma unroll
-        for (int r = 0; r < 6; r++) {
-            const int cc = r % 3, c1 = (cc + 1) % 3, c2 = (cc + 2) % 3, wrow = r < 3 ? 0 : 3;
+        for (int r = 0; r < 6; r++)
 #pragma unroll
-            for (int k = 0; k < N; k++) {
-                if (k >= i || r < 3) { // H_i[r, k], methods.cpp:16-32 (zero for the angular rows below the diagonal)
-                    const int lo = k >= i ? i : k, hi = k >= i ? k : i;
-                    const real u1 = j[(3 + c1) * N + lo], u2 = j[(3 + c2) * N + lo];
-                    const real w1 = j[(wrow + c1) * N + hi], w2 = j[(wrow + c2) * N + hi];
-                    acc = fma(fma(u1, w2, -(u2 * w1)), G[r * N + k], acc);
-                }
-            }
-        }
+            for (int k = 0; k < N; k++)
+                if (k >= i || r < 3) acc = fma(b2k_hess_term<real>(jx, i, r, k), G[r * N + k], acc);
         Jm[row * N + i] = m * acc;
     }
 }

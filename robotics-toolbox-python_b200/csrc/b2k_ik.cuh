@@ -190,6 +190,123 @@ __device__ __forceinline__ bool ik_chol_solve(real *A, real *b)
     return ok;
 }
 
+// ------------------------------------------------------------------ manipulability Jacobian pieces (ETS.jacobm, all six axes)
+// For a 6 x N Jacobian (jx(a, k) = J[a, k]) with Gram matrix A = J J^T and Yoshikawa's m = sqrt(det A):
+//   jacobm[i] = m * sum_{b,k} H_i[b,k] G[b,k],   G[:, k] = A^-1 J[:, k]   (A^-1 symmetric)
+// k_jacobm_all (b2k_extra.cu) and the null-space term of the IK step below both use these two functions.
+// b2k_gram_chol6: A = J J^T factorised in place by ik_chol_factor; returns m = prod L_aa (false: not factorisable;
+// m and the factor are then inf / nan, as numpy's inv leaves them in the reference).
+template <typename real, int N, typename JX>
+__device__ __forceinline__ bool b2k_gram_chol6(JX jx, real *A, real &m)
+{
+#pragma unroll
+    for (int a = 0; a < 6; a++)
+#pragma unroll
+        for (int b = 0; b <= a; b++) {
+            real s = 0;
+#pragma unroll
+            for (int k = 0; k < N; k++) s = fma(jx(a, k), jx(b, k), s);
+            A[a * (a + 1) / 2 + b] = s;
+        }
+    const bool ok = ik_chol_factor<real, 6>(A);
+    m = 1;
+#pragma unroll
+    for (int a = 0; a < 6; a++) m *= A[a * (a + 1) / 2 + a]; // the diagonal holds 1 / L_aa
+    m = (real)1 / m;
+    return ok;
+}
+
+// H_i[r, k] of the Hessian (methods.cpp:16-32) formed from J on the fly.  Only for k >= i or r < 3: the angular rows
+// below the diagonal are zero and the callers skip them.
+template <typename real, typename JX>
+__device__ __forceinline__ real b2k_hess_term(JX jx, int i, int r, int k)
+{
+    const int cc = r % 3, c1 = (cc + 1) % 3, c2 = (cc + 2) % 3, wrow = r < 3 ? 0 : 3;
+    const int lo = k >= i ? i : k, hi = k >= i ? k : i;
+    const real u1 = jx(3 + c1, lo), u2 = jx(3 + c2, lo);
+    const real w1 = jx(wrow + c1, hi), w2 = jx(wrow + c2, hi);
+    return fma(u1, w2, -(u2 * w1));
+}
+
+// ------------------------------------------------------------------ null-space motion of the Python solver loop
+// Reference IKSolver._calc_qnull / _null_Σ (restated in DESIGN (f-7)); host side: b2k_ikine_null.
+//   qnull = (I - J^T (J J^T)^-1 J) g,   g = inv_kq sigma(q) + inv_km jacobm(q)
+//   sigma_i = +((q_i - l_i) - pi_i)^2 / (ps - pi_i)^2   if q_i - l_i <= pi_i
+//           = -((h_i - q_i) - pi_i)^2 / (ps - pi_i)^2   if h_i - q_i <= pi_i   (wins when both hold)
+// use_q / use_m switch the terms (gain > 0 in the reference); inv_kq = 1 / kq, inv_km = 1 / km.
+template <typename real, int N>
+struct IkNs {
+    real inv_kq, inv_km, ps;
+    real pi[N];
+    int use_q, use_m;
+};
+
+// qn <- qnull at q, from the unweighted base-frame J (J[k][a]).  The projector I - pinv(J) J is formed from the
+// Cholesky factor of J J^T that the manipulability term needs anyway.  False when J J^T cannot be factorised (J has
+// lost row rank): the caller abandons the search, as the step itself does at a singular normal matrix.
+template <typename real, int N>
+__device__ __forceinline__ bool ik_null_motion(const IkP<real, N> &K, const IkNs<real, N> &S, const real (*J)[6],
+                                               const real *q, real *qn)
+{
+    auto jx = [&](int a, int k) { return J[k][a]; };
+    real A[21], m;
+    const bool ok = b2k_gram_chol6<real, N>(jx, A, m);
+#pragma unroll
+    for (int i = 0; i < N; i++) {
+        real s = 0;
+        if (S.use_q) {
+            const real dl = q[i] - K.qlim_l[i], dh = K.qlim_h[i] - q[i], d = S.ps - S.pi[i];
+            if (dh <= S.pi[i]) {
+                const real t = dh - S.pi[i];
+                s = -(t * t) / (d * d);
+            } else if (dl <= S.pi[i]) {
+                const real t = dl - S.pi[i];
+                s = (t * t) / (d * d);
+            }
+            s *= S.inv_kq;
+        }
+        qn[i] = s;
+    }
+    if (S.use_m) {
+        // G is streamed one column at a time (x = A^-1 J[:, k]) into the N sums instead of being held whole
+        real acc[N];
+#pragma unroll
+        for (int i = 0; i < N; i++) acc[i] = 0;
+#pragma unroll
+        for (int k = 0; k < N; k++) {
+            real x[6];
+#pragma unroll
+            for (int a = 0; a < 6; a++) x[a] = J[k][a];
+            ik_chol_subst<real, 6>(A, x);
+#pragma unroll
+            for (int i = 0; i < N; i++)
+#pragma unroll
+                for (int r = 0; r < 6; r++)
+                    if (k >= i || r < 3) acc[i] = fma(b2k_hess_term<real>(jx, i, r, k), x[r], acc[i]);
+        }
+        const real c = S.inv_km * m;
+#pragma unroll
+        for (int i = 0; i < N; i++) qn[i] = fma(c, acc[i], qn[i]);
+    }
+    real y[6];
+#pragma unroll
+    for (int a = 0; a < 6; a++) {
+        real s = 0;
+#pragma unroll
+        for (int k = 0; k < N; k++) s = fma(J[k][a], qn[k], s);
+        y[a] = s;
+    }
+    ik_chol_subst<real, 6>(A, y);
+#pragma unroll
+    for (int k = 0; k < N; k++) {
+        real s = qn[k];
+#pragma unroll
+        for (int a = 0; a < 6; a++) s = fma(-J[k][a], y[a], s);
+        qn[k] = s;
+    }
+    return ok;
+}
+
 // ------------------------------------------------------------------ one LM evaluation (+ update) in registers
 // Evaluates the pose error e and cost E at q, then forms the Jacobian, the normal equations and the
 // damped update dq (left in g).  Returns false when A cannot be factorised.
@@ -254,9 +371,11 @@ __device__ __forceinline__ bool ik_pinv_step(const IkP<real, N> &K, real (*J)[6]
     }
 }
 
-template <typename real, int N, int PROF, int STEP = 0>
+// NS: add the null-space motion of IkNs S (Python semantics, N >= 7 only) to the update; S is unused otherwise.
+template <typename real, int N, int PROF, int STEP = 0, bool NS = false>
 __device__ __forceinline__ bool ik_eval(const ChainP<real, N> &P, const IkP<real, N> &K, const real *Tp, const real *q,
-                                        real &Ecur, real *g, bool skip_step_if_converged)
+                                        real &Ecur, real *g, bool skip_step_if_converged,
+                                        const IkNs<real, N> *S = nullptr)
 {
     Pose<real> Te;
     real zj[N][3], pj[N][3], e[6];
@@ -289,7 +408,18 @@ __device__ __forceinline__ bool ik_eval(const ChainP<real, N> &P, const IkP<real
             J[j][3] = 0; J[j][4] = 0; J[j][5] = 0;
         }
     }
-    if (STEP == 1) return ik_pinv_step<real, N>(K, J, e, g);
+    real qn[N];
+    bool nok = true;
+    if constexpr (NS) nok = ik_null_motion<real, N>(K, *S, J, q, qn); // before ik_pinv_step weighs J in place
+    auto add_null = [&](bool ok) { // q += dq + qnull (IK_LM.step / IK_NR.step / IK_GN.step)
+        if constexpr (NS) {
+#pragma unroll
+            for (int i = 0; i < N; i++) g[i] += qn[i];
+            return ok && nok;
+        }
+        return ok;
+    };
+    if (STEP == 1) return add_null(ik_pinv_step<real, N>(K, J, e, g));
     const real wn = (K.method == B2K_LM_CHAN) ? K.lambda * E : (K.method == B2K_LM_WAMPLER) ? K.lambda : (E + K.lambda);
     real A[N * (N + 1) / 2];
     if (K.unit_w) {
@@ -323,7 +453,7 @@ __device__ __forceinline__ bool ik_eval(const ChainP<real, N> &P, const IkP<real
             }
         }
     }
-    return ik_chol_solve<real, N>(A, g);
+    return add_null(ik_chol_solve<real, N>(A, g));
 }
 
 // wrap to [-pi, pi) the way each reference loop does, and test the joint limits
@@ -359,14 +489,21 @@ template <typename real> constexpr int ik_min_blocks() { return B2K_IK_MINB; }
 #else
 template <typename real> constexpr int ik_min_blocks() { return sizeof(real) == 4 ? 4 : 3; }
 #endif
-template <typename real, int N, int PROF, int STEP = 0>
-__global__ void __launch_bounds__(B2K_THREADS, ik_min_blocks<real>())
-k_ik_lm(const __grid_constant__ ChainP<real, N> P, const __grid_constant__ IkP<real, N> K,
-        const real *__restrict__ Tep, const real *__restrict__ q0, long long nprob, real *__restrict__ q_out,
-        int *__restrict__ success, int *__restrict__ iterations, int *__restrict__ searches,
-        real *__restrict__ residual, int two_phase, int *__restrict__ hard_idx, int *__restrict__ hard_count,
-        int iter_cap, const int *__restrict__ in_list, const int *__restrict__ in_count, int *__restrict__ cont_idx,
-        int *__restrict__ cont_count)
+// The kernels with the null-space term (k_ik_lm_ns, k_ik_restarts_ns) hold J, the Gram factor and the N Hessian sums
+// at once.  Chosen from -Xptxas -v: fp32 fits 168 registers (3 blocks) without spilling up to N = 9 and 255 (2 blocks)
+// at N = 10; fp64 at 255 (2 blocks) spills less than the plain fp64 k_ik_lm does at 168 (DESIGN (f-7) has the table).
+template <typename real, int N> constexpr int ik_ns_min_blocks() { return sizeof(real) == 4 && N <= 9 ? 3 : 2; }
+
+// The bodies of the two kernels are shared by the plain kernels (k_ik_lm, k_ik_restarts) and their null-space
+// variants (k_ik_lm_ns, k_ik_restarts_ns, NS = true, S = their IkNs parameter); S is unused when NS is false.
+template <typename real, int N, int PROF, int STEP, bool NS>
+__device__ __forceinline__ void
+ik_lm_body(const ChainP<real, N> &P, const IkP<real, N> &K, const IkNs<real, N> *S,
+           const real *__restrict__ Tep, const real *__restrict__ q0, long long nprob, real *__restrict__ q_out,
+           int *__restrict__ success, int *__restrict__ iterations, int *__restrict__ searches,
+           real *__restrict__ residual, int two_phase, int *__restrict__ hard_idx, int *__restrict__ hard_count,
+           int iter_cap, const int *__restrict__ in_list, const int *__restrict__ in_count, int *__restrict__ cont_idx,
+           int *__restrict__ cont_count)
 {
     // Segmented first search (two_phase only): with iter_cap > 0 a problem that is still iterating after iter_cap
     // evaluations in THIS launch parks its state (q in q_out, the search's evaluation count in iterations) and is
@@ -457,7 +594,7 @@ k_ik_lm(const __grid_constant__ ChainP<real, N> P, const __grid_constant__ IkP<r
         real g[N], Ecur;
         // one call site for both loop orders (the evaluation is ~600 instructions; two inlined copies only cost
         // instruction-cache misses): the C++ order skips the step when the test before it has already passed
-        const bool ok = ik_eval<real, N, PROF, STEP>(P, K, Tp, q, Ecur, g, cpp);
+        const bool ok = ik_eval<real, N, PROF, STEP, NS>(P, K, Tp, q, Ecur, g, cpp, S);
         E = Ecur;
         if (cpp) {
             // test before stepping (ik.cpp:44-58)
@@ -493,6 +630,34 @@ k_ik_lm(const __grid_constant__ ChainP<real, N> P, const __grid_constant__ IkP<r
     }
 }
 
+template <typename real, int N, int PROF, int STEP = 0>
+__global__ void __launch_bounds__(B2K_THREADS, ik_min_blocks<real>())
+k_ik_lm(const __grid_constant__ ChainP<real, N> P, const __grid_constant__ IkP<real, N> K,
+        const real *__restrict__ Tep, const real *__restrict__ q0, long long nprob, real *__restrict__ q_out,
+        int *__restrict__ success, int *__restrict__ iterations, int *__restrict__ searches,
+        real *__restrict__ residual, int two_phase, int *__restrict__ hard_idx, int *__restrict__ hard_count,
+        int iter_cap, const int *__restrict__ in_list, const int *__restrict__ in_count, int *__restrict__ cont_idx,
+        int *__restrict__ cont_count)
+{
+    ik_lm_body<real, N, PROF, STEP, false>(P, K, nullptr, Tep, q0, nprob, q_out, success, iterations, searches, residual,
+                                           two_phase, hard_idx, hard_count, iter_cap, in_list, in_count, cont_idx,
+                                           cont_count);
+}
+
+template <typename real, int N, int PROF, int STEP>
+__global__ void __launch_bounds__(B2K_THREADS, ik_ns_min_blocks<real, N>())
+k_ik_lm_ns(const __grid_constant__ ChainP<real, N> P, const __grid_constant__ IkP<real, N> K,
+           const real *__restrict__ Tep, const real *__restrict__ q0, long long nprob, real *__restrict__ q_out,
+           int *__restrict__ success, int *__restrict__ iterations, int *__restrict__ searches,
+           real *__restrict__ residual, int two_phase, int *__restrict__ hard_idx, int *__restrict__ hard_count,
+           int iter_cap, const int *__restrict__ in_list, const int *__restrict__ in_count, int *__restrict__ cont_idx,
+           int *__restrict__ cont_count, const __grid_constant__ IkNs<real, N> S)
+{
+    ik_lm_body<real, N, PROF, STEP, true>(P, K, &S, Tep, q0, nprob, q_out, success, iterations, searches, residual,
+                                          two_phase, hard_idx, hard_count, iter_cap, in_list, in_count, cont_idx,
+                                          cont_count);
+}
+
 // ------------------------------------------------------------------ phase B: G lanes per hard problem, searches in parallel
 // The restart draws are counter-based (seed, row, search, joint), so search s of a problem does not
 // depend on searches 0..s-1.  A group of G lanes therefore runs G consecutive searches of one hard
@@ -500,13 +665,13 @@ k_ik_lm(const __grid_constant__ ChainP<real, N> P, const __grid_constant__ IkP<r
 // is the sum of the contributions of all lower-numbered searches plus its own -- exactly what
 // the sequential loop reports, but the latency of a problem needing k restarts drops from
 // k x ilimit LM iterations to ceil(k / G) x ilimit.
-template <typename real, int N, int PROF, int G, int STEP = 0>
-__global__ void __launch_bounds__(B2K_THREADS, ik_min_blocks<real>())
-k_ik_restarts(const __grid_constant__ ChainP<real, N> P, const __grid_constant__ IkP<real, N> K,
-              const real *__restrict__ Tep, real *__restrict__ q_out, int *__restrict__ success,
-              int *__restrict__ iterations, int *__restrict__ searches, real *__restrict__ residual,
-              const int *__restrict__ hard_idx, const int *__restrict__ hard_count, int s_first, int max_batches,
-              int *__restrict__ out_idx, int *__restrict__ out_count)
+template <typename real, int N, int PROF, int G, int STEP, bool NS>
+__device__ __forceinline__ void
+ik_restarts_body(const ChainP<real, N> &P, const IkP<real, N> &K, const IkNs<real, N> *S,
+                 const real *__restrict__ Tep, real *__restrict__ q_out, int *__restrict__ success,
+                 int *__restrict__ iterations, int *__restrict__ searches, real *__restrict__ residual,
+                 const int *__restrict__ hard_idx, const int *__restrict__ hard_count, int s_first, int max_batches,
+                 int *__restrict__ out_idx, int *__restrict__ out_count)
 {
     // s_first: first (0-based) search of this launch; max_batches: batches of G searches a problem may run here.
     // A problem still unsolved after max_batches batches is appended to out_idx (its iteration total parked in
@@ -544,7 +709,7 @@ k_ik_restarts(const __grid_constant__ ChainP<real, N> P, const __grid_constant__
             while (__any_sync(FULL, going)) {
                 if (going) {
                     real g[N], Ecur;
-                    const bool ok = ik_eval<real, N, PROF, STEP>(P, K, Tp, q, Ecur, g, cpp);
+                    const bool ok = ik_eval<real, N, PROF, STEP, NS>(P, K, Tp, q, Ecur, g, cpp, S);
                     E = Ecur;
                     if (cpp) {
                         if (Ecur < K.tol) {
@@ -621,11 +786,49 @@ k_ik_restarts(const __grid_constant__ ChainP<real, N> P, const __grid_constant__
     }
 }
 
-template <typename real, int N, int STEP>
+template <typename real, int N, int PROF, int G, int STEP = 0>
+__global__ void __launch_bounds__(B2K_THREADS, ik_min_blocks<real>())
+k_ik_restarts(const __grid_constant__ ChainP<real, N> P, const __grid_constant__ IkP<real, N> K,
+              const real *__restrict__ Tep, real *__restrict__ q_out, int *__restrict__ success,
+              int *__restrict__ iterations, int *__restrict__ searches, real *__restrict__ residual,
+              const int *__restrict__ hard_idx, const int *__restrict__ hard_count, int s_first, int max_batches,
+              int *__restrict__ out_idx, int *__restrict__ out_count)
+{
+    ik_restarts_body<real, N, PROF, G, STEP, false>(P, K, nullptr, Tep, q_out, success, iterations, searches, residual,
+                                                    hard_idx, hard_count, s_first, max_batches, out_idx, out_count);
+}
+
+template <typename real, int N, int PROF, int G, int STEP>
+__global__ void __launch_bounds__(B2K_THREADS, ik_ns_min_blocks<real, N>())
+k_ik_restarts_ns(const __grid_constant__ ChainP<real, N> P, const __grid_constant__ IkP<real, N> K,
+                 const real *__restrict__ Tep, real *__restrict__ q_out, int *__restrict__ success,
+                 int *__restrict__ iterations, int *__restrict__ searches, real *__restrict__ residual,
+                 const int *__restrict__ hard_idx, const int *__restrict__ hard_count, int s_first, int max_batches,
+                 int *__restrict__ out_idx, int *__restrict__ out_count, const __grid_constant__ IkNs<real, N> S)
+{
+    ik_restarts_body<real, N, PROF, G, STEP, true>(P, K, &S, Tep, q_out, success, iterations, searches, residual,
+                                                   hard_idx, hard_count, s_first, max_batches, out_idx, out_count);
+}
+
+// kernel selection for ik_launch_n: the plain kernels, or (NS) their null-space variants
+template <typename real, int N, int PROF, int STEP, bool NS>
+constexpr auto ik_kernel_a()
+{
+    if constexpr (NS) return &k_ik_lm_ns<real, N, PROF, STEP>;
+    else return &k_ik_lm<real, N, PROF, STEP>;
+}
+template <typename real, int N, int PROF, int G, int STEP, bool NS>
+constexpr auto ik_kernel_b()
+{
+    if constexpr (NS) return &k_ik_restarts_ns<real, N, PROF, G, STEP>;
+    else return &k_ik_restarts<real, N, PROF, G, STEP>;
+}
+
+template <typename real, int N, int STEP, bool NS = false>
 int ik_launch_n(const b2k_chain_s *c, const real *Tep, long long nprob, const real *q0, int ilimit, int slimit,
                 double tol, int reject_jl, const double *we, double lambda, int method, unsigned long long seed,
                 int semantics, int rng_per_row, real *q_out, int *success, int *iterations, int *searches,
-                real *residual, cudaStream_t st)
+                real *residual, cudaStream_t st, const IkNullArgs *ns = nullptr)
 {
     ChainP<real, N> P;
     b2k_fill_chain<real, N>(c, nullptr, nullptr, true, P);
@@ -641,6 +844,20 @@ int ik_launch_n(const b2k_chain_s *c, const real *Tep, long long nprob, const re
     K.lambda = (real)lambda; K.tol = (real)tol;
     K.ilimit = ilimit; K.slimit = slimit; K.method = method; K.reject_jl = reject_jl ? 1 : 0;
     K.semantics = semantics; K.rng_per_row = rng_per_row ? 1 : 0; K.has_q0 = q0 ? 1 : 0; K.seed = seed;
+    IkNs<real, N> S{};
+    if constexpr (NS) {
+        S.use_q = ns->kq > 0 ? 1 : 0;
+        S.use_m = ns->km > 0 ? 1 : 0;
+        S.inv_kq = S.use_q ? (real)(1.0 / ns->kq) : (real)0; // the reference scales by 1.0 / λ (IK.py _calc_qnull)
+        S.inv_km = S.use_m ? (real)(1.0 / ns->km) : (real)0;
+        S.ps = (real)ns->ps;
+        for (int i = 0; i < N; i++) S.pi[i] = (real)ns->pi[i];
+    }
+    // one launch of kern (NS: with S appended as its last argument)
+    auto go = [&](auto kern, long long grid, auto... a) {
+        if constexpr (NS) kern<<<(unsigned)grid, B2K_THREADS, 0, st>>>(a..., S);
+        else kern<<<(unsigned)grid, B2K_THREADS, 0, st>>>(a...);
+    };
     // Two phases when restarts are allowed and the batch is large enough to matter: phase A runs the
     // first search of every problem (one lane each); phase B runs the restarts of the problems that
     // failed it with B2K_IK_GROUP lanes per problem.  Scratch (hard list + counter) is stream-ordered.
@@ -671,15 +888,13 @@ int ik_launch_n(const b2k_chain_s *c, const real *Tep, long long nprob, const re
         if (grid > need || mode >= 1) grid = need;
         if (grid < 1) grid = 1;
         const bool seg = mode == 2 && ilimit > IK_SEG1 + 2;
-        kern<<<(unsigned)grid, B2K_THREADS, 0, st>>>(P, K, Tep, q0, nprob, q_out, success, iterations, searches, residual,
-                                                     two_phase ? 1 : 0, hard_idx, hard_count, seg ? IK_SEG1 : 0, nullptr,
-                                                     nullptr, cont_idx, park_count);
+        go(kern, grid, P, K, Tep, q0, nprob, q_out, success, iterations, searches, residual, two_phase ? 1 : 0, hard_idx,
+           hard_count, seg ? IK_SEG1 : 0, (const int *)nullptr, (const int *)nullptr, cont_idx, park_count);
         b2k_count_launch();
         B2K_CUDA(cudaGetLastError());
         if (seg) { // second segment: the parked problems, re-packed (the list length is only known on the device)
-            kern<<<(unsigned)grid, B2K_THREADS, 0, st>>>(P, K, Tep, q0, nprob, q_out, success, iterations, searches,
-                                                         residual, 1, hard_idx, hard_count, 0, cont_idx, park_count, nullptr,
-                                                         nullptr);
+            go(kern, grid, P, K, Tep, q0, nprob, q_out, success, iterations, searches, residual, 1, hard_idx, hard_count, 0,
+               (const int *)cont_idx, (const int *)park_count, (int *)nullptr, (int *)nullptr);
             b2k_count_launch();
             B2K_CUDA(cudaGetLastError());
         }
@@ -694,13 +909,13 @@ int ik_launch_n(const b2k_chain_s *c, const real *Tep, long long nprob, const re
         long long need = (nprob * g + B2K_THREADS - 1) / B2K_THREADS; // upper bound: every problem hard
         if (grid > need) grid = need;
         if (grid < 1) grid = 1;
-        kern<<<(unsigned)grid, B2K_THREADS, 0, st>>>(P, K, Tep, q_out, success, iterations, searches, residual, list, count,
-                                                     s_first, max_batches, out_list, out_cnt);
+        go(kern, grid, P, K, Tep, q_out, success, iterations, searches, residual, list, count, s_first, max_batches,
+           out_list, out_cnt);
         b2k_count_launch();
         B2K_CUDA(cudaGetLastError());
         return B2K_OK;
     };
-    int rc = c->dh_like ? launch_a(k_ik_lm<real, N, 1, STEP>) : launch_a(k_ik_lm<real, N, 0, STEP>);
+    int rc = c->dh_like ? launch_a(ik_kernel_a<real, N, 1, STEP, NS>()) : launch_a(ik_kernel_a<real, N, 0, STEP, NS>());
     if (rc == B2K_OK && two_phase) {
         // B2K_IK_ROUNDS: 1 = a single round of 8-lane groups; 2 = 4 lanes for searches 1-4, then 8 lanes to the end;
         // 3 (default) = 4 lanes, ONE batch of 8 lanes (searches 5-12), then whole warps (32 searches per batch) for the
@@ -709,20 +924,20 @@ int ik_launch_n(const b2k_chain_s *c, const real *Tep, long long nprob, const re
         static const int rounds_env = getenv("B2K_IK_ROUNDS") ? atoi(getenv("B2K_IK_ROUNDS")) : 3;
         constexpr int G1 = 4, G3 = 32;
         if (rounds_env >= 2 && slimit > 1 + G1) {
-            rc = c->dh_like ? launch_b(k_ik_restarts<real, N, 1, G1, STEP>, G1, hard_idx, hard_count, 1, 1, cont_idx, cont_count)
-                            : launch_b(k_ik_restarts<real, N, 0, G1, STEP>, G1, hard_idx, hard_count, 1, 1, cont_idx, cont_count);
+            rc = c->dh_like ? launch_b(ik_kernel_b<real, N, 1, G1, STEP, NS>(), G1, hard_idx, hard_count, 1, 1, cont_idx, cont_count)
+                            : launch_b(ik_kernel_b<real, N, 0, G1, STEP, NS>(), G1, hard_idx, hard_count, 1, 1, cont_idx, cont_count);
             if (rc == B2K_OK && rounds_env >= 3 && slimit > 1 + G1 + G) {
-                rc = c->dh_like ? launch_b(k_ik_restarts<real, N, 1, G, STEP>, G, cont_idx, cont_count, 1 + G1, 1, hard_idx, third_count)
-                                : launch_b(k_ik_restarts<real, N, 0, G, STEP>, G, cont_idx, cont_count, 1 + G1, 1, hard_idx, third_count);
+                rc = c->dh_like ? launch_b(ik_kernel_b<real, N, 1, G, STEP, NS>(), G, cont_idx, cont_count, 1 + G1, 1, hard_idx, third_count)
+                                : launch_b(ik_kernel_b<real, N, 0, G, STEP, NS>(), G, cont_idx, cont_count, 1 + G1, 1, hard_idx, third_count);
                 if (rc == B2K_OK)
-                    rc = c->dh_like ? launch_b(k_ik_restarts<real, N, 1, G3, STEP>, G3, hard_idx, third_count, 1 + G1 + G, 0x7fffffff, nullptr, nullptr)
-                                    : launch_b(k_ik_restarts<real, N, 0, G3, STEP>, G3, hard_idx, third_count, 1 + G1 + G, 0x7fffffff, nullptr, nullptr);
+                    rc = c->dh_like ? launch_b(ik_kernel_b<real, N, 1, G3, STEP, NS>(), G3, hard_idx, third_count, 1 + G1 + G, 0x7fffffff, nullptr, nullptr)
+                                    : launch_b(ik_kernel_b<real, N, 0, G3, STEP, NS>(), G3, hard_idx, third_count, 1 + G1 + G, 0x7fffffff, nullptr, nullptr);
             } else if (rc == B2K_OK)
-                rc = c->dh_like ? launch_b(k_ik_restarts<real, N, 1, G, STEP>, G, cont_idx, cont_count, 1 + G1, 0x7fffffff, nullptr, nullptr)
-                                : launch_b(k_ik_restarts<real, N, 0, G, STEP>, G, cont_idx, cont_count, 1 + G1, 0x7fffffff, nullptr, nullptr);
+                rc = c->dh_like ? launch_b(ik_kernel_b<real, N, 1, G, STEP, NS>(), G, cont_idx, cont_count, 1 + G1, 0x7fffffff, nullptr, nullptr)
+                                : launch_b(ik_kernel_b<real, N, 0, G, STEP, NS>(), G, cont_idx, cont_count, 1 + G1, 0x7fffffff, nullptr, nullptr);
         } else {
-            rc = c->dh_like ? launch_b(k_ik_restarts<real, N, 1, G, STEP>, G, hard_idx, hard_count, 1, 0x7fffffff, nullptr, nullptr)
-                            : launch_b(k_ik_restarts<real, N, 0, G, STEP>, G, hard_idx, hard_count, 1, 0x7fffffff, nullptr, nullptr);
+            rc = c->dh_like ? launch_b(ik_kernel_b<real, N, 1, G, STEP, NS>(), G, hard_idx, hard_count, 1, 0x7fffffff, nullptr, nullptr)
+                            : launch_b(ik_kernel_b<real, N, 0, G, STEP, NS>(), G, hard_idx, hard_count, 1, 0x7fffffff, nullptr, nullptr);
         }
     }
     if (scratch) {
@@ -748,6 +963,34 @@ int ik_launch(const b2k_chain_s *c, const void *Tep, long long nprob, const void
         B2K_CASE(6) B2K_CASE(7) B2K_CASE(8) B2K_CASE(9) B2K_CASE(10)
     default:
         b2k_set_error("ik_lm: unsupported joint count %d", c->n);
+        return B2K_ERR_INVALID;
+    }
+#undef B2K_CASE
+}
+
+// b2k_ikine_null: the Python solver loop with the null-space term, for 7..10 joints (a full-rank J of a chain with n <= 6
+// has an empty null space; the host sends those chains to ik_launch).  STEP as the method asks.
+template <typename real>
+int ik_ns_launch(const b2k_chain_s *c, const void *Tep, long long nprob, const void *q0, int ilimit, int slimit, double tol,
+                 int reject_jl, const double *we, double lambda, int method, unsigned long long seed, int rng_per_row,
+                 void *q_out, int *success, int *iterations, int *searches, void *residual, const IkNullArgs &ns,
+                 cudaStream_t st)
+{
+#define B2K_CASE(NN)                                                                                                   \
+    case NN:                                                                                                           \
+        return pinv ? ik_launch_n<real, NN, 1, true>(c, (const real *)Tep, nprob, (const real *)q0, ilimit, slimit, tol,  \
+                                                     reject_jl, we, lambda, method, seed, B2K_IK_SEM_PYTHON,           \
+                                                     rng_per_row, (real *)q_out, success, iterations, searches,        \
+                                                     (real *)residual, st, &ns)                                        \
+                    : ik_launch_n<real, NN, 0, true>(c, (const real *)Tep, nprob, (const real *)q0, ilimit, slimit, tol,  \
+                                                     reject_jl, we, lambda, method, seed, B2K_IK_SEM_PYTHON,           \
+                                                     rng_per_row, (real *)q_out, success, iterations, searches,        \
+                                                     (real *)residual, st, &ns);
+    const bool pinv = method == B2K_IK_NR || method == B2K_IK_GN;
+    switch (c->n) {
+        B2K_CASE(7) B2K_CASE(8) B2K_CASE(9) B2K_CASE(10)
+    default:
+        b2k_set_error("ikine_null: unsupported joint count %d (7..10)", c->n);
         return B2K_ERR_INVALID;
     }
 #undef B2K_CASE

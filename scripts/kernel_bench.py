@@ -370,3 +370,55 @@ if want("ik_"):
             report(name, ms, M, (16 + 7 + 4) * np.dtype(dt).itemsize,
                    {"solves_per_s": M / (ms * 1e-3), "success": float(s.float().mean()), "mean_it": float(it.float().mean()),
                     "max_it": int(it.max()), "mean_searches": float(sr.float().mean()), "max_searches": int(sr.max())})
+
+# IK with the null-space terms (b2k_ikine_null) against the same loop without them: config 4's targets (Panda, reachable,
+# seed 2), the Python solver loop (ikine_LM: chan k = 1.0, joint limits checked, restarts shared by all rows), gains 1.0,
+# ps = 0, pi = 0.3.  "off" is b2k_ik_lm in the same semantics.  The card's name and power limit are read in the same run.
+if want("ikine_null_"):
+    import subprocess
+
+    try:
+        plim = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True,
+                              text=True, timeout=30).stdout.strip()
+    except Exception as e:  # the figure is context, the timing does not depend on it
+        plim = f"unavailable ({type(e).__name__})"
+    card = {"gpu": torch.cuda.get_device_name(0), "power_limit": plim}
+    panda = rtb.models.Panda().ets()
+    M = args.ik_rows
+    Tep = panda.eval(np.random.default_rng(2).uniform(-np.pi, np.pi, (M, 7)))
+    Lb = rtb._lib.lib()
+    chn = panda._chain
+    stp = torch.cuda.current_stream().cuda_stream
+    pi = np.full(7, 0.3)
+    for dt in (np.float32, np.float64):
+        tag = "f64" if dt == np.float64 else "f32"
+        Td = torch.from_numpy(Tep.astype(dt)).to(dev)
+        codei = rtb._lib.F64 if dt == np.float64 else rtb._lib.F32
+        for var, kq, km in (("off", 0.0, 0.0), ("kq", 1.0, 0.0), ("km", 0.0, 1.0), ("both", 1.0, 1.0)):
+            name = f"ikine_null_panda_{tag}_{var}"
+            if not want(name):
+                continue
+            qo = torch.empty((M, 7), dtype=Td.dtype, device=dev)
+            so, io, ro = (torch.empty(M, dtype=torch.int32, device=dev) for _ in range(3))
+            Eo = torch.empty(M, dtype=Td.dtype, device=dev)
+
+            def run(i):
+                if var == "off":
+                    rc = Lb.b2k_ik_lm(chn, codei, Td.data_ptr(), M, None, 30, 100, 1e-6, 1, None, 1.0, 0, 5 + i,
+                                      rtb._lib.SEM_PYTHON, 0, qo.data_ptr(), so.data_ptr(), io.data_ptr(), ro.data_ptr(),
+                                      Eo.data_ptr(), stp)
+                else:
+                    rc = Lb.b2k_ikine_null(chn, codei, Td.data_ptr(), M, None, 30, 100, 1e-6, 1, None, 1.0, 0, 5 + i, 0,
+                                           kq, km, 0.0, rtb._lib.dptr(pi), qo.data_ptr(), so.data_ptr(), io.data_ptr(),
+                                           ro.data_ptr(), Eo.data_ptr(), stp)
+                rtb._lib.check(rc)
+
+            steps, args.steps = args.steps, 10
+            wu, args.warmup = args.warmup, 2
+            ms = timeit(run, 1 << 30)
+            args.steps, args.warmup = steps, wu
+            report(name, ms, M, (16 + 7 + 4) * np.dtype(dt).itemsize,
+                   dict(card, solves_per_s=M / (ms * 1e-3), success=float(so.float().mean()), mean_it=float(io.float().mean()),
+                        mean_searches=float(ro.float().mean())))
+            del qo, so, io, ro, Eo
+        del Td
