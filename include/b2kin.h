@@ -339,6 +339,7 @@ int b2k_ikine_6s(int dtype, const double *dh, const double *base, const double *
 /* ---------------------------------------------------------------- pure functions of the Jacobian
  * b2k_hessian replaces fknm.ETS_hessian0 / ETS_hessiane (fknm.cpp:583-783 -> _ETS_hessian
  * methods.cpp:16-32): H (N,n,6,n) from J (N,6,n); pass jacob0 for hessian0, jacobe for hessiane.
+ * These and the other functions of J below take n = 1..B2K_MAX_JOINTS; any other n is rejected before any CUDA call.
  * b2k_manipulability is the Yoshikawa measure of ETS.manipulability (ETS.py:1780-1787):
  * m = sqrt|det(Ja Ja^T)| over the Cartesian rows selected by axes_mask (bit k = row k of J;
  * 63 = all, 7 = translational, 56 = rotational); |det Ja| when Ja is square. */

@@ -522,11 +522,7 @@ class ETS:
             raise ValueError("one of q or J must be supplied")
         if J is None:
             J = self.jacob0(q, dtype=dtype)
-        host = not B.is_tensor(J)
-        dt = B.pick_dtype(J, dtype)
-        Jd = B.to_device(J, dt)
-        single = Jd.dim() == 2
-        Jd = (Jd.reshape(1, 6, -1) if single else Jd).contiguous()
+        Jd, dt, host, single = self._jprep(J, dtype)
         N = Jd.shape[0]
         m = B.empty((N,), dt, like=Jd)
         if method == "yoshikawa":

@@ -592,6 +592,7 @@ extern "C" int b2k_hessian(int dtype, int n, const void *J, int64_t N, void *H, 
 {
     if (N < 0 || (N > 0 && (!J || !H))) { b2k_set_error("b2k_hessian: bad arguments"); return B2K_ERR_INVALID; }
     if (dtype != B2K_F32 && dtype != B2K_F64) { b2k_set_error("b2k_hessian: bad dtype"); return B2K_ERR_INVALID; }
+    if (n < 1 || n > B2K_MAX_JOINTS) { b2k_set_error("b2k_hessian: unsupported joint count %d", n); return B2K_ERR_INVALID; }
     if (N == 0) return B2K_OK;
     B2K_ON_DEVICE_OF(J);
     return dtype == B2K_F64 ? extra_launch<double>(0, n, J, N, 0, H, (cudaStream_t)stream)
@@ -602,6 +603,7 @@ extern "C" int b2k_manipulability(int dtype, int n, const void *J, int64_t N, ui
 {
     if (N < 0 || (N > 0 && (!J || !m))) { b2k_set_error("b2k_manipulability: bad arguments"); return B2K_ERR_INVALID; }
     if (dtype != B2K_F32 && dtype != B2K_F64) { b2k_set_error("b2k_manipulability: bad dtype"); return B2K_ERR_INVALID; }
+    if (n < 1 || n > B2K_MAX_JOINTS) { b2k_set_error("b2k_manipulability: unsupported joint count %d", n); return B2K_ERR_INVALID; }
     if ((axes_mask & 63u) == 0) { b2k_set_error("b2k_manipulability: no Cartesian axis selected"); return B2K_ERR_INVALID; }
     if (N == 0) return B2K_OK;
     B2K_ON_DEVICE_OF(J);
@@ -614,6 +616,7 @@ extern "C" int b2k_manipulability_svd(int dtype, int n, const void *J, int64_t N
 {
     if (N < 0 || (N > 0 && (!J || !m))) { b2k_set_error("b2k_manipulability_svd: bad arguments"); return B2K_ERR_INVALID; }
     if (dtype != B2K_F32 && dtype != B2K_F64) { b2k_set_error("b2k_manipulability_svd: bad dtype"); return B2K_ERR_INVALID; }
+    if (n < 1 || n > B2K_MAX_JOINTS) { b2k_set_error("b2k_manipulability_svd: unsupported joint count %d", n); return B2K_ERR_INVALID; }
     if ((axes_mask & 63u) == 0) { b2k_set_error("b2k_manipulability_svd: no Cartesian axis selected"); return B2K_ERR_INVALID; }
     if (kind != 0 && kind != 1) { b2k_set_error("b2k_manipulability_svd: kind must be 0 (minsingular) or 1 (invcondition)"); return B2K_ERR_INVALID; }
     if (N == 0) return B2K_OK;
@@ -626,6 +629,7 @@ extern "C" int b2k_jacob_dot(int dtype, int n, const void *J, const void *qd, in
 {
     if (N < 0 || (N > 0 && (!J || !qd || !Jd))) { b2k_set_error("b2k_jacob_dot: bad arguments"); return B2K_ERR_INVALID; }
     if (dtype != B2K_F32 && dtype != B2K_F64) { b2k_set_error("b2k_jacob_dot: bad dtype"); return B2K_ERR_INVALID; }
+    if (n < 1 || n > B2K_MAX_JOINTS) { b2k_set_error("b2k_jacob_dot: unsupported joint count %d", n); return B2K_ERR_INVALID; }
     if (N == 0) return B2K_OK;
     B2K_ON_DEVICE_OF(J);
     return dtype == B2K_F64 ? extra_launch<double>(2, n, J, N, 0, Jd, (cudaStream_t)stream, qd)
@@ -636,6 +640,7 @@ extern "C" int b2k_jacobm(int dtype, int n, const void *J, int64_t N, uint32_t a
 {
     if (N < 0 || (N > 0 && (!J || !Jm))) { b2k_set_error("b2k_jacobm: bad arguments"); return B2K_ERR_INVALID; }
     if (dtype != B2K_F32 && dtype != B2K_F64) { b2k_set_error("b2k_jacobm: bad dtype"); return B2K_ERR_INVALID; }
+    if (n < 1 || n > B2K_MAX_JOINTS) { b2k_set_error("b2k_jacobm: unsupported joint count %d", n); return B2K_ERR_INVALID; }
     if ((axes_mask & 63u) == 0) { b2k_set_error("b2k_jacobm: no Cartesian axis selected"); return B2K_ERR_INVALID; }
     if (N == 0) return B2K_OK;
     B2K_ON_DEVICE_OF(J);

@@ -1,4 +1,7 @@
 """GPU parity of the rows widened in round 2 (SURVEY 8f): singular-value manipulability measures, ..."""
+import os
+import sys
+
 import numpy as np
 import pytest
 
@@ -9,6 +12,9 @@ torch = pytest.importorskip("torch")
 import b2kin as rtb  # noqa: E402
 from oracle import chains as ch  # noqa: E402
 from oracle import oracle as orc  # noqa: E402
+
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+import jacfun_ref  # noqa: E402
 
 
 def dev(a, dt=np.float64):
@@ -302,19 +308,6 @@ def test_fkine_all_of_a_branched_urdf_robot(single_walk, monkeypatch):
     np.testing.assert_allclose(one, got[0], rtol=1e-12, atol=1e-13)
 
 
-def _hessian_batch(J):
-    """methods.cpp:16-32 over a batch: J (N,6,n) -> H (N,n,6,n); the oracle's loop (oracle.hessian) vectorised over rows."""
-    N, _, n = J.shape
-    H = np.zeros((N, n, 6, n))
-    for a in range(n):
-        for b in range(a, n):
-            H[:, a, :3, b] = np.cross(J[:, 3:, a], J[:, :3, b])
-            H[:, a, 3:, b] = np.cross(J[:, 3:, a], J[:, 3:, b])
-            if b != a:
-                H[:, b, :3, a] = H[:, a, :3, b]
-    return H
-
-
 def test_hessian_every_joint_count_grid_stride_and_alignment():
     """k_hessian (b2k_extra.cu): every instantiated joint count, both dtypes, more rows than one wave of warps (each warp
     walks several rows with its per-thread index table), a ragged last block, and an output pointer that is only
@@ -325,11 +318,11 @@ def test_hessian_every_joint_count_grid_stride_and_alignment():
     rng = np.random.default_rng(77)
     Jc = rng.normal(size=(3, 6, 5))
     for k in range(3):
-        np.testing.assert_allclose(_hessian_batch(Jc)[k], orc.hessian(Jc[k]), rtol=0, atol=1e-15)
+        np.testing.assert_allclose(jacfun_ref.hessian_batch(Jc)[k], orc.hessian(Jc[k]), rtol=0, atol=1e-15)
     for n in range(1, 11):
         N = 9001 if n not in (6, 7) else 150_003
         J = rng.normal(size=(N, 6, n))
-        ref = _hessian_batch(J)
+        ref = jacfun_ref.hessian_batch(J)
         for dt, tol in ((np.float64, dict(rtol=0, atol=1e-14)), (np.float32, dict(rtol=0, atol=2e-6))):
             Jd = dev(J, dt)
             H = torch.full((N * 6 * n * n + 1,), float("nan"), dtype=Jd.dtype, device="cuda")
