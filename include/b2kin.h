@@ -206,6 +206,13 @@ int b2k_rne_create(int n, int mdh, const double *L, b2k_rne_t *out);
 int b2k_rne_destroy(b2k_rne_t rne);
 int b2k_rne(b2k_rne_t rne, int dtype, const void *q, const void *qd, const void *qdd, int64_t N,
             const double *grav, const double *fext, void *tau, void *stream);
+/* b2k_rne_wrench: b2k_rne plus the base wrench of every row (DHRobot.rne(..., base_wrench=True)).  tau is what
+ * b2k_rne writes; wbase (N,6) device = [fx, fy, fz, mx, my, mz], the force and moment the base exerts on link 1,
+ * expressed in frame 0 (the frame of grav), moment about the origin of frame 0.  The actuator terms (Jm, G, B, Tc) act
+ * inside the joints and do not enter it; fext enters as it enters tau.  wbase must be 2*sizeof(real)-byte aligned.
+ * Rejects what b2k_rne rejects plus a NULL (N > 0) or misaligned wbase, before any CUDA call. */
+int b2k_rne_wrench(b2k_rne_t rne, int dtype, const void *q, const void *qd, const void *qdd, int64_t N,
+                   const double *grav, const double *fext, void *tau, void *wbase, void *stream);
 
 /* Robot-specialised kernels.  For all-revolute arms b2k_rne (and the dynamics entry points below) run a kernel that is
  * generated for THIS robot's link table and compiled for sm_90a at first use (NVRTC): terms whose link parameter is zero
@@ -213,7 +220,8 @@ int b2k_rne(b2k_rne_t rne, int dtype, const void *q, const void *qd, const void 
  * b2k_rne_spec.cu).  Results equal the generic kernel's to rounding.  Environment: B2K_RNE_SPEC=0 disables it, =2 makes a
  * failure to specialise an error; B2K_NVRTC_PATH names libnvrtc.so.12 when it is not on the loader path.
  *   b2k_rne_spec_info  writes a one-line description of the kernel that serves (mode, dtype, grav pattern, has_fext) for
- *                      this robot into buf -- mode: 0 rne, 1 inertia, 2 gravload, 3 itorque, 4 coriolis, 5 accel.
+ *                      this robot into buf -- mode: 0 rne, 1 inertia, 2 gravload, 3 itorque, 4 coriolis, 5 accel,
+ *                      6 rne with the base wrench (b2k_rne_wrench; codegen: n + 6 outputs, tau then wbase).
  *   b2k_rne_codegen    returns the generated row function (plain C in terms of `real`; also valid host C++) and its
  *                      constant bank, so the generator can be checked against the oracle without a GPU;
  *                      counts[3] = multiplications, fused multiply-adds, additions per row. */
@@ -427,6 +435,10 @@ int b2k_fkine_host(b2k_chain_t chain, int dtype, const void *q_host, int64_t N, 
 int b2k_rne_host(b2k_rne_t rne, int dtype, const void *q_host, const void *qd_host,
                  const void *qdd_host, int64_t N, const double *grav, const double *fext,
                  void *tau_host, int device);
+/* the host-buffer form of b2k_rne_wrench: tau_host (N,n) and wbase_host (N,6) */
+int b2k_rne_wrench_host(b2k_rne_t rne, int dtype, const void *q_host, const void *qd_host,
+                        const void *qdd_host, int64_t N, const double *grav, const double *fext,
+                        void *tau_host, void *wbase_host, int device);
 
 /* number of kernel launches this library has issued in the calling process (all threads);
  * bench.py reports the delta over its timed region as "gpu_launches". */

@@ -347,9 +347,11 @@ class DHRobot:
 
     def rne(self, q, qd=None, qdd=None, gravity=None, fext=None, base_wrench=False, dtype=None):
         """Inverse dynamics tau = RNE(q, qd, qdd): (n,) for one state, (N,n) for a trajectory
-        (reference DHRobot.rne 1373-1456 -> frne.frne per row)."""
-        if base_wrench:
-            raise NotImplementedError("base_wrench uses the reference's pure-Python rne_python; outside the accelerated path")
+        (reference DHRobot.rne 1373-1456 -> frne.frne per row).
+
+        ``base_wrench=True`` returns ``(tau, wbase)``: tau as above and wbase (6,) / (N,6) = [fx, fy, fz, mx, my, mz],
+        the wrench the base exerts on link 1, expressed in frame 0 (the chain's base frame, after ``robot.base``) with
+        the moment about its origin.  Both come from the same recursion (one kernel launch)."""
         if self._rne_ob is None or self._dynchanged:  # @_check_rne, DHLink.py:24-51
             self.delete_rne()
             self._init_rne()
@@ -383,13 +385,26 @@ class DHRobot:
             t = B.require_cuda()
             qh, qdh, qddh = (np.ascontiguousarray(x, dtype=dt) for x in (q2, qd2, qdd2))
             tau = _lib.host_result((N, n), dt)
-            _lib.check(L.b2k_rne_host(self._rne_ob, B.code(dt), qh.ctypes.data, qdh.ctypes.data, qddh.ctypes.data, N,
-                                      _lib.dptr(ng), _lib.dptr(fx), tau.ctypes.data, t.cuda.current_device()))
+            if base_wrench:
+                wb = _lib.host_result((N, 6), dt)
+                _lib.check(L.b2k_rne_wrench_host(self._rne_ob, B.code(dt), qh.ctypes.data, qdh.ctypes.data, qddh.ctypes.data, N,
+                                                 _lib.dptr(ng), _lib.dptr(fx), tau.ctypes.data, wb.ctypes.data,
+                                                 t.cuda.current_device()))
+            else:
+                _lib.check(L.b2k_rne_host(self._rne_ob, B.code(dt), qh.ctypes.data, qdh.ctypes.data, qddh.ctypes.data, N,
+                                          _lib.dptr(ng), _lib.dptr(fx), tau.ctypes.data, t.cuda.current_device()))
         else:
             qt, qdt, qddt = (B.to_device(x, dt) for x in (q2, qd2, qdd2))
             tau = B.empty((N, n), dt, like=qt)
-            _lib.check(L.b2k_rne(self._rne_ob, B.code(dt), B.ptr(qt), B.ptr(qdt), B.ptr(qddt), N, _lib.dptr(ng),
-                                 _lib.dptr(fx), B.ptr(tau), B.stream_ptr(qt)))
+            if base_wrench:
+                wb = B.empty((N, 6), dt, like=qt)
+                _lib.check(L.b2k_rne_wrench(self._rne_ob, B.code(dt), B.ptr(qt), B.ptr(qdt), B.ptr(qddt), N, _lib.dptr(ng),
+                                            _lib.dptr(fx), B.ptr(tau), B.ptr(wb), B.stream_ptr(qt)))
+            else:
+                _lib.check(L.b2k_rne(self._rne_ob, B.code(dt), B.ptr(qt), B.ptr(qdt), B.ptr(qddt), N, _lib.dptr(ng),
+                                     _lib.dptr(fx), B.ptr(tau), B.stream_ptr(qt)))
+        if base_wrench:
+            return (tau[0], wb[0]) if single else (tau, wb)
         return tau[0] if single else tau
 
     def nofriction(self, coulomb: bool = True, viscous: bool = False) -> "DHRobot":
@@ -442,7 +457,7 @@ class DHRobot:
         return _fdyn(self, _lib.lib().b2k_rne_fdyn if not callable(Q) else None, self._rne_ob, kernel_gravity, T, q0, Q=Q, Q_args=Q_args,
                      qd0=qd0, solver=solver, solver_args=solver_args, dt=dt, gravity=gravity, max_steps=max_steps, dtype=dtype)
 
-    _RNE_MODES = {"rne": 0, "inertia": 1, "gravload": 2, "itorque": 3, "coriolis": 4, "accel": 5}
+    _RNE_MODES = {"rne": 0, "inertia": 1, "gravload": 2, "itorque": 3, "coriolis": 4, "accel": 5, "rne_wrench": 6}
 
     def rne_kernel_info(self, op="rne", dtype=np.float64, gravity=None, fext=None) -> str:
         """Which kernel serves `op` for this robot: the robot-specialised one (generated from the link table and

@@ -50,6 +50,7 @@ _PROTOS = {
     "b2k_rne_create": (C.c_int, [C.c_int, C.c_int, dp, C.POINTER(vp)]),
     "b2k_rne_destroy": (C.c_int, [vp]),
     "b2k_rne": (C.c_int, [vp, C.c_int, vp, vp, vp, i64, dp, dp, vp, vp]),
+    "b2k_rne_wrench": (C.c_int, [vp, C.c_int, vp, vp, vp, i64, dp, dp, vp, vp, vp]),
     "b2k_rne_codegen": (C.c_int, [vp, C.c_int, C.c_int, C.c_int, C.c_char_p, i64, dp, C.c_int32, ip, ip]),
     "b2k_rne_spec_info": (C.c_int, [vp, C.c_int, C.c_int, dp, C.c_int, C.c_char_p, i64]),
     "b2k_rne_fdyn": (C.c_int, [vp, C.c_int, vp, vp, i64, C.c_double, dp, C.c_int, dp, vp, dp, dp, dp, C.c_double, C.c_double,
@@ -88,6 +89,7 @@ _PROTOS = {
     "b2k_fkine_jacob0_host": (C.c_int, [vp, C.c_int, vp, i64, i64, dp, dp, vp, vp, C.c_int]),
     "b2k_fkine_host": (C.c_int, [vp, C.c_int, vp, i64, i64, dp, dp, vp, C.c_int]),
     "b2k_rne_host": (C.c_int, [vp, C.c_int, vp, vp, vp, i64, dp, dp, vp, C.c_int]),
+    "b2k_rne_wrench_host": (C.c_int, [vp, C.c_int, vp, vp, vp, i64, dp, dp, vp, vp, C.c_int]),
     "b2k_launch_count": (C.c_int64, []),
     "b2k_set_variant": (C.c_int, [C.c_int]),
     "b2k_selftest_sincos": (C.c_int, [C.c_int, vp, i64, vp, vp, vp]),

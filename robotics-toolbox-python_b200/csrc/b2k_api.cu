@@ -22,6 +22,8 @@ int b2k_fkw_launch(const b2k_chain_s *, int dtype, int mode, const void *, long 
                    const double *, void *, void *, cudaStream_t);
 int b2k_rne_launch(const b2k_rne_s *, int dtype, const void *, const void *, const void *, long long, const double *,
                    const double *, void *, cudaStream_t);
+int b2k_rne_wrench_launch(const b2k_rne_s *, int dtype, const void *, const void *, const void *, long long, const double *,
+                          const double *, void *, void *, cudaStream_t);
 
 enum { FKJ_T = 1, FKJ_J0 = 2, FKJ_JE = 4 };
 
@@ -201,10 +203,10 @@ extern "C" int b2k_fkine_jacobe(b2k_chain_t c, int dtype, const void *q, int64_t
     return fkj_dispatch("b2k_fkine_jacobe", c, dtype, FKJ_T | FKJ_JE, q, N, ldq, base, tool, T, J, stream);
 }
 
-extern "C" int b2k_rne(b2k_rne_t r, int dtype, const void *q, const void *qd, const void *qdd, int64_t N,
-                       const double *grav, const double *fext, void *tau, void *stream)
+// b2k_rne and b2k_rne_wrench (wrench: also the base wrench, wbase (N, 6)); every argument is checked before any CUDA call
+static int rne_run(const char *fn, b2k_rne_t r, int dtype, const void *q, const void *qd, const void *qdd, int64_t N,
+                   const double *grav, const double *fext, void *tau, bool wrench, void *wbase, void *stream)
 {
-    const char *fn = "b2k_rne";
     if (!r) { b2k_set_error("%s: rne handle is NULL", fn); return B2K_ERR_INVALID; }
     if (dtype != B2K_F32 && dtype != B2K_F64) { b2k_set_error("%s: dtype must be B2K_F32 or B2K_F64", fn); return B2K_ERR_INVALID; }
     if (N < 0) { b2k_set_error("%s: N is negative", fn); return B2K_ERR_INVALID; }
@@ -214,15 +216,33 @@ extern "C" int b2k_rne(b2k_rne_t r, int dtype, const void *q, const void *qd, co
     if ((rc = check_out(fn, "q", q, N, es)) || (rc = check_out(fn, "qd", qd, N, es)) || (rc = check_out(fn, "qdd", qdd, N, es)) ||
         (rc = check_out(fn, "tau", tau, N, es)))
         return rc;
+    // a row of wbase is 3 pairs of reals: the kernels store it in 2-element units
+    if (wrench && (rc = check_out(fn, "wbase", wbase, N, 2 * es))) return rc;
     if (N == 0) return B2K_OK;
     B2K_ON_DEVICE_OF(q);
     // the robot-specialised kernel (b2k_rne_spec.cu) serves the full 32-row tiles, the generic one the ragged tail
-    const long long done = b2k_rne_spec_launch(r, 0 /* B2K_GEN_RNE */, dtype, q, qd, qdd, N, grav, fext, tau, (cudaStream_t)stream);
+    const long long done = b2k_rne_spec_launch(r, wrench ? 6 /* B2K_GEN_RNE_WRENCH */ : 0 /* B2K_GEN_RNE */, dtype, q, qd, qdd, N, grav,
+                                               fext, tau, wrench ? wbase : nullptr, (cudaStream_t)stream);
     if (done < 0) return (int)done;
     if (done == N) return B2K_OK;
     const size_t off = (size_t)done * r->n * es;
+    if (wrench)
+        return b2k_rne_wrench_launch(r, dtype, (const char *)q + off, (const char *)qd + off, (const char *)qdd + off, N - done, grav,
+                                     fext, (char *)tau + off, (char *)wbase + (size_t)done * 6 * es, (cudaStream_t)stream);
     return b2k_rne_launch(r, dtype, (const char *)q + off, (const char *)qd + off, (const char *)qdd + off, N - done, grav, fext,
                           (char *)tau + off, (cudaStream_t)stream);
+}
+
+extern "C" int b2k_rne(b2k_rne_t r, int dtype, const void *q, const void *qd, const void *qdd, int64_t N,
+                       const double *grav, const double *fext, void *tau, void *stream)
+{
+    return rne_run("b2k_rne", r, dtype, q, qd, qdd, N, grav, fext, tau, false, nullptr, stream);
+}
+
+extern "C" int b2k_rne_wrench(b2k_rne_t r, int dtype, const void *q, const void *qd, const void *qdd, int64_t N,
+                              const double *grav, const double *fext, void *tau, void *wbase, void *stream)
+{
+    return rne_run("b2k_rne_wrench", r, dtype, q, qd, qdd, N, grav, fext, tau, true, wbase, stream);
 }
 
 // ------------------------------------------------------------------ host-buffer front ends
@@ -435,6 +455,26 @@ extern "C" int b2k_rne_host(b2k_rne_t r, int dtype, const void *q, const void *q
     });
 }
 
+extern "C" int b2k_rne_wrench_host(b2k_rne_t r, int dtype, const void *q, const void *qd, const void *qdd, int64_t N,
+                                   const double *grav, const double *fext, void *tau, void *wbase, int device)
+{
+    const char *fn = "b2k_rne_wrench_host";
+    if (!r) { b2k_set_error("%s: rne handle is NULL", fn); return B2K_ERR_INVALID; }
+    if (dtype != B2K_F32 && dtype != B2K_F64) { b2k_set_error("%s: bad dtype", fn); return B2K_ERR_INVALID; }
+    if (N < 0 || (N > 0 && (!q || !qd || !qdd || !tau || !grav))) { b2k_set_error("%s: NULL argument", fn); return B2K_ERR_INVALID; }
+    const size_t es = dtype == B2K_F64 ? 8 : 4;
+    int rc;
+    if ((rc = check_out(fn, "wbase", wbase, N, (unsigned)es))) return rc;
+    if (N == 0) return B2K_OK;
+    const void *h_in[3] = {q, qd, qdd};
+    size_t in_b[3] = {r->n * es, r->n * es, r->n * es};
+    void *h_out[2] = {tau, wbase};
+    size_t out_b[2] = {r->n * es, 6 * es};
+    return run_pipeline(device, N, 3, h_in, in_b, 2, h_out, out_b, [&](Slot &s, long long rows) {
+        return b2k_rne_wrench(r, dtype, s.d_in[0], s.d_in[1], s.d_in[2], rows, grav, fext, s.d_out[0], s.d_out[1], s.st);
+    });
+}
+
 // ------------------------------------------------------------------ inverse kinematics
 int b2k_ik_launch_f32(const b2k_chain_s *, const void *, long long, const void *, int, int, double, int, const double *,
                       double, int, unsigned long long, int, int, void *, int *, int *, int *, void *, cudaStream_t);
@@ -555,7 +595,7 @@ static int fan_dispatch(const char *fn, b2k_rne_t r, int dtype, int mode, const 
     if (N == 0) return B2K_OK;
     B2K_ON_DEVICE_OF(in0);
     cudaStream_t st = (cudaStream_t)stream;
-    const long long done = b2k_rne_spec_launch(r, mode + 1 /* FAN_* -> B2K_GEN_* */, dtype, in0, in1, in2, N, grav, nullptr, out, st);
+    const long long done = b2k_rne_spec_launch(r, mode + 1 /* FAN_* -> B2K_GEN_* */, dtype, in0, in1, in2, N, grav, nullptr, out, nullptr, st);
     if (done < 0) return (int)done;
     if (done == N) return B2K_OK;
     const size_t off = (size_t)done * r->n * es;

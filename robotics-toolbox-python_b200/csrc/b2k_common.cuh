@@ -114,9 +114,9 @@ struct b2k_rne_s {
 void b2k_rne_spec_attach(b2k_rne_s *r);
 void b2k_rne_spec_detach(b2k_rne_s *r);
 // mode = B2K_GEN_* (b2k_rne_gen.h); returns the rows served by the specialised kernel (a multiple of 32, possibly 0)
-// or a negative b2k_status
+// or a negative b2k_status.  out2: the base wrench (nrows, 6) of B2K_GEN_RNE_WRENCH, NULL for every other mode.
 long long b2k_rne_spec_launch(const b2k_rne_s *r, int mode, int dtype, const void *in0, const void *in1, const void *in2,
-                              long long nrows, const double *grav, const double *fext, void *out, cudaStream_t st);
+                              long long nrows, const double *grav, const double *fext, void *out, void *out2, cudaStream_t st);
 
 // ---- error plumbing (b2k_api.cu)
 void b2k_set_error(const char *fmt, ...);

@@ -153,9 +153,20 @@ __device__ __forceinline__ void rne_sincos(const RneP<real, N> &P, const real *m
     }
 }
 
-template <typename real, int N, bool MDH>
+// The base wrench (WRENCH): the force and moment the base exerts on link 1, in frame 0, the moment about the origin of
+// frame 0: wb = [R_1 f_1, R_1 n_1] for DH (n_1 is already about O_0), [R_1 f_1, R_1 n_1 + p*_1 x R_1 f_1] for MDH
+// (n_1 is about O_1: one more step of the backward recursion, onto a massless link 0).  The actuator terms act inside
+// the joints and do not enter it.
+template <typename real>
+__device__ __forceinline__ void rne_put_wrench(V3<real> f0, V3<real> n0, real *wb)
+{
+    wb[0] = f0.x; wb[1] = f0.y; wb[2] = f0.z;
+    wb[3] = n0.x; wb[4] = n0.y; wb[5] = n0.z;
+}
+
+template <typename real, int N, bool MDH, bool WRENCH = false>
 __device__ __forceinline__ void rne_row_allrev(const RneP<real, N> &P, const real *sth, const real *cth, const real *mqd,
-                                               const real *mqdd, V3<real> gravity, real *tq)
+                                               const real *mqdd, V3<real> gravity, real *tq, real *wb = nullptr)
 {
     V3<real> Fm[N], Nm[N];
     V3<real> w = {0, 0, 0}, wd = {0, 0, 0}, acc = {0, 0, 0};
@@ -238,14 +249,21 @@ __device__ __forceinline__ void rne_row_allrev(const RneP<real, N> &P, const rea
         t += (qdj > 0 ? P.c_tcp[j] : (real)0) + (qdj < 0 ? P.c_tcm[j] : (real)0);
         tq[j] = t;
     }
+    if constexpr (WRENCH) {
+        const FRot<real, MDH> R = {sth[0], cth[0], P.sa[0], P.ca[0]};
+        const V3<real> f0 = R.mul(f);
+        const V3<real> ps = {P.ps[0][0], P.ps[0][1], P.ps[0][2]};
+        rne_put_wrench(f0, MDH ? R.mul_acc(nn, vcross(ps, f0)) : R.mul(nn), wb);
+    }
 }
 
 // ------------------------------------------------------------------ generic row (any mix of revolute / prismatic links)
 // Mirrors ne.c operation by operation, including its quirks for a prismatic first joint under
 // modified DH (ne.c:187-204).
-template <typename real, int N, bool MDH>
+template <typename real, int N, bool MDH, bool WRENCH = false>
 __device__ __forceinline__ void rne_row_generic(const RneP<real, N> &P, const real *mq, const real *sth, const real *cth,
-                                                const real *mqd, const real *mqdd, V3<real> gravity, real *tq)
+                                                const real *mqd, const real *mqdd, V3<real> gravity, real *tq,
+                                                real *wb = nullptr)
 {
     // stash for the backward recursion
     V3<real> Fm[N], Nm[N];
@@ -416,17 +434,27 @@ __device__ __forceinline__ void rne_row_generic(const RneP<real, N> &P, const re
         t += (qdj > 0 ? P.c_tcp[j] : (real)0) + (qdj < 0 ? P.c_tcm[j] : (real)0);
         tq[j] = t;
     }
+    if constexpr (WRENCH) { // the MDH prismatic-first-joint quirk above carries over: wb is what that recursion gives
+        const LinkRot<real, MDH> R(sth[0], cth[0], P.sa[0], P.ca[0]);
+        const V3<real> f0 = R.mul(f);
+        V3<real> n0 = R.mul(nn);
+        if (MDH) {
+            const real d = P.prismatic[0] ? (mq[0] + P.offset[0]) : P.D[0];
+            n0 = vadd(n0, vcross(V3<real>{P.A[0], -d * P.sa[0], d * P.ca[0]}, f0));
+        }
+        rne_put_wrench(f0, n0, wb);
+    }
     // ---------------- stage tau and write it back coalesced
 
 }
 
 // ALLREV: every joint is revolute (the usual case) -- strips the prismatic code, which the compiler
-// would otherwise if-convert into always-executed select chains.
-template <typename real, int N, bool MDH, bool ALLREV>
-__global__ void __launch_bounds__(B2K_THREADS, (sizeof(real) == 4 || (ALLREV && N <= 6)) ? 4 : 3)
-k_rne(const __grid_constant__ RneP<real, N> P, const real *__restrict__ q, const real *__restrict__ qd,
-      const real *__restrict__ qdd, long long nrows, real *__restrict__ tau, int warp_smem_bytes, int in_bytes,
-      int qmode)
+// would otherwise if-convert into always-executed select chains.  WRENCH: also the base wrench of every row, staged
+// behind tau in shared memory and written to its own (nrows, 6) array.
+template <typename real, int N, bool MDH, bool ALLREV, bool WRENCH>
+__device__ __forceinline__ void rne_tiles(const RneP<real, N> &P, const real *__restrict__ q, const real *__restrict__ qd,
+                                          const real *__restrict__ qdd, long long nrows, real *__restrict__ tau,
+                                          real *__restrict__ wbase_out, int warp_smem_bytes, int in_bytes, int qmode)
 {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int lane = threadIdx.x & 31;
@@ -458,20 +486,40 @@ k_rne(const __grid_constant__ RneP<real, N> P, const real *__restrict__ q, const
         const int myrow = (lane < rows_here ? lane : 0) * lds;
         const real *mq = sq + myrow, *mqd = sqd + myrow, *mqdd = sqdd + myrow;
 
-        real tq[N], sth[N], cth[N];
+        real tq[N], sth[N], cth[N], wb[6];
         rne_sincos<real, N, ALLREV>(P, mq, sth, cth);
         const V3<real> grav = {P.grav[0], P.grav[1], P.grav[2]};
-        if constexpr (ALLREV) rne_row_allrev<real, N, MDH>(P, sth, cth, mqd, mqdd, grav, tq);
-        else rne_row_generic<real, N, MDH>(P, mq, sth, cth, mqd, mqdd, grav, tq);
+        if constexpr (ALLREV) rne_row_allrev<real, N, MDH, WRENCH>(P, sth, cth, mqd, mqdd, grav, tq, wb);
+        else rne_row_generic<real, N, MDH, WRENCH>(P, mq, sth, cth, mqd, mqdd, grav, tq, wb);
         // the inputs of this tile are dead (tq holds the results): prefetch the next tile behind the drain
         __syncwarp();
         if (tile + tstride < ntiles) load_inputs(tile + tstride);
         TileStage<real, N>::put_row(sout, lane, tq);
+        if constexpr (WRENCH) TileStage<real, 6>::put_row(sout + TileStage<real, N>::BYTES, lane, wb);
         __syncwarp();
         TileStage<real, N>::drain(sout, tau + row0 * N, rows_here, lane);
+        if constexpr (WRENCH) TileStage<real, 6>::drain(sout + TileStage<real, N>::BYTES, wbase_out + row0 * 6, rows_here, lane);
         __syncwarp();
     }
     cp_async_wait_all();
+}
+
+template <typename real, int N, bool MDH, bool ALLREV>
+__global__ void __launch_bounds__(B2K_THREADS, (sizeof(real) == 4 || (ALLREV && N <= 6)) ? 4 : 3)
+k_rne(const __grid_constant__ RneP<real, N> P, const real *__restrict__ q, const real *__restrict__ qd,
+      const real *__restrict__ qdd, long long nrows, real *__restrict__ tau, int warp_smem_bytes, int in_bytes,
+      int qmode)
+{
+    rne_tiles<real, N, MDH, ALLREV, false>(P, q, qd, qdd, nrows, tau, nullptr, warp_smem_bytes, in_bytes, qmode);
+}
+
+template <typename real, int N, bool MDH, bool ALLREV>
+__global__ void __launch_bounds__(B2K_THREADS, (sizeof(real) == 4 || (ALLREV && N <= 6)) ? 4 : 3)
+k_rne_wrench(const __grid_constant__ RneP<real, N> P, const real *__restrict__ q, const real *__restrict__ qd,
+             const real *__restrict__ qdd, long long nrows, real *__restrict__ tau, real *__restrict__ wbase,
+             int warp_smem_bytes, int in_bytes, int qmode)
+{
+    rne_tiles<real, N, MDH, ALLREV, true>(P, q, qd, qdd, nrows, tau, wbase, warp_smem_bytes, in_bytes, qmode);
 }
 
 // ------------------------------------------------------------------ dynamics fan-outs of the recursion (SURVEY 8f-1)
@@ -681,17 +729,25 @@ void rne_fill_params(const b2k_rne_s *r, const double *grav, const double *fext,
     b2k_fill_trig<real>(P.trig);
 }
 
-template <typename real, int N>
+template <typename real, int N, bool MDH, bool ALLREV, bool WRENCH>
+constexpr auto rne_kernel()
+{
+    if constexpr (WRENCH) return k_rne_wrench<real, N, MDH, ALLREV>;
+    else return k_rne<real, N, MDH, ALLREV>;
+}
+
+template <typename real, int N, bool WRENCH>
 int rne_launch_n(const b2k_rne_s *r, const real *q, const real *qd, const real *qdd, long long nrows,
-                 const double *grav, const double *fext, real *tau, cudaStream_t st)
+                 const double *grav, const double *fext, real *tau, real *wbase, cudaStream_t st)
 {
     RneP<real, N> P;
     rne_fill_params<real, N>(r, grav, fext, P);
     const size_t inb = fkj_q_bytes<real>(N);
-    const size_t wsm = (3 * inb + (size_t)TileStage<real, N>::BYTES + 15) & ~(size_t)15;
+    const size_t wsm = (3 * inb + (size_t)TileStage<real, N>::BYTES + (WRENCH ? (size_t)TileStage<real, 6>::BYTES : 0) + 15) & ~(size_t)15;
     const size_t smem = wsm * B2K_WARPS_PER_BLOCK;
     const int qmode = (fkj_qmode<real>(q, N) && fkj_qmode<real>(qd, N) && fkj_qmode<real>(qdd, N)) ? 1 : 0;
     if (((uintptr_t)tau) % TileStage<real, N>::UB) { b2k_set_error("rne: tau must be %d-byte aligned", TileStage<real, N>::UB); return B2K_ERR_INVALID; }
+    if (WRENCH && ((uintptr_t)wbase) % TileStage<real, 6>::UB) { b2k_set_error("rne: wbase must be %d-byte aligned", TileStage<real, 6>::UB); return B2K_ERR_INVALID; }
     const long long ntiles = (nrows + 31) / 32;
     const long long nblk_needed = (ntiles + B2K_WARPS_PER_BLOCK - 1) / B2K_WARPS_PER_BLOCK;
     auto launch = [&](auto kern) -> int {
@@ -703,23 +759,25 @@ int rne_launch_n(const b2k_rne_s *r, const real *q, const real *qd, const real *
             if (grid > nblk_needed) grid = nblk_needed;
         }
         if (grid < 1) grid = 1;
-        kern<<<(unsigned)grid, B2K_THREADS, smem, st>>>(P, q, qd, qdd, nrows, tau, (int)wsm, (int)inb, qmode);
+        if constexpr (WRENCH) kern<<<(unsigned)grid, B2K_THREADS, smem, st>>>(P, q, qd, qdd, nrows, tau, wbase, (int)wsm, (int)inb, qmode);
+        else kern<<<(unsigned)grid, B2K_THREADS, smem, st>>>(P, q, qd, qdd, nrows, tau, (int)wsm, (int)inb, qmode);
         b2k_count_launch();
         B2K_CUDA(cudaGetLastError());
         return B2K_OK;
     };
     bool allrev = true;
     for (int j = 0; j < N; j++) allrev = allrev && !P.prismatic[j];
-    if (r->mdh) return allrev ? launch(k_rne<real, N, true, true>) : launch(k_rne<real, N, true, false>);
-    return allrev ? launch(k_rne<real, N, false, true>) : launch(k_rne<real, N, false, false>);
+    if (r->mdh) return allrev ? launch(rne_kernel<real, N, true, true, WRENCH>()) : launch(rne_kernel<real, N, true, false, WRENCH>());
+    return allrev ? launch(rne_kernel<real, N, false, true, WRENCH>()) : launch(rne_kernel<real, N, false, false, WRENCH>());
 }
 
-template <typename real>
+// WRENCH: k_rne_wrench (tau and the base wrench wbase (nrows, 6)); otherwise k_rne and wbase is unused
+template <typename real, bool WRENCH>
 int rne_launch(const b2k_rne_s *r, const void *q, const void *qd, const void *qdd, long long nrows, const double *grav,
-               const double *fext, void *tau, cudaStream_t st)
+               const double *fext, void *tau, void *wbase, cudaStream_t st)
 {
 #define B2K_CASE(NN) \
-    case NN: return rne_launch_n<real, NN>(r, (const real *)q, (const real *)qd, (const real *)qdd, nrows, grav, fext, (real *)tau, st);
+    case NN: return rne_launch_n<real, NN, WRENCH>(r, (const real *)q, (const real *)qd, (const real *)qdd, nrows, grav, fext, (real *)tau, (real *)wbase, st);
     switch (r->n) {
         B2K_CASE(1) B2K_CASE(2) B2K_CASE(3) B2K_CASE(4) B2K_CASE(5)
         B2K_CASE(6) B2K_CASE(7) B2K_CASE(8) B2K_CASE(9) B2K_CASE(10)

@@ -254,6 +254,7 @@ struct Inputs { // one evaluation of the recursion: per-joint velocity / acceler
     std::vector<Sym> qd, qdd;
     V3 grav, ftip, ntip;
     bool friction = true;
+    bool wrench = false; // also return the base wrench (6 symbols after the n torques)
 };
 
 // One Luh-Walker-Paul recursion over symbolic inputs; returns the joint torques as symbols.
@@ -396,6 +397,17 @@ std::vector<Sym> recursion(Gen &g, const std::vector<Link> &L, bool mdh, const I
         }
         tau[j] = tq;
     }
+    if (in.wrench) { // what the base exerts on link 1, in frame 0: R_1 f_1, R_1 n_1 (+ p*_1 x R_1 f_1 for MDH); b2k_rne.cuh
+        const V3 f0 = v.fix(R(L[0], f));
+        V3 n0;
+        if (mdh) {
+            const V3 pxf = v.cross_acc(L[0].ps, f0);
+            n0 = R(L[0], nn, &pxf);
+        } else {
+            n0 = R(L[0], nn);
+        }
+        for (const Sym &s : {f0.x, f0.y, f0.z, n0.x, n0.y, n0.z}) tau.push_back(s);
+    }
     return tau;
 }
 
@@ -427,7 +439,7 @@ int assemble(Gen &g, int N, const b2k_gen_opts &o, const RecFn &rec, std::vector
     Vops vo(g);
     Inputs in;
     in.grav = vo.zero(); in.ftip = vo.zero(); in.ntip = vo.zero();
-    if (o.mode == B2K_GEN_RNE) {
+    if (o.mode == B2K_GEN_RNE || o.mode == B2K_GEN_RNE_WRENCH) { // RNE_WRENCH: out = [tau (n) | base wrench (6)]
         sig = "rne_row(const real *C, const real *grav, const real *fext, const real *st, const real *ct, const real *qq, "
               "const real *qd, const real *qdd, real *out)";
         in.qd = jvec("qd"); in.qdd = jvec("qdd");
@@ -436,8 +448,9 @@ int assemble(Gen &g, int N, const b2k_gen_opts &o, const RecFn &rec, std::vector
             in.ftip = {g.var("fext[0]"), g.var("fext[1]"), g.var("fext[2]")};
             in.ntip = {g.var("fext[3]"), g.var("fext[4]"), g.var("fext[5]")};
         }
+        in.wrench = o.mode == B2K_GEN_RNE_WRENCH;
         std::vector<Sym> tau = rec(in);
-        for (int j = 0; j < N; j++) tail.push_back(assign(g, "out[" + std::to_string(j) + "]", tau[j]));
+        for (int j = 0; j < (int)tau.size(); j++) tail.push_back(assign(g, "out[" + std::to_string(j) + "]", tau[j]));
     } else if (o.mode == B2K_GEN_GRAVLOAD) { // rne(q, 0, 0, g)  Dynamics.py:912-915
         sig = "rne_row(const real *C, const real *grav, const real *fext, const real *st, const real *ct, const real *qq, "
               "const real *in1, const real *in2, real *out)";
@@ -615,6 +628,7 @@ struct TreeOps {
 
 int b2k_tree_generate(const b2k_tree_s *t, const b2k_gen_opts &o, b2k_gen_out &out)
 {
+    if (o.mode == B2K_GEN_RNE_WRENCH) { out.error = "the base wrench is not available for rigid-body trees"; return -1; }
     const int N = t->n;
     Gen g;
     TreeOps T(g);

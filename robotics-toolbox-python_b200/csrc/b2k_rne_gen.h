@@ -6,7 +6,8 @@
 
 #include "b2k_common.cuh"
 
-enum { B2K_GEN_RNE = 0, B2K_GEN_INERTIA = 1, B2K_GEN_GRAVLOAD = 2, B2K_GEN_ITORQUE = 3, B2K_GEN_CORIOLIS = 4, B2K_GEN_ACCEL = 5 };
+enum { B2K_GEN_RNE = 0, B2K_GEN_INERTIA = 1, B2K_GEN_GRAVLOAD = 2, B2K_GEN_ITORQUE = 3, B2K_GEN_CORIOLIS = 4, B2K_GEN_ACCEL = 5,
+       B2K_GEN_RNE_WRENCH = 6 };
 
 struct b2k_gen_opts {
     int mode = B2K_GEN_RNE;
@@ -36,5 +37,6 @@ struct b2k_tree_s {
 int b2k_tree_generate(const b2k_tree_s *t, const b2k_gen_opts &o, b2k_gen_out &out);
 
 // outputs of the generated function: RNE / GRAVLOAD / ITORQUE n values; INERTIA / CORIOLIS n*n; ACCEL n*n + n
-// (rows of M followed by torque - rne(q, qd, 0), the wrapper solves the system)
+// (rows of M followed by torque - rne(q, qd, 0), the wrapper solves the system); RNE_WRENCH n + 6 (tau, then the wrench
+// [f; m] the base exerts on link 1, in frame 0, moment about its origin).  Trees (b2k_tree_generate) reject RNE_WRENCH.
 int b2k_rne_generate(const b2k_rne_s *r, const b2k_gen_opts &o, b2k_gen_out &out);

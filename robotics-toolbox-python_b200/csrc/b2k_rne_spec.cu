@@ -31,7 +31,8 @@ namespace {
 // ------------------------------------------------------------------ the fixed part of the kernel source
 // Macros supplied on the NVRTC command line: REAL, NJ (joints), NC (constant-bank entries), MODE
 // (B2K_GEN_*), NIN (input arrays), NOUT (reals written per row), NRES (reals the row function returns),
-// PADIN (1: padded input rows, element-wise tile load), MINB (resident blocks per SM to aim for).
+// PADIN (1: padded input rows, element-wise tile load), MINB (resident blocks per SM to aim for); NOUT2 (only for
+// B2K_GEN_RNE_WRENCH: reals per row of a second output array, res[NOUT..NOUT+NOUT2), staged and copied on its own).
 const char *kPrologue = R"B2KSRC(
 typedef REAL real;
 typedef unsigned long long u64;
@@ -128,8 +129,11 @@ const char *kKernel = R"B2KSRC(
 #define LDI (PADIN ? (NJ | 1) : NJ)                  /* smem row stride of the input tiles, in reals */
 #define IN_BYTES ((32 * LDI * (int)sizeof(real) + 15) & ~15)
 #define OUT_BYTES (32 * NOUT * (int)sizeof(real))
+#ifndef NOUT2
+#define NOUT2 0
+#endif
 #define NBUF (TPW > 1 ? 2 : 1)                        /* input buffers per warp */
-#define WARP_BYTES (NBUF * NIN * IN_BYTES + OUT_BYTES)
+#define WARP_BYTES (NBUF * NIN * IN_BYTES + OUT_BYTES + 32 * NOUT2 * (int)sizeof(real))
 
 __device__ __forceinline__ void load_tile(real *s, const real *g, int lane)
 {
@@ -156,7 +160,11 @@ __device__ __forceinline__ void load_tile(real *s, const real *g, int lane)
 // per SM the kernel was latency-bound (ncu: long-scoreboard the top stall, FP64 pipe 62 % busy).
 extern "C" __global__ void __launch_bounds__(128, MINB)
 k_rne_spec(const __grid_constant__ SpecP P, const real *__restrict__ in0, const real *__restrict__ in1,
-           const real *__restrict__ in2, real *__restrict__ out, long long ntiles)
+           const real *__restrict__ in2, real *__restrict__ out,
+#if NOUT2
+           real *__restrict__ out2,
+#endif
+           long long ntiles)
 {
     extern __shared__ __align__(16) unsigned char smem[];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -241,6 +249,11 @@ k_rne_spec(const __grid_constant__ SpecP P, const real *__restrict__ in0, const 
         }
 #pragma unroll
         for (int k = 0; k < NOUT; k++) so[lane * NOUT + k] = o[k];
+#if NOUT2
+        real *so2 = so + 32 * NOUT; // the second output's tile, right behind the first (a multiple of 16 bytes)
+#pragma unroll
+        for (int k = 0; k < NOUT2; k++) so2[lane * NOUT2 + k] = o[NOUT + k];
+#endif
         // the staged tile is the exact image of the output block: one TMA bulk copy (shared -> global) by lane 0
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
         __syncwarp();
@@ -248,6 +261,10 @@ k_rne_spec(const __grid_constant__ SpecP P, const real *__restrict__ in0, const 
             const unsigned ss = (unsigned)__cvta_generic_to_shared(so);
             asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(out + (size_t)tile * 32 * NOUT), "r"(ss),
                          "r"((unsigned)OUT_BYTES) : "memory");
+#if NOUT2
+            asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(out2 + (size_t)tile * 32 * NOUT2),
+                         "r"((unsigned)__cvta_generic_to_shared(so2)), "r"((unsigned)(32 * NOUT2 * sizeof(real))) : "memory");
+#endif
             asm volatile("cp.async.bulk.commit_group;" ::: "memory");
         }
     }
@@ -526,7 +543,7 @@ struct Program {
     std::string why;          // why not, when !ok
     std::string cubin;        // sm_90a image
     std::vector<double> consts;
-    int nin = 1, nout = 0, nres = 0, nc = 1, tpw = 1;
+    int nin = 1, nout = 0, nout2 = 0, nres = 0, nc = 1, tpw = 1;
     const char *entry = "k_rne_spec";
     int n_mul = 0, n_fma = 0, n_add = 0, regs = 0;
     size_t smem = 0;
@@ -565,9 +582,10 @@ std::string build_source(const GenFn &gen, int n, int mode, int dtype, Program &
     p.consts = g.consts;
     p.nc = (int)g.consts.size();
     p.n_mul = g.n_mul; p.n_fma = g.n_fma; p.n_add = g.n_add;
-    p.nin = (mode == B2K_GEN_RNE || mode == B2K_GEN_ACCEL) ? 3 : ((mode == B2K_GEN_ITORQUE || mode == B2K_GEN_CORIOLIS) ? 2 : 1);
+    p.nin = (mode == B2K_GEN_RNE || mode == B2K_GEN_ACCEL || mode == B2K_GEN_RNE_WRENCH) ? 3 : ((mode == B2K_GEN_ITORQUE || mode == B2K_GEN_CORIOLIS) ? 2 : 1);
     p.nout = (mode == B2K_GEN_INERTIA || mode == B2K_GEN_CORIOLIS) ? n * n : n;
-    p.nres = mode == B2K_GEN_ACCEL ? n * n + n : p.nout;
+    p.nout2 = mode == B2K_GEN_RNE_WRENCH ? 6 : 0; // tau (N, n) and the base wrench (N, 6)
+    p.nres = mode == B2K_GEN_ACCEL ? n * n + n : p.nout + p.nout2;
     const int es = dtype == B2K_F64 ? 8 : 4;
     // one-row-per-lane reads of an exact-image tile: conflict degree gcd(row words, banks served per wavefront)
     const int padin = gcd_i(n * es / 4, es == 8 ? 32 : 32) > (es == 8 ? 4 : 2) ? 1 : 0;
@@ -581,11 +599,11 @@ std::string build_source(const GenFn &gen, int n, int mode, int dtype, Program &
     // lane as f32x2 pairs (FFMA2 / FMUL2: 35 % fewer issued instructions, same time -- an FFMA2 still holds the FP32
     // pipe for two cycles and the kernel is not bound by issue at this size) and a persistent grid-stride loop with
     // double-buffered tiles (fp32 equal, fp64 slower: the second buffer's registers spill).
-    const bool light = mode == B2K_GEN_RNE || mode == B2K_GEN_GRAVLOAD || mode == B2K_GEN_ITORQUE;
+    const bool light = mode == B2K_GEN_RNE || mode == B2K_GEN_GRAVLOAD || mode == B2K_GEN_ITORQUE || mode == B2K_GEN_RNE_WRENCH;
     int tpw = (dtype == B2K_F32 && light) ? 2 : 1;
     if (const char *e = getenv("B2K_RNE_SPEC_TPW")) tpw = atoi(e) > 0 ? atoi(e) : tpw;
     p.tpw = tpw;
-    p.smem = 4 * ((tpw > 1 ? 2 : 1) * p.nin * in_bytes + (size_t)32 * p.nout * es);
+    p.smem = 4 * ((tpw > 1 ? 2 : 1) * p.nin * in_bytes + (size_t)32 * (p.nout + p.nout2) * es);
     if (p.smem > 220 * 1024) { p.why = "a tile of this operation does not fit the shared memory of an SM (" + std::to_string(p.smem) + " B)"; return std::string(); }
     int minb = (int)((200 * 1024) / (p.smem + 1024));
     // resident blocks to aim for (swept: fp64 96 registers / 5 blocks, fp32 64 registers / 8 blocks)
@@ -597,6 +615,7 @@ std::string build_source(const GenFn &gen, int n, int mode, int dtype, Program &
     defs.push_back(std::string("-DREAL=") + (es == 8 ? "double" : "float"));
     D("REAL_IS_F64", es == 8);
     D("NJ", n); D("NC", p.nc); D("MODE", mode); D("NIN", p.nin); D("NOUT", p.nout); D("NRES", p.nres); D("PADIN", padin); D("MINB", minb); D("TPW", tpw);
+    if (p.nout2) D("NOUT2", p.nout2);
     // in1 / in2 of the generated function are the second / third input rows; the RNE proper names them qd / qdd
     return std::string(kPrologue) + g.source + (kernel_text ? kernel_text : kKernel);
 }
@@ -730,11 +749,12 @@ std::vector<unsigned char> spec_params(Program *p, int n, int dtype, const doubl
 }
 
 int launch_tiles(Program *p, CUfunction fn, int n, int dtype, const double *offset, const void *in0, const void *in1, const void *in2,
-                 void *out, long long ntiles, const double *grav, const double *fext, cudaStream_t st)
+                 void *out, void *out2, long long ntiles, const double *grav, const double *fext, cudaStream_t st)
 {
     std::vector<unsigned char> pb = spec_params(p, n, dtype, offset, grav, fext);
     long long nt = ntiles;
-    void *args[6] = {pb.data(), (void *)&in0, (void *)&in1, (void *)&in2, (void *)&out, (void *)&nt};
+    void *args[7] = {pb.data(), (void *)&in0, (void *)&in1, (void *)&in2, (void *)&out, (void *)&nt, nullptr};
+    if (p->nout2) { args[5] = (void *)&out2; args[6] = (void *)&nt; } // k_rne_spec(..., out, out2, ntiles)
     const long long per_block = 4LL * p->tpw;
     const unsigned grid = (unsigned)((ntiles + per_block - 1) / per_block);
     CUresult rc = driver()->LaunchKernel(fn, grid, 1, 1, 128, 1, 1, (unsigned)p->smem, (CUstream)st, args, nullptr);
@@ -769,7 +789,7 @@ void b2k_rne_spec_detach(b2k_rne_s *r)
 // Tries the specialised kernel for the first (N / 32) * 32 rows.  Returns the number of rows it served (0 when the
 // call must go to the generic kernel entirely), or a negative b2k_status when B2K_RNE_SPEC=2 demands it and it failed.
 long long b2k_rne_spec_launch(const b2k_rne_s *r, int mode, int dtype, const void *in0, const void *in1, const void *in2,
-                              long long nrows, const double *grav, const double *fext, void *out, cudaStream_t st)
+                              long long nrows, const double *grav, const double *fext, void *out, void *out2, cudaStream_t st)
 {
     const int setting = spec_setting();
     if (setting == 0 || !r->spec) return 0;
@@ -779,12 +799,13 @@ long long b2k_rne_spec_launch(const b2k_rne_s *r, int mode, int dtype, const voi
     };
     const long long ntiles = nrows / 32;
     if (ntiles == 0) return 0;
-    const uintptr_t al = (uintptr_t)in0 | (uintptr_t)(in1 ? in1 : in0) | (uintptr_t)(in2 ? in2 : in0) | (uintptr_t)out;
+    const uintptr_t al = (uintptr_t)in0 | (uintptr_t)(in1 ? in1 : in0) | (uintptr_t)(in2 ? in2 : in0) | (uintptr_t)out | (uintptr_t)(out2 ? out2 : out);
     if (al & 15) return refuse("arrays are not 16-byte aligned");
+    const bool rne = mode == B2K_GEN_RNE || mode == B2K_GEN_RNE_WRENCH;
     int has_fext = 0;
-    if (mode == B2K_GEN_RNE && fext)
+    if (rne && fext)
         for (int k = 0; k < 6; k++) has_fext |= (fext[k] != 0.0);
-    const bool uses_grav = mode == B2K_GEN_RNE || mode == B2K_GEN_GRAVLOAD || mode == B2K_GEN_ACCEL;
+    const bool uses_grav = rne || mode == B2K_GEN_GRAVLOAD || mode == B2K_GEN_ACCEL;
     const Key key(mode, dtype, uses_grav ? grav_mask_of(grav) : 0, has_fext);
     Program *p = get_program(static_cast<SpecCache *>(r->spec), dh_gen(r, key), r->n, key);
     if (!p || !p->ok) return refuse(p ? p->why : "no cache");
@@ -796,7 +817,7 @@ long long b2k_rne_spec_launch(const b2k_rne_s *r, int mode, int dtype, const voi
     }
     double offset[B2K_MAX_JOINTS];
     for (int j = 0; j < r->n; j++) offset[j] = r->L[j][5];
-    const int lrc = launch_tiles(p, fn, r->n, dtype, offset, in0, in1, in2, out, ntiles, uses_grav ? grav : nullptr,
+    const int lrc = launch_tiles(p, fn, r->n, dtype, offset, in0, in1, in2, out, out2, ntiles, uses_grav ? grav : nullptr,
                                  has_fext ? fext : nullptr, st);
     if (lrc) return lrc;
     return ntiles * 32;
@@ -833,7 +854,7 @@ extern "C" int b2k_rne_spec_info(b2k_rne_t r, int mode, int dtype, const double 
         {
             // mode 200 + m: the forward-dynamics integrator built around operation m (only m = accel exists)
             const int gm = mode % 100;
-            const bool ug = gm == B2K_GEN_RNE || gm == B2K_GEN_GRAVLOAD || gm == B2K_GEN_ACCEL;
+            const bool ug = gm == B2K_GEN_RNE || gm == B2K_GEN_GRAVLOAD || gm == B2K_GEN_ACCEL || gm == B2K_GEN_RNE_WRENCH;
             const Key key(mode, dtype, ug ? grav_mask_of(grav) : 0, has_fext);
             const Key gkey(gm, dtype, ug ? grav_mask_of(grav) : 0, has_fext);
             Program *p = get_program(static_cast<SpecCache *>(r->spec), dh_gen(r, gkey), r->n, key);
@@ -935,7 +956,7 @@ static int tree_run(const char *fn, b2k_tree_t t, int mode, int dtype, const voi
     const long long ntiles = N / 32, tail = N - ntiles * 32;
     const double *gv = ug ? grav : nullptr;
     int rc = B2K_OK;
-    if (ntiles) rc = launch_tiles(p, f, n, dtype, nullptr, in0, in1, in2, out, ntiles, gv, nullptr, st);
+    if (ntiles) rc = launch_tiles(p, f, n, dtype, nullptr, in0, in1, in2, out, nullptr, ntiles, gv, nullptr, st);
     if (rc == B2K_OK && tail) { // ragged tail: one padded tile through stream-ordered scratch
         b2k_keep_mempool();
         char *scr = nullptr;
@@ -945,7 +966,7 @@ static int tree_run(const char *fn, b2k_tree_t t, int mode, int dtype, const voi
         const void *src[3] = {in0, in1, in2};
         for (int i = 0; i < nin; i++) cudaMemcpyAsync(scr + i * 32 * rowb, (const char *)src[i] + off, tail * rowb, cudaMemcpyDeviceToDevice, st);
         char *so = scr + 3 * 32 * rowb;
-        rc = launch_tiles(p, f, n, dtype, nullptr, scr, scr + 32 * rowb, scr + 2 * 32 * rowb, so, 1, gv, nullptr, st);
+        rc = launch_tiles(p, f, n, dtype, nullptr, scr, scr + 32 * rowb, scr + 2 * 32 * rowb, so, nullptr, 1, gv, nullptr, st);
         cudaMemcpyAsync((char *)out + (size_t)ntiles * 32 * orowb, so, tail * orowb, cudaMemcpyDeviceToDevice, st);
         cudaFreeAsync(scr, st);
         cudaError_t e = cudaGetLastError();

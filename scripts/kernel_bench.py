@@ -123,6 +123,32 @@ for dt in (np.float64, np.float32):
     os.environ["B2K_RNE_SPEC"] = "1"
     del bufs, tau
 
+# rne with the base wrench (DHRobot.rne(base_wrench=True)): tau (N,6) and wbase (N,6) from one recursion; bytes per row
+# = sizeof(real) (4n + 6), against 4n for plain rne
+for dt in (np.float64, np.float32):
+    tag = "f64" if dt == np.float64 else "f32"
+    if not want(f"rne_wrench_puma_{tag}"):
+        continue
+    es = np.dtype(dt).itemsize
+    nbuf = 3
+    ql = puma.qlim
+    bufs = [tuple(torch.from_numpy(a.astype(dt)).to(dev) for a in (rng.uniform(ql[0], ql[1], (N, 6)), rng.normal(size=(N, 6)), rng.normal(size=(N, 6)))) for _ in range(nbuf)]
+    tau = torch.empty((N, 6), dtype=tdt[dt], device=dev)
+    wb = torch.empty((N, 6), dtype=tdt[dt], device=dev)
+    puma.rne(*bufs[0])
+    L = rtb._lib.lib()
+    st = torch.cuda.current_stream().cuda_stream
+    code = rtb._lib.F64 if dt == np.float64 else rtb._lib.F32
+    g = np.ascontiguousarray(-puma.gravity)
+    for variant, setting in (("", "1"), ("_generic", "0")):
+        if variant and not want(f"rne_wrench_puma_{tag}{variant}"):
+            continue
+        os.environ["B2K_RNE_SPEC"] = setting
+        report(f"rne_wrench_puma_{tag}{variant}", timeit(lambda i: L.b2k_rne_wrench(puma._rne_ob, code, bufs[i][0].data_ptr(), bufs[i][1].data_ptr(), bufs[i][2].data_ptr(), N, rtb._lib.dptr(g), None, tau.data_ptr(), wb.data_ptr(), st), nbuf), N, (4 * 6 + 6) * es,
+               {"kernel": puma.rne_kernel_info("rne_wrench", dt)})
+    os.environ["B2K_RNE_SPEC"] = "1"
+    del bufs, tau, wb
+
 # dynamics fan-outs over the RNE recursion (SURVEY 8f-1): Puma560, fp64
 if want("dyn_"):
     Nd = max(1, N // 4)
