@@ -92,11 +92,19 @@ __device__ __forceinline__ void rotvel_inverse(int rep, const real g[3], real A[
         A[0][0] = -cp * ct / st; A[0][1] = -sp * ct / st; A[0][2] = 1;
         A[1][0] = -sp;           A[1][1] = cp;            A[1][2] = 0;
         A[2][0] = cp / st;       A[2][1] = sp / st;       A[2][2] = 0;
-    } else { // exponential coordinates: A^-1 = I - [v]x / 2 + [v]x^2 (1 - (theta / 2) sin / (1 - cos)) / theta^2
+    } else { // exponential coordinates: A^-1 = I - [v]x / 2 + k2 [v]x^2, k2 = (1 - x cot x) / theta^2, x = theta / 2
+        // The equal form (1 - x sin(theta) / (1 - cos(theta))) / theta^2 loses the digits of 1 - cos(theta) to
+        // cancellation at small theta (fp32: cos rounds to 1 below theta ~ 3.5e-4 and k2 is -inf).  Below theta0 (0.1
+        // fp64, 0.5 fp32) the series, whose first omitted term theta^8 / 47900160 is below the dtype's rounding there;
+        // above it 1 - x cot x >= theta0^2 / 12 loses a few bits, which the factor theta^2 of [v]x^2 gives back.
         const real th2 = g[0] * g[0] + g[1] * g[1] + g[2] * g[2], th = sqrt(th2);
         real k2;
-        if (th < (real)1e-4) k2 = (real)1 / 12; // series: 1/12 + theta^2 / 720
-        else k2 = (1 - (th / 2) * sin(th) / (1 - cos(th))) / th2;
+        if (th < (sizeof(real) == 8 ? (real)0.1 : (real)0.5))
+            k2 = (real)1 / 12 + th2 * ((real)1 / 720 + th2 * ((real)1 / 30240 + th2 * ((real)1 / 1209600)));
+        else {
+            const real x = th / 2;
+            k2 = (1 - x * cos(x) / sin(x)) / th2;
+        }
         const real S[3][3] = {{0, -g[2], g[1]}, {g[2], 0, -g[0]}, {-g[1], g[0], 0}};
         for (int i = 0; i < 3; i++)
             for (int j = 0; j < 3; j++) {
@@ -353,12 +361,16 @@ extern "C" int b2k_ctraj(int dtype, const double *T0, const double *T1, const vo
     host_r2q(T1, P.q1);
     double dot = 0;
     for (int k = 0; k < 4; k++) dot += P.q0[k] * P.q1[k];
-    if (dot < 0) { // shortest arc (qslerp: q0 = -q0)
+    if (dot < 0) // shortest arc (qslerp: q0 = -q0)
         for (int k = 0; k < 4; k++) P.q0[k] = -P.q0[k];
-        dot = -dot;
+    // the angle between the unit quaternions as 2 atan2(|q1 - q0|, |q1 + q0|): acos(dot) keeps only half the digits of
+    // a small angle and is 0 below ~1e-8, where the orientation would then stay at T0's all the way and jump at s = 1
+    double dm = 0, ds = 0;
+    for (int k = 0; k < 4; k++) {
+        dm += (P.q1[k] - P.q0[k]) * (P.q1[k] - P.q0[k]);
+        ds += (P.q1[k] + P.q0[k]) * (P.q1[k] + P.q0[k]);
     }
-    if (dot > 1) dot = 1;
-    P.theta = acos(dot);
+    P.theta = 2 * atan2(sqrt(dm), sqrt(ds));
     P.sin_theta = sin(P.theta);
     P.lerp_only = !(fabs(P.theta) > 10 * 2.220446049250313e-16);
     for (int k = 0; k < 3; k++) { P.p0[k] = T0[4 * k + 3]; P.p1[k] = T1[4 * k + 3]; }

@@ -259,6 +259,7 @@ if want("extra_"):
         ("extra_jacobm_from_J_f64", lambda i: pe.jacobm(J=Jx), (42 + 7) * 8),
         ("extra_jacob0_dot_f64", lambda i: pe.jacob0_dot(qd=QDx, J0=Jx), (42 + 7 + 42) * 8),
         ("extra_jacob0_analytical_rpy_f64", lambda i: pe.jacob0_analytical(Qx), (7 + 42) * 8),
+        ("extra_jacob0_analytical_exp_f64", lambda i: pe.jacob0_analytical(Qx, representation="exp"), (7 + 42) * 8),
         ("extra_angle_axis_f64", lambda i: rtb.angle_axis(Tx, Ty), (32 + 6) * 8),
         ("extra_p_servo_rpy_f64", lambda i: rtb.p_servo(Tx, Ty), (32 + 6) * 8 + 1),
         ("extra_jtraj_f64", lambda i: rtb.jtraj(np.zeros(7), np.ones(7), NX, device=True), 21 * 8),
