@@ -284,6 +284,33 @@ int b2k_rne_coriolis(b2k_rne_t rne, int dtype, const void *q, const void *qd, in
 int b2k_rne_accel(b2k_rne_t rne, int dtype, const void *q, const void *qd, const void *torque, int64_t N,
                   const double *grav, void *qdd, void *stream);
 
+/* ---------------------------------------------------------------- static forces (DynamicsMixin, robot/Dynamics.py)
+ * One forward walk over a compiled chain per row (base and tool as the chain has them, as for b2k_jacob0); q is (N, ldq)
+ * with the joint coordinates at the chain's joint indices.  Unlike b2k_rne, `grav` is the world-frame gravity AS THE
+ * ROBOT STORES IT (host 3-vector, not negated).  `mass` is a host table of n x 4 doubles (m_j, c_j): c_j is link j's
+ * centre of mass in the frame right after joint j's elementary transform.  Flipped joints follow the chain, as in
+ * b2k_jacob0 (b2k_rne ignores flip).  Wrenches W = [fx fy fz mx my mz] are device arrays: w_stride 0 = one wrench for
+ * every row, 6 = (N, 6).  frame 0: W in the world frame; 1: in the end-effector frame.  Arguments are validated before
+ * any CUDA call (NULL pointers, n range, frame, natural alignment); N = 0 returns without touching the device.
+ *   b2k_gravjac      taug (N,n) = -sum_i J_ci^T m_i g and J0 (N,6,n) = jacob0       DynamicsMixin.gravjac
+ *   b2k_pay          tau (N,n) = -J^T W, J = jacob0 (frame 0) or jacobe (frame 1)  DynamicsMixin.pay (given q)
+ *   b2k_pay_jacobian tau (N,n) = -J^T W from a given J (N,6,n)                      DynamicsMixin.pay (given J)
+ *   b2k_paycap       wmax (N,n), joint (N) int32: with w^ = w / |w| per row, tau_B the gravity load and
+ *                    tau_P = pay(w^), wmax_j = (tauR[j,0] - tau_B,j) / tau_P,j if tau_P,j > 0, (tauR[j,1] - tau_B,j) /
+ *                    tau_P,j if < 0, +inf if 0; joint = first argmin; a zero w row gives NaN and -1.
+ *                    tauR: host n x 2 doubles (max, min)                              DynamicsMixin.paycap
+ *   b2k_friction     tau (N,n) = -(G^2 B qd + |G| Tc(qd)), Tc(qd) = Tc+ (qd > 0), Tc- (qd < 0), 0;
+ *                    params: host n x 4 doubles (B, G, Tc+, Tc-)                      Link.friction / DynamicsMixin.friction
+ */
+int b2k_gravjac(b2k_chain_t chain, int dtype, const void *q, int64_t N, int64_t ldq, const double *mass, const double *grav,
+                void *taug, void *J0, void *stream);
+int b2k_pay(b2k_chain_t chain, int dtype, const void *q, int64_t N, int64_t ldq, const void *W, int64_t w_stride, int frame,
+            void *tau, void *stream);
+int b2k_pay_jacobian(int dtype, int n, const void *J, const void *W, int64_t w_stride, int64_t N, void *tau, void *stream);
+int b2k_paycap(b2k_chain_t chain, int dtype, const void *q, int64_t N, int64_t ldq, const double *mass, const double *grav,
+               const void *w, int64_t w_stride, int frame, const double *tauR, void *wmax, int32_t *joint, void *stream);
+int b2k_friction(int dtype, int n, const double *params, const void *qd, int64_t N, void *tau, void *stream);
+
 /* b2k_rne_fdyn integrates the forward dynamics of an ENSEMBLE of initial states (DynamicsMixin.fdyn, Dynamics.py:185-422,
  * integrates one): one lane per trajectory, Dormand-Prince 5(4) with scipy RK45's step control (rtol, atol, max_step,
  * first_step <= 0: automatic), every stage's acceleration from the robot-specialised recursion.  q0, qd0 (ntraj,n) device

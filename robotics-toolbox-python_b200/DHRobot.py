@@ -16,6 +16,7 @@ import numpy as np
 from . import _buffers as B
 from . import _lib
 from . import _opspace
+from . import _static
 from ._se3 import SE3
 from .DHLink import DHLink
 from .ET import ET
@@ -44,6 +45,7 @@ class DHRobot:
         self._dynchanged = False
         self._ets_cache = None
         self._prefix_cache = None
+        self._static_mass = None
         self._configs = {}
 
     # ---- structure
@@ -306,11 +308,13 @@ class DHRobot:
         packed RNE table are both stale (reference DHLink.py:448-563 @_listen_dyn on theta/d/a/alpha/sigma/mdh)."""
         self._ets_cache = None
         self._prefix_cache = None
+        self._static_mass = None
         self._dynchanged = True
 
     def dynchanged(self, what=None):
         """Mark the packed dynamic parameters stale (reference BaseRobot.py:383-398)."""
         self._dynchanged = True
+        self._static_mass = None
 
     def _pack_rne(self) -> np.ndarray:
         """24 doubles per link (reference DHRobot._init_rne 1340-1358)."""
@@ -526,6 +530,60 @@ class DHRobot:
         """Forward dynamics qdd = M(q)^-1 (torque - rne(q, qd, 0)), joint friction included
         (reference Dynamics.accel, Dynamics.py:424-510)."""
         return self._dyn("b2k_rne_accel", [q, qd, torque], (self.n,), gravity=gravity, use_gravity=True, dtype=dtype)
+
+    # ---- static forces (reference DynamicsMixin, Dynamics.py): _static.py, csrc/b2k_static.cu
+    def _static_mass_table(self) -> np.ndarray:
+        """n x 4 doubles (m_j, c_j) for b2k_gravjac / b2k_paycap: c_j is link j's centre of mass in the frame right after
+        its joint, tail_j r_j, with tail_j the link's elementary transforms behind the joint (DHLink._to_ets)."""
+        if self._static_mass is None:
+            M = np.zeros((self.n, 4))
+            for j, l in enumerate(self.links):
+                ets = list(l.ets)
+                tail = np.eye(4)
+                for et in ets[next(i for i, et in enumerate(ets) if et.isjoint) + 1:]:
+                    tail = tail @ et.A()
+                M[j, 0] = l.m
+                M[j, 1:] = tail[:3, :3] @ l.r + tail[:3, 3]
+            self._static_mass = np.ascontiguousarray(M)
+        return self._static_mass
+
+    def gravjac(self, q, gravity=None, dtype=None):
+        """Gravity load and base-frame Jacobian from one walk (reference DynamicsMixin.gravjac): ``(tau, J0)``, tau (n,) /
+        (N,n) = -sum_i J_ci^T m_i g from the link centre-of-mass Jacobians, g the world-frame gravity (default
+        ``robot.gravity``); J0 (6,n) / (N,6,n) equals ``jacob0(q)`` (base and tool included).  tau equals ``gravload`` for
+        robots without flipped joints; a flipped joint follows the chain here, as in ``jacob0``, while ``rne`` and
+        ``gravload`` ignore ``flip`` (as the reference's frne does)."""
+        return _static.gravjac(self, q, gravity=gravity, dtype=dtype)
+
+    def pay(self, W, q=None, J=None, frame=1, dtype=None):
+        """Joint torques of a payload wrench W = [fx fy fz mx my mz] applied to the end effector (reference
+        DynamicsMixin.pay): tau = -J^T W, (n,) / (N,n).  W (6,) is one wrench for every row, (N,6) one per row; it is in
+        the end-effector frame for ``frame=1`` (J = jacobe) and the world frame for ``frame=0`` (J = jacob0).  Give
+        exactly one of q and J; a given J (6,n) / (N,6,n) is used as it is and ``frame`` does not enter."""
+        return _static.pay(self.ets(), W, q=q, J=J, frame=frame, dtype=dtype)
+
+    def paycap(self, w, tauR, frame=1, q=None, gravity=None, dtype=None):
+        """Static payload capacity under joint torque limits (reference DynamicsMixin.paycap): ``(wmax, joint)``.
+        With w^ = w / |w| per row, tau_B the gravity load and tau_P = pay(w^, q, frame), wmax_j = (tauR[j,0] - tau_B,j) /
+        tau_P,j where tau_P,j > 0, (tauR[j,1] - tau_B,j) / tau_P,j where tau_P,j < 0, +inf where tau_P,j = 0; joint is
+        the first argmin, so the capacity of a pose is wmax[joint].  tauR is (n,2): column 0 the largest torque, column 1
+        the smallest.  wmax (n,) / (N,n); joint an int / (N,) int32 array.  A zero row of an (N,6) w gives NaN and -1."""
+        return _static.paycap(self, w, tauR, frame=frame, q=q, gravity=gravity, dtype=dtype)
+
+    def friction(self, qd, dtype=None):
+        """Joint friction torque (reference DynamicsMixin.friction / Link.friction): tau_j = -(G_j^2 B_j qd_j +
+        |G_j| Tc_j(qd_j)), Tc_j = Tc+ for qd_j > 0, Tc- for qd_j < 0, 0 at rest -- the terms ``rne`` adds, negated.
+        (n,) / (N,n)."""
+        return _static.friction(self, qd, dtype=dtype)
+
+    def payload(self, m, p=(0.0, 0.0, 0.0)):
+        """Put a point mass m at p (in the last link's frame; the tool does not enter) on the last link (reference
+        DynamicsMixin.payload): its mass and centre of mass are replaced, its inertia tensor is kept.  ``payload(0)``
+        removes the last link's mass.  Goes through the link setters, so the next rne / gravload / gravjac / paycap
+        sees the new mass."""
+        last = self.links[-1]
+        last.m = m
+        last.r = p
 
     # ---- operational-space dynamics (reference DynamicsMixin, Dynamics.py between gravload and itorque): _opspace.py
     def inertia_x(self, q, pinv=False, representation="rpy/xyz", Ji=None, dtype=None):

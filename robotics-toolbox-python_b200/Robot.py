@@ -13,6 +13,7 @@ import numpy as np
 from . import _buffers as B
 from . import _lib
 from . import _opspace
+from . import _static
 from ._se3 import SE3
 from .DHLink import _inertia
 from .ET import ET
@@ -316,6 +317,18 @@ class Robot:
     # RobotKinematics.py:158 / 219: the Jacobians do NOT see the base
     def jacob0(self, q, end=None, start=None, tool=None, **kw):
         return self.ets(start, end).jacob0(q, tool=self._tool_arg(tool), **kw)
+
+    def pay(self, W, q=None, J=None, frame=1, end=None, start=None, tool=None, dtype=None):
+        """Joint torques -J^T W of a payload wrench on the end effector of ``ets(start, end)`` (reference
+        DynamicsMixin.pay); see DHRobot.pay.  J = jacobe (frame 1) or jacob0 (frame 0) of that chain with the tool, as
+        ``jacobe`` / ``jacob0`` give them; tau has one entry per joint of the chain, in chain order (the columns of J)."""
+        e = self.ets(start, end)
+        T = self._tool_arg(tool)
+        if T is not None and q is not None:
+            T = _mat44(T, "tool")
+            if not np.array_equal(T, np.eye(4)):
+                e = ETS([*e, ET.SE3(T)])
+        return _static.pay(e, W, q=q, J=J, frame=frame, dtype=dtype)
 
     def jacobe(self, q, end=None, start=None, tool=None, **kw):
         return self.ets(start, end).jacobe(q, tool=self._tool_arg(tool), **kw)

@@ -68,6 +68,11 @@ _PROTOS = {
     "b2k_rne_itorque": (C.c_int, [vp, C.c_int, vp, vp, i64, vp, vp]),
     "b2k_rne_coriolis": (C.c_int, [vp, C.c_int, vp, vp, i64, vp, vp]),
     "b2k_rne_accel": (C.c_int, [vp, C.c_int, vp, vp, vp, i64, dp, vp, vp]),
+    "b2k_gravjac": (C.c_int, [vp, C.c_int, vp, i64, i64, dp, dp, vp, vp, vp]),
+    "b2k_pay": (C.c_int, [vp, C.c_int, vp, i64, i64, vp, i64, C.c_int, vp, vp]),
+    "b2k_pay_jacobian": (C.c_int, [C.c_int, C.c_int, vp, vp, i64, i64, vp, vp]),
+    "b2k_paycap": (C.c_int, [vp, C.c_int, vp, i64, i64, dp, dp, vp, i64, C.c_int, dp, vp, vp, vp]),
+    "b2k_friction": (C.c_int, [C.c_int, C.c_int, dp, vp, i64, vp, vp]),
     "b2k_hessian": (C.c_int, [C.c_int, C.c_int, vp, i64, vp, vp]),
     "b2k_manipulability": (C.c_int, [C.c_int, C.c_int, vp, i64, C.c_uint32, vp, vp]),
     "b2k_manipulability_svd": (C.c_int, [C.c_int, C.c_int, vp, i64, C.c_uint32, C.c_int, vp, vp]),

@@ -149,6 +149,50 @@ for dt in (np.float64, np.float32):
     os.environ["B2K_RNE_SPEC"] = "1"
     del bufs, tau, wb
 
+# static forces (csrc/b2k_static.cu): one chain walk per row.  Algorithmic bytes per row, sizeof(real) = es:
+#   static_gravjac_puma             q (n) in; tau (n) and J0 (6n) out                       = 8n es
+#   static_gravload_plus_jacob0     the two launches gravjac replaces: q read by each       = 9n es
+#   static_pay_panda                q (n) in, tau (n) out, one wrench for every row         = 2n es
+#   static_paycap_puma              q (n) and w (6) in; wmax (n) and joint (4 B) out        = (2n + 6) es + 4
+for dt in (np.float64, np.float32):
+    tag = "f64" if dt == np.float64 else "f32"
+    if not want(f"static_{tag}") and not any(want(f"static_{c}_{tag}") for c in ("gravjac_puma", "gravload_plus_jacob0_puma", "pay_panda", "paycap_puma")):
+        continue
+    es = np.dtype(dt).itemsize
+    code = rtb._lib.F64 if dt == np.float64 else rtb._lib.F32
+    L = rtb._lib.lib()
+    st = torch.cuda.current_stream().cuda_stream
+    nbuf = 3
+    ql = puma.qlim
+    qs = [torch.from_numpy(rng.uniform(ql[0], ql[1], (N, 6)).astype(dt)).to(dev) for _ in range(nbuf)]
+    tau = torch.empty((N, 6), dtype=tdt[dt], device=dev)
+    J = torch.empty((N, 6, 6), dtype=tdt[dt], device=dev)
+    pch, mass = puma.ets()._chain, puma._static_mass_table()
+    g = np.ascontiguousarray(puma.gravity)
+    ng = np.ascontiguousarray(-puma.gravity)
+    puma.gravload(qs[0][:64])  # builds the RNE handle (and the specialised kernel)
+    if want(f"static_gravjac_puma_{tag}"):
+        report(f"static_gravjac_puma_{tag}", timeit(lambda i: L.b2k_gravjac(pch, code, qs[i].data_ptr(), N, 6, rtb._lib.dptr(mass), rtb._lib.dptr(g), tau.data_ptr(), J.data_ptr(), st), nbuf), N, 8 * 6 * es)
+    if want(f"static_gravload_plus_jacob0_puma_{tag}"):
+        def two(i):
+            L.b2k_rne_gravload(puma._rne_ob, code, qs[i].data_ptr(), N, rtb._lib.dptr(ng), tau.data_ptr(), st)
+            L.b2k_jacob0(pch, code, qs[i].data_ptr(), N, 6, None, J.data_ptr(), st)
+        report(f"static_gravload_plus_jacob0_puma_{tag}", timeit(two, nbuf), N, 9 * 6 * es, {"gravload_kernel": puma.rne_kernel_info("gravload", dt)})
+    if want(f"static_paycap_puma_{tag}"):
+        tauR = np.ascontiguousarray(np.tile([[100.0, -100.0]], (6, 1)))
+        w = torch.tensor([0.0, 0.0, -1.0, 0.0, 0.0, 0.0], dtype=tdt[dt], device=dev)
+        jt = torch.empty((N,), dtype=torch.int32, device=dev)
+        report(f"static_paycap_puma_{tag}", timeit(lambda i: L.b2k_paycap(pch, code, qs[i].data_ptr(), N, 6, rtb._lib.dptr(mass), rtb._lib.dptr(g), w.data_ptr(), 0, 1, rtb._lib.dptr(tauR), tau.data_ptr(), jt.data_ptr(), st), nbuf), N, (2 * 6 + 6) * es + 4)
+    del qs, tau, J
+    if want(f"static_pay_panda_{tag}"):
+        pe = rtb.models.Panda().ets()
+        n = pe.n
+        qs = [torch.from_numpy(rng.uniform(-np.pi, np.pi, (N, n)).astype(dt)).to(dev) for _ in range(nbuf)]
+        tau = torch.empty((N, n), dtype=tdt[dt], device=dev)
+        W = torch.tensor([1.0, -2.0, 3.0, 0.1, 0.2, -0.3], dtype=tdt[dt], device=dev)
+        report(f"static_pay_panda_{tag}", timeit(lambda i: L.b2k_pay(pe._chain, code, qs[i].data_ptr(), N, n, W.data_ptr(), 0, 1, tau.data_ptr(), st), nbuf), N, 2 * n * es)
+        del qs, tau
+
 # dynamics fan-outs over the RNE recursion (SURVEY 8f-1): Puma560, fp64
 if want("dyn_"):
     Nd = max(1, N // 4)
