@@ -161,8 +161,12 @@ static int fkj_dispatch(const char *fn, b2k_chain_t c, int dtype, int mode, cons
 {
     int rc = check_common(fn, c, dtype, q, N, ldq);
     if (rc) return rc;
-    if ((mode & FKJ_T) && (rc = check_out(fn, "T", T, N))) return rc;
-    if ((mode & (FKJ_J0 | FKJ_JE)) && (rc = check_out(fn, "J", J, N))) return rc;
+    // T is stored in 32-byte pieces; J leaves through a shared-memory stage whose copy unit (TileStage<real, 6n>::UB in
+    // b2k_fkj.cuh) is 16 bytes when a 6n-element row is a whole number of 16-byte units, else 8
+    const unsigned es = dtype == B2K_F64 ? 8u : 4u;
+    const unsigned jub = (6u * (unsigned)c->n * es) % 16u == 0 ? 16u : 8u;
+    if ((mode & FKJ_T) && (rc = check_out(fn, "T", T, N, 32))) return rc;
+    if ((mode & (FKJ_J0 | FKJ_JE)) && (rc = check_out(fn, "J", J, N, jub))) return rc;
     if ((rc = check_affine(fn, "base", base)) || (rc = check_affine(fn, "tool", tool))) return rc;
     if (N == 0) return B2K_OK;
     B2K_ON_DEVICE_OF(q);

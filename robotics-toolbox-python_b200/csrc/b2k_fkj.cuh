@@ -954,11 +954,7 @@ int fkj_launch_n(const b2k_chain_s *c, int mode, const real *q, long long nrows,
     const size_t wsm = (fkj_warp_smem<real, N>(ldq, wt, wj0 || wje) + 15) & ~(size_t)15;
     const size_t smem = wsm * B2K_WARPS_PER_BLOCK;
     const float inv_ldq = 1.0f / (float)ldq;
-    if (wt && (((uintptr_t)T) & 31)) { b2k_set_error("fkj: T must be 32-byte aligned"); return B2K_ERR_INVALID; }
-    if ((wj0 || wje) && (((uintptr_t)J) % TileStage<real, 6 * N>::UB)) {
-        b2k_set_error("fkj: J must be %d-byte aligned", TileStage<real, 6 * N>::UB);
-        return B2K_ERR_INVALID;
-    }
+    // (the caller, fkj_dispatch, has checked that T is 32-byte aligned and J aligned to TileStage<real, 6 * N>::UB)
 
     const int variant = b2k_get_variant();
     const int dbg = variant == 2 ? 1 : (variant == 3 ? 2 : 0);
