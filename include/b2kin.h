@@ -475,14 +475,6 @@ int64_t b2k_launch_count(void);
  * its accuracy can be checked in isolation: s[i], c[i] = sin(x[i]), cos(x[i]). */
 int b2k_selftest_sincos(int dtype, const void *x, int64_t n, void *s, void *c, void *stream);
 
-/* kernel variant switch for measurements: 0 = default (lane-per-configuration, warp-tiled
- * I/O), 1 = literal warp-per-configuration walk (one joint configuration per warp),
- * 2 = memory skeleton (default kernel without the chain walk: outputs are NOT valid),
- * 3 = arithmetic skeleton (default kernel without the output stores),
- * 4 = persistent grid-stride scheduling instead of the default one-tile-per-warp grid.
- * Affects b2k_fkine / b2k_jacob0 / b2k_fkine_jacob0 only; never set it in production. */
-int b2k_set_variant(int variant);
-
 #ifdef __cplusplus
 }
 #endif

@@ -19,7 +19,6 @@ slow Python (ETS.py:1075-1078) is deliberately not reproduced.
 from __future__ import annotations
 
 import ctypes as C
-import os
 from typing import List, Optional, Union
 
 import numpy as np
@@ -306,27 +305,6 @@ class ETS:
         N = qd.shape[0]
         base = _mat44(base, "base")
         b0 = np.eye(4) if base is None else base
-        if not ETS.frames_single_walk:
-            # one pose launch per frame over the prefix chains into frame-major memory (each launch re-reads q and
-            # re-walks its prefix); kept selectable for measurement
-            frames = B.empty((len(chains) + 1, N, 4, 4), dt, like=qd)
-            t = B.require_cuda()
-            b0 = np.eye(4) if base is None else base
-            frames[0] = t.as_tensor(b0, dtype=frames.dtype, device=frames.device)
-            L = _lib.lib()
-            for k, e in enumerate(chains):
-                if e.n == 0:  # a static frame (a link before the first joint): base times the constant transforms
-                    Tc = b0.copy()
-                    for et in e:
-                        Tc = Tc @ et.A()
-                    frames[k + 1] = t.as_tensor(Tc, dtype=frames.dtype, device=frames.device)
-                    continue
-                _lib.check(L.b2k_fkine(e._chain, B.code(dt), B.ptr(qd), N, qd.shape[1], _lib.dptr(base), None, B.ptr(frames[k + 1]),
-                                       B.stream_ptr(qd)))
-            out = frames.permute(1, 0, 2, 3)
-            if host:
-                out = np.ascontiguousarray(B.to_host(out.contiguous()))
-            return out[0] if single else out
         K = len(chains)
         out = B.empty((N, K + 1, 4, 4), dt, like=qd)
         L = _lib.lib()
@@ -341,7 +319,6 @@ class ETS:
             out = B.to_host(out)
         return out[0] if single else out
 
-    frames_single_walk = os.environ.get("B2K_FRAMES_SINGLE_WALK", "1") != "0"
     _frame_plans: dict = {}  # tuple(id(chain)) -> (the chains (kept alive: their ids stay theirs), launches)
 
     @staticmethod

@@ -11,7 +11,7 @@ IKSolution, IK_LM, models.*).  The directory name is not a Python identifier; im
 There is no CPU fallback in this package.
 """
 from . import _lib  # noqa: F401
-from ._lib import B2KError, launch_count, pinned_empty, set_variant  # noqa: F401
+from ._lib import B2KError, launch_count, pinned_empty  # noqa: F401
 from ._se3 import SE3  # noqa: F401
 from .ET import ET  # noqa: F401
 from .IK import IK_GN, IK_LM, IK_NR, IKSolution  # noqa: F401

@@ -96,7 +96,6 @@ _PROTOS = {
     "b2k_rne_host": (C.c_int, [vp, C.c_int, vp, vp, vp, i64, dp, dp, vp, C.c_int]),
     "b2k_rne_wrench_host": (C.c_int, [vp, C.c_int, vp, vp, vp, i64, dp, dp, vp, vp, C.c_int]),
     "b2k_launch_count": (C.c_int64, []),
-    "b2k_set_variant": (C.c_int, [C.c_int]),
     "b2k_selftest_sincos": (C.c_int, [C.c_int, vp, i64, vp, vp, vp]),
 }
 
@@ -154,10 +153,6 @@ def f64_or_none(a, shape):
 
 def launch_count() -> int:
     return int(lib().b2k_launch_count())
-
-
-def set_variant(v: int):
-    check(lib().b2k_set_variant(int(v)))
 
 
 class _PinnedPool:

@@ -18,8 +18,6 @@ int b2k_fkj_launch_f32(const b2k_chain_s *, int, const void *, long long, long l
                        void *, void *, cudaStream_t);
 int b2k_fkj_launch_f64(const b2k_chain_s *, int, const void *, long long, long long, const double *, const double *,
                        void *, void *, cudaStream_t);
-int b2k_fkw_launch(const b2k_chain_s *, int dtype, int mode, const void *, long long, long long, const double *,
-                   const double *, void *, void *, cudaStream_t);
 int b2k_rne_launch(const b2k_rne_s *, int dtype, const void *, const void *, const void *, long long, const double *,
                    const double *, void *, cudaStream_t);
 int b2k_rne_wrench_launch(const b2k_rne_s *, int dtype, const void *, const void *, const void *, long long, const double *,
@@ -30,7 +28,6 @@ enum { FKJ_T = 1, FKJ_J0 = 2, FKJ_JE = 4 };
 // ------------------------------------------------------------------ error / accounting plumbing
 static thread_local char g_err[512] = "";
 static std::atomic<long long> g_launches{0};
-static std::atomic<int> g_variant{0};
 
 void b2k_set_error(const char *fmt, ...)
 {
@@ -47,7 +44,6 @@ int b2k_cuda_fail(cudaError_t e, const char *what)
 }
 
 void b2k_count_launch(int n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
-int b2k_get_variant() { return g_variant.load(std::memory_order_relaxed); }
 
 int b2k_num_sms(int *device_out)
 {
@@ -87,13 +83,6 @@ int b2k_blocks_per_sm(const void *func, int threads, size_t smem)
     return per_sm;
 }
 
-int b2k_tiles_per_warp(bool with_jacobian)
-{
-    static const int pose = [] { const char *e = getenv("B2K_TPW_POSE"); int v = e ? atoi(e) : 1; return v < 1 ? 1 : v; }();
-    static const int jac = [] { const char *e = getenv("B2K_TPW_JAC"); int v = e ? atoi(e) : 1; return v < 1 ? 1 : v; }();
-    return with_jacobian ? jac : pose;
-}
-
 void b2k_keep_mempool()
 {
     static std::mutex mu;
@@ -113,12 +102,6 @@ void b2k_keep_mempool()
 extern "C" const char *b2k_last_error(void) { return g_err; }
 extern "C" int b2k_version(void) { return B2K_VERSION; }
 extern "C" int64_t b2k_launch_count(void) { return (int64_t)g_launches.load(); }
-extern "C" int b2k_set_variant(int v)
-{
-    if (v < 0 || v > 4) { b2k_set_error("b2k_set_variant: variant must be 0..4"); return B2K_ERR_INVALID; }
-    g_variant.store(v);
-    return B2K_OK;
-}
 
 // ------------------------------------------------------------------ validation helpers
 // q_on_device: the pointer is read by a kernel (element-wise at worst: only the natural alignment of the element
@@ -171,8 +154,6 @@ static int fkj_dispatch(const char *fn, b2k_chain_t c, int dtype, int mode, cons
     if (N == 0) return B2K_OK;
     B2K_ON_DEVICE_OF(q);
     cudaStream_t st = (cudaStream_t)stream;
-    if (b2k_get_variant() == 1 && !(mode & FKJ_JE))
-        return b2k_fkw_launch(c, dtype, mode, q, N, ldq, base, tool, T, J, st);
     if (dtype == B2K_F64) return b2k_fkj_launch_f64(c, mode, q, N, ldq, base, tool, T, J, st);
     return b2k_fkj_launch_f32(c, mode, q, N, ldq, base, tool, T, J, st);
 }

@@ -10,9 +10,6 @@
 
 #define B2K_WARPS_PER_BLOCK 4
 #define B2K_THREADS (32 * B2K_WARPS_PER_BLOCK)
-#ifndef B2K_L2_PREFETCH_TILES
-#define B2K_L2_PREFETCH_TILES 4 // how many of a warp's tiles ahead its q block is prefetched into L2
-#endif
 
 // Structure classes of a folded SE(3) constant A = [Ra | ta] (exact 0/1 pattern tests on the
 // host, so the specialised device paths are bit-identical to the general product).
@@ -122,15 +119,12 @@ long long b2k_rne_spec_launch(const b2k_rne_s *r, int mode, int dtype, const voi
 void b2k_set_error(const char *fmt, ...);
 int b2k_cuda_fail(cudaError_t e, const char *what);
 void b2k_count_launch(int n = 1);
-int b2k_get_variant();
 int b2k_num_sms(int *device_out = nullptr);
 // resident blocks per SM for (kernel, threads, dynamic smem), cached; also raises the kernel's
 // dynamic shared-memory limit.  <0 on CUDA error.
 int b2k_blocks_per_sm(const void *func, int threads, size_t smem);
 // once per device: keep freed stream-ordered allocations cached in the default memory pool
 void b2k_keep_mempool();
-// consecutive 32-row tiles one warp processes (tunable through env B2K_TPW_POSE / B2K_TPW_JAC for experiments)
-int b2k_tiles_per_warp(bool with_jacobian);
 
 #define B2K_CUDA(call)                                   \
     do {                                                 \

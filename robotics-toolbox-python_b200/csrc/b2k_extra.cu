@@ -539,13 +539,6 @@ __global__ void __launch_bounds__(128) k_singular(const real *__restrict__ J, lo
     m[row] = kind == 0 ? smin : (smax > 0 ? smin / smax : (real)0);
 }
 
-// B2K_HESSIAN_LUT=1 keeps every call on the warp-per-row kernel (measurement / tests of that path)
-static bool hessian_lut_only()
-{
-    static const bool v = [] { const char *e = getenv("B2K_HESSIAN_LUT"); return e && atoi(e) != 0; }();
-    return v;
-}
-
 template <typename real>
 static int extra_launch(int what, int n, const void *J, long long N, unsigned axes_mask, void *out, cudaStream_t st,
                         const void *aux = nullptr)
@@ -558,7 +551,7 @@ static int extra_launch(int what, int n, const void *J, long long N, unsigned ax
             /* index table is set up once per ~200 rows                                                             */ \
             const long long cap = (long long)b2k_num_sms() * (what == 0 ? 4 : 16);                                    \
             if (blocks > cap) blocks = cap;                                                                           \
-            if (what == 0 && NN >= 3 && ((uintptr_t)out & 15) == 0 && !hessian_lut_only() &&                          \
+            if (what == 0 && NN >= 3 && ((uintptr_t)out & 15) == 0 &&                                                \
                 b2k_blocks_per_sm((const void *)k_hessian_tile<real, NN>, 128, HessTile<real, NN>::SMEM) >= 1)         \
                 k_hessian_tile<real, NN><<<(unsigned)((N + 31) / 32), 128, HessTile<real, NN>::SMEM, st>>>((const real *)J, N, (real *)out); \
             else if (what == 0) k_hessian<real, NN><<<(unsigned)blocks, 256, 0, st>>>((const real *)J, N, (real *)out, (int)(((uintptr_t)out & (2 * sizeof(real) - 1)) == 0)); \

@@ -392,11 +392,10 @@ struct TileStage {
     }
 
     // Asynchronous drain through the TMA engine (cp.async.bulk shared -> global): no LDS/STG
-    // instructions, no registers, and the warp moves on to its next tile while the copy is in
-    // flight.  Exact-image stages go out as ONE bulk copy issued by lane 0; padded stages as one
-    // bulk copy per row issued by the lane that owns the row.  Returns false when this tile cannot
-    // use bulk copies (size / alignment not a multiple of 16 bytes): caller falls back to drain().
-    // Call wait_reads() before the stage is written again.
+    // instructions and no registers.  Exact-image stages go out as ONE bulk copy issued by lane 0;
+    // padded stages as one bulk copy per row issued by the lane that owns the row.  Returns false
+    // when this tile cannot use bulk copies (size / alignment not a multiple of 16 bytes): caller
+    // falls back to drain().  Call wait_all() before the warp exits.
     static __device__ __forceinline__ bool drain_async(unsigned char *stage, real *gout, int rows_here, int lane)
     {
         if constexpr (EXACT) {
@@ -424,12 +423,6 @@ struct TileStage {
         } else {
             return false;
         }
-    }
-    // every lane's outstanding bulk copies have finished READING shared memory
-    static __device__ __forceinline__ void wait_reads()
-    {
-        asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-        __syncwarp();
     }
     static __device__ __forceinline__ void wait_all()
     {
@@ -507,7 +500,7 @@ __device__ __forceinline__ void store_pose_row(const Pose<real> &T, real *grow)
 
 // ------------------------------------------------------------------ q tile loading
 // qmode 1: the smem tile is the exact image of the 32 x ldq global block, filled with 16-byte
-//          cp.async (no registers, asynchronous: used to prefetch the next tile);
+//          cp.async (no registers);
 // qmode 0: padded rows (stride ldq|1), element-wise copy -- used when the exact image would make
 //          the one-row-per-lane reads collide (gcd(ldq, banks) > 2) or q is not 16-byte aligned.
 __device__ __forceinline__ void cp_async16(void *smem, const void *gmem)
@@ -541,28 +534,13 @@ __device__ __forceinline__ void load_q_tile(real *sq, const real *__restrict__ g
     }
 }
 
-// Under a saturated write stream a DRAM read waits far longer than one tile's worth of work
-// (ncu: the warps' top stall was the cp.async wait), so the q block of a
-// tile further ahead is pulled into L2 with fire-and-forget prefetches; the cp.async that later
-// stages it into shared memory is then an L2 hit.  Costs one instruction, no registers, no smem.
-template <typename real>
-__device__ __forceinline__ void prefetch_q_tile_l2(const real *gq, int rows_here, int ldq, int lane)
-{
-    const char *p = reinterpret_cast<const char *>(gq);
-    const char *first = reinterpret_cast<const char *>(reinterpret_cast<uintptr_t>(p) & ~(uintptr_t)127);
-    const char *end = p + (size_t)rows_here * ldq * sizeof(real);
-    for (const char *a = first + (size_t)lane * 128; a < end; a += 32 * 128)
-        asm volatile("prefetch.global.L2 [%0];" ::"l"(a));
-}
-
-// bytes of per-warp shared memory: [q tile][output stage]
+// bytes of per-warp shared memory: [q tile][output stage]; the pose block is stored straight from registers
 template <typename real>
 inline size_t fkj_q_bytes(int ldq) { return ((size_t)32 * (ldq | 1) * sizeof(real) + 15) & ~(size_t)15; }
 
 template <typename real, int N>
-inline size_t fkj_warp_smem(int ldq, bool wt, bool wj)
+inline size_t fkj_warp_smem(int ldq, bool wj)
 {
-    (void)wt; // the pose block is stored straight from registers
     size_t j = wj ? (size_t)TileStage<real, 6 * N>::BYTES : 0;
     return fkj_q_bytes<real>(ldq) + j;
 }
@@ -578,100 +556,48 @@ template <typename real, int N, bool WT, bool WJ, int PROF>
 __global__ void __launch_bounds__(B2K_THREADS, FkjBounds<real, N, WJ>::MINB)
 k_fkj_forward(const __grid_constant__ ChainP<real, N> P, const real *__restrict__ q, long long nrows, int ldq,
               float inv_ldq, int qmode, real *__restrict__ Tout, real *__restrict__ Jout, int warp_smem_bytes,
-              int q_bytes, int tpw, int dbg)
+              int q_bytes)
 {
-    // dbg (measurement skeletons, b2k_set_variant 2 / 3): bit 0 = skip the chain walk (memory
-    // traffic only), bit 1 = skip the output stores (arithmetic only).  0 in normal operation.
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int lane = threadIdx.x & 31;
     const int warp = threadIdx.x >> 5;
+    const long long tile = (long long)blockIdx.x * B2K_WARPS_PER_BLOCK + warp;
+    const long long row0 = tile << 5;
+    if (row0 >= nrows) return;
+    const int rows_here = (int)((nrows - row0) < 32 ? (nrows - row0) : 32);
     unsigned char *wbase = smem_raw + (size_t)warp * warp_smem_bytes;
     real *sq = reinterpret_cast<real *>(wbase);
     unsigned char *so = wbase + q_bytes;
     const int ldqs = qmode ? ldq : (ldq | 1);
-    const long long ntiles = (nrows + 31) >> 5;
-    // a warp owns `tpw` CONSECUTIVE tiles (one-shot grid: tpw small; persistent measurement variant: all of its share)
-    const long long tstride = 1;
-    long long tile = ((long long)blockIdx.x * B2K_WARPS_PER_BLOCK + warp) * tpw;
-    const long long tile_end = (tile + tpw < ntiles) ? tile + tpw : ntiles;
-    if (tile < tile_end) {
-        const long long row0 = tile << 5;
-        load_q_tile<real>(sq, q + row0 * ldq, (int)((nrows - row0) < 32 ? (nrows - row0) : 32), ldq, inv_ldq, qmode, lane);
-#pragma unroll
-        for (int k = 1; k < B2K_L2_PREFETCH_TILES; k++) {
-            const long long ft = tile + k * tstride;
-            if (ft < tile_end) {
-                const long long r0 = ft << 5;
-                prefetch_q_tile_l2<real>(q + r0 * ldq, (int)((nrows - r0) < 32 ? (nrows - r0) : 32), ldq, lane);
-            }
-        }
-    }
-    for (; tile < tile_end; tile += tstride) {
-        const long long row0 = tile << 5;
-        const int rows_here = (int)((nrows - row0) < 32 ? (nrows - row0) : 32);
-        cp_async_wait_all();
-        __syncwarp();
-        const real *myq = sq + (lane < rows_here ? lane : 0) * ldqs;
-
-        Pose<real> T;
-        real zj[WJ ? N : 1][3], pj[WJ ? N : 1][3];
-        real qrow[N];
-#pragma unroll
-        for (int j = 0; j < N; j++) qrow[j] = myq[P.jidx[j]];
-        __syncwarp(); // every lane holds its q row in registers: prefetch the next tile's q now
-        {
-            const long long nt = tile + tstride;
-            if (nt < tile_end) {
-                const long long r0 = nt << 5;
-                load_q_tile<real>(sq, q + r0 * ldq, (int)((nrows - r0) < 32 ? (nrows - r0) : 32), ldq, inv_ldq, qmode, lane);
-            }
-            const long long ft = tile + B2K_L2_PREFETCH_TILES * tstride;
-            if (ft < tile_end) {
-                const long long r0 = ft << 5;
-                prefetch_q_tile_l2<real>(q + r0 * ldq, (int)((nrows - r0) < 32 ? (nrows - r0) : 32), ldq, lane);
-            }
-        }
-        if (dbg & 1) { // memory skeleton: fabricate outputs from q without walking the chain
-            pose_from_const(T, P.A[0]);
-            T.p[0] = qrow[0];
-            if (WJ) {
-#pragma unroll
-                for (int j = 0; j < N; j++)
-#pragma unroll
-                    for (int i = 0; i < 3; i++) { zj[j][i] = qrow[j]; pj[j][i] = qrow[(j + i) % N]; }
-            }
-        } else {
-            chain_forward<real, N, WJ, PROF>(P, [&](int j, int) { return qrow[j]; }, T, zj, pj);
-        }
-        if (dbg & 2) { // arithmetic skeleton: keep the results alive without writing them
-            real acc = T.p[0] + T.c0[0] + T.c1[1] + T.c2[2] + T.p[1] + T.p[2];
-            if (WJ) {
-#pragma unroll
-                for (int j = 0; j < N; j++) acc += zj[j][0] * pj[j][1] + zj[j][1] * pj[j][2] + zj[j][2] * pj[j][0];
-            }
-            if (acc == (real)123456.789) Tout[row0] = acc;
-            continue;
-        }
-        if (WT) {
-            Pose<real> Tb = T;
-            if (P.has_base) pose_mul_const_left(Tb, P.B, AK_GEN | AK_TX | AK_TY | AK_TZ);
-            if (lane < rows_here) store_pose_row<real>(Tb, Tout + (row0 + lane) * 16);
-        }
-        if (WJ) {
-            typedef TileStage<real, 6 * N> JS;
-            real row[6 * N];
-            jacob0_row<real, N, PROF>(P, T, zj, pj, row);
-            JS::wait_reads(); // the previous tile's bulk copy has finished reading the stage
-            JS::put_row(so, lane, row);
-            if (!JS::drain_async(so, Jout + row0 * (6 * N), rows_here, lane)) {
-                __syncwarp();
-                JS::drain(so, Jout + row0 * (6 * N), rows_here, lane);
-                __syncwarp();
-            }
-        }
-    }
+    load_q_tile<real>(sq, q + row0 * ldq, rows_here, ldq, inv_ldq, qmode, lane);
     cp_async_wait_all();
-    if (WJ) TileStage<real, 6 * N>::wait_all();
+    __syncwarp();
+    const real *myq = sq + (lane < rows_here ? lane : 0) * ldqs;
+
+    Pose<real> T;
+    real zj[WJ ? N : 1][3], pj[WJ ? N : 1][3];
+    real qrow[N];
+#pragma unroll
+    for (int j = 0; j < N; j++) qrow[j] = myq[P.jidx[j]];
+    chain_forward<real, N, WJ, PROF>(P, [&](int j, int) { return qrow[j]; }, T, zj, pj);
+    if (WT) {
+        Pose<real> Tb = T;
+        if (P.has_base) pose_mul_const_left(Tb, P.B, AK_GEN | AK_TX | AK_TY | AK_TZ);
+        if (lane < rows_here) store_pose_row<real>(Tb, Tout + (row0 + lane) * 16);
+    }
+    if (WJ) {
+        typedef TileStage<real, 6 * N> JS;
+        real row[6 * N];
+        jacob0_row<real, N, PROF>(P, T, zj, pj, row);
+        JS::put_row(so, lane, row);
+        real *gout = Jout + row0 * (6 * N);
+        if (!JS::drain_async(so, gout, rows_here, lane)) {
+            __syncwarp();
+            JS::drain(so, gout, rows_here, lane);
+        } else {
+            JS::wait_all(); // the bulk copy reads this warp's shared memory: it must finish before the block may retire
+        }
+    }
 }
 
 // Backward walk of a DH-like chain (unflipped Rz joints, Rx-form inter-joint constants): U starts at the tail
@@ -706,8 +632,8 @@ __device__ __forceinline__ void backward_walk_dh(const ChainP<real, N> &P, const
 }
 
 // ------------------------------------------------------------------ forward walk, lean form for the common call
-// k_fkj_forward above is general: any row stride / jindex permutation / alignment, ragged tiles, several tiles per
-// warp, measurement skeletons.  ncu on the pose-only fp32 kernel showed what that
+// k_fkj_forward above is general: any row stride / jindex permutation / alignment, ragged tiles.  ncu on the
+// pose-only fp32 kernel showed what that
 // generality costs on a one-shot grid, where every warp pays the prologue for a single tile: ~300 of 714 issued
 // instructions per tile were integer / control (IMAD, ISETP, LOP3, BRA, BSSY ...), and the kernel was issue-bound.
 // This kernel is the same walk with everything about the call fixed at compile time: DH-like chain (PROF 1),
@@ -847,85 +773,66 @@ template <typename real, int N, bool WT, int PROF>
 __global__ void __launch_bounds__(B2K_THREADS, FkjBounds<real, N, true>::MINB)
 k_fkj_backward(const __grid_constant__ ChainP<real, N> P, const real *__restrict__ q, long long nrows, int ldq,
                float inv_ldq, int qmode, real *__restrict__ Tout, real *__restrict__ Jout, int warp_smem_bytes,
-               int q_bytes, int tpw)
+               int q_bytes)
 {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int lane = threadIdx.x & 31;
     const int warp = threadIdx.x >> 5;
+    const long long tile = (long long)blockIdx.x * B2K_WARPS_PER_BLOCK + warp;
+    const long long row0 = tile << 5;
+    if (row0 >= nrows) return;
+    const int rows_here = (int)((nrows - row0) < 32 ? (nrows - row0) : 32);
     unsigned char *wbase = smem_raw + (size_t)warp * warp_smem_bytes;
     real *sq = reinterpret_cast<real *>(wbase);
     unsigned char *so = wbase + q_bytes;
     const int ldqs = qmode ? ldq : (ldq | 1);
-    const long long ntiles = (nrows + 31) >> 5;
-    // a warp owns `tpw` CONSECUTIVE tiles (one-shot grid: tpw small; persistent measurement variant: all of its share)
-    const long long tstride = 1;
-    long long tile = ((long long)blockIdx.x * B2K_WARPS_PER_BLOCK + warp) * tpw;
-    const long long tile_end = (tile + tpw < ntiles) ? tile + tpw : ntiles;
-    if (tile < tile_end) {
-        const long long row0 = tile << 5;
-        load_q_tile<real>(sq, q + row0 * ldq, (int)((nrows - row0) < 32 ? (nrows - row0) : 32), ldq, inv_ldq, qmode, lane);
-    }
-    for (; tile < tile_end; tile += tstride) {
-        const long long row0 = tile << 5;
-        const int rows_here = (int)((nrows - row0) < 32 ? (nrows - row0) : 32);
-        cp_async_wait_all();
-        __syncwarp();
-        const real *myq = sq + (lane < rows_here ? lane : 0) * ldqs;
-
-        Pose<real> U;
-        real row[6 * N]; // Je, row-major 6 x N
-        pose_from_const(U, P.A[N]);
-        if constexpr (PROF == 1) { // DH-like chain: straight-line walk, batched sincos
-            real eta[N];
-#pragma unroll
-            for (int j = 0; j < N; j++) eta[j] = myq[P.jidx[j]];
-            backward_walk_dh<real, N>(P, eta, U, row);
-        } else {
-#pragma unroll
-            for (int j = N - 1; j >= 0; j--) {
-                const int ax = P.axis[j];
-                const real sg = P.flip[j] ? (real)-1 : (real)1;
-                real col[6];
-                switch (ax) {
-                case B2K_RX: je_col_rev<real, 0>(U, sg, col); break;
-                case B2K_RY: je_col_rev<real, 1>(U, sg, col); break;
-                case B2K_RZ: je_col_rev<real, 2>(U, sg, col); break;
-                case B2K_TX: je_col_pri<real, 0>(U, sg, col); break;
-                case B2K_TY: je_col_pri<real, 1>(U, sg, col); break;
-                default: je_col_pri<real, 2>(U, sg, col); break;
-                }
-#pragma unroll
-                for (int k = 0; k < 6; k++) row[k * N + j] = col[k];
-                pose_joint_left(U, ax, sg * myq[P.jidx[j]], P.trig);
-                pose_mul_const_left(U, P.A[j], P.akind[j]);
-            }
-        }
-        __syncwarp();
-        {
-            const long long nt = tile + tstride;
-            if (nt < tile_end) {
-                const long long r0 = nt << 5;
-                load_q_tile<real>(sq, q + r0 * ldq, (int)((nrows - r0) < 32 ? (nrows - r0) : 32), ldq, inv_ldq, qmode, lane);
-            }
-        }
-        if (WT) {
-            Pose<real> Tb = U;
-            if (P.has_base) pose_mul_const_left(Tb, P.B, AK_GEN | AK_TX | AK_TY | AK_TZ);
-            if (lane < rows_here) store_pose_row<real>(Tb, Tout + (row0 + lane) * 16);
-        }
-        {
-            typedef TileStage<real, 6 * N> JS;
-            JS::wait_reads();
-            JS::put_row(so, lane, row);
-            if (!JS::drain_async(so, Jout + row0 * (6 * N), rows_here, lane)) {
-                __syncwarp();
-                JS::drain(so, Jout + row0 * (6 * N), rows_here, lane);
-                __syncwarp();
-            }
-        }
-    }
+    load_q_tile<real>(sq, q + row0 * ldq, rows_here, ldq, inv_ldq, qmode, lane);
     cp_async_wait_all();
-    TileStage<real, 6 * N>::wait_all();
+    __syncwarp();
+    const real *myq = sq + (lane < rows_here ? lane : 0) * ldqs;
+
+    Pose<real> U;
+    real row[6 * N]; // Je, row-major 6 x N
+    pose_from_const(U, P.A[N]);
+    if constexpr (PROF == 1) { // DH-like chain: straight-line walk, batched sincos
+        real eta[N];
+#pragma unroll
+        for (int j = 0; j < N; j++) eta[j] = myq[P.jidx[j]];
+        backward_walk_dh<real, N>(P, eta, U, row);
+    } else {
+#pragma unroll
+        for (int j = N - 1; j >= 0; j--) {
+            const int ax = P.axis[j];
+            const real sg = P.flip[j] ? (real)-1 : (real)1;
+            real col[6];
+            switch (ax) {
+            case B2K_RX: je_col_rev<real, 0>(U, sg, col); break;
+            case B2K_RY: je_col_rev<real, 1>(U, sg, col); break;
+            case B2K_RZ: je_col_rev<real, 2>(U, sg, col); break;
+            case B2K_TX: je_col_pri<real, 0>(U, sg, col); break;
+            case B2K_TY: je_col_pri<real, 1>(U, sg, col); break;
+            default: je_col_pri<real, 2>(U, sg, col); break;
+            }
+#pragma unroll
+            for (int k = 0; k < 6; k++) row[k * N + j] = col[k];
+            pose_joint_left(U, ax, sg * myq[P.jidx[j]], P.trig);
+            pose_mul_const_left(U, P.A[j], P.akind[j]);
+        }
+    }
+    if (WT) {
+        Pose<real> Tb = U;
+        if (P.has_base) pose_mul_const_left(Tb, P.B, AK_GEN | AK_TX | AK_TY | AK_TZ);
+        if (lane < rows_here) store_pose_row<real>(Tb, Tout + (row0 + lane) * 16);
+    }
+    typedef TileStage<real, 6 * N> JS;
+    JS::put_row(so, lane, row);
+    real *gout = Jout + row0 * (6 * N);
+    if (!JS::drain_async(so, gout, rows_here, lane)) {
+        __syncwarp();
+        JS::drain(so, gout, rows_here, lane);
+    } else {
+        JS::wait_all();
+    }
 }
 
 // ------------------------------------------------------------------ launcher
@@ -951,43 +858,30 @@ int fkj_launch_n(const b2k_chain_s *c, int mode, const real *q, long long nrows,
     // pose-only: base folded into the first constant; fused: base applied to the pose at the end
     b2k_fill_chain<real, N>(c, base, tool, /*base_into_chain=*/(wt && !wj0 && !wje), P);
     const size_t qb = fkj_q_bytes<real>(ldq);
-    const size_t wsm = (fkj_warp_smem<real, N>(ldq, wt, wj0 || wje) + 15) & ~(size_t)15;
+    const size_t wsm = (fkj_warp_smem<real, N>(ldq, wj0 || wje) + 15) & ~(size_t)15;
     const size_t smem = wsm * B2K_WARPS_PER_BLOCK;
     const float inv_ldq = 1.0f / (float)ldq;
     // (the caller, fkj_dispatch, has checked that T is 32-byte aligned and J aligned to TileStage<real, 6 * N>::UB)
 
-    const int variant = b2k_get_variant();
-    const int dbg = variant == 2 ? 1 : (variant == 3 ? 2 : 0);
-    auto launch_impl = [&](auto kern, auto... extra) -> int {
+    // One tile per warp on a one-shot grid: the hardware block scheduler hands out row ranges in address order as SMs
+    // free up, which keeps the set of DRAM pages being written compact.  A persistent grid measured lower write
+    // bandwidth for this store pattern.
+    auto launch = [&](auto kern) -> int {
         // (q, nrows, T, J are read here, at launch time: the lean path below may have advanced them to the ragged tail)
         const long long ntiles = (nrows + 31) / 32;
-        const long long nblk_needed = (ntiles + B2K_WARPS_PER_BLOCK - 1) / B2K_WARPS_PER_BLOCK;
+        const long long grid = (ntiles + B2K_WARPS_PER_BLOCK - 1) / B2K_WARPS_PER_BLOCK;
+        if (grid > 0x7fffffffLL) { b2k_set_error("fkj: batch too large for one launch"); return B2K_ERR_INVALID; }
         const int qmode = fkj_qmode<real>(q, ldq);
         int per_sm = b2k_blocks_per_sm((const void *)kern, B2K_THREADS, smem);
         if (per_sm < 1) return per_sm < 0 ? per_sm : (b2k_set_error("fkj kernel does not fit on an SM (smem %zu B)", smem), B2K_ERR_INVALID);
-        // One-shot grid, a few consecutive tiles per warp: the hardware block scheduler hands out
-        // row ranges in address order as SMs free up, which keeps the set of DRAM pages being
-        // written compact.  A persistent grid (variant 4) measured lower write bandwidth for this
-        // store pattern.
-        long long tpw = b2k_tiles_per_warp(wj0 || wje);
-        if (variant == 4) { // persistent: as many blocks as fit, each warp a contiguous share of the tiles
-            long long g = (long long)b2k_num_sms() * per_sm;
-            if (g > nblk_needed) g = nblk_needed;
-            tpw = (ntiles + g * B2K_WARPS_PER_BLOCK - 1) / (g * B2K_WARPS_PER_BLOCK);
-        }
-        long long grid = (ntiles + B2K_WARPS_PER_BLOCK * tpw - 1) / (B2K_WARPS_PER_BLOCK * tpw);
-        if (grid < 1) grid = 1;
-        if (grid > 0x7fffffffLL || tpw > 0x7fffffffLL) { b2k_set_error("fkj: batch too large for one launch"); return B2K_ERR_INVALID; }
-        kern<<<(unsigned)grid, B2K_THREADS, smem, st>>>(P, q, nrows, ldq, inv_ldq, qmode, T, J, (int)wsm, (int)qb, (int)tpw, extra...);
+        kern<<<(unsigned)grid, B2K_THREADS, smem, st>>>(P, q, nrows, ldq, inv_ldq, qmode, T, J, (int)wsm, (int)qb);
         b2k_count_launch();
         B2K_CUDA(cudaGetLastError());
         return B2K_OK;
     };
-    auto launch = [&](auto kern) -> int { return launch_impl(kern, dbg); };   // forward kernels take dbg
-    auto launch_b = [&](auto kern) -> int { return launch_impl(kern); };      // backward kernels do not
 
     // Lean kernel for the common call (see k_fkj_fast): full tiles there, a ragged tail through the general kernel.
-    if (c->dh_like && c->dense_jindex && ldq == N && variant == 0 && !(((uintptr_t)q) & 15) && nrows >= 32 &&
+    if (c->dh_like && c->dense_jindex && ldq == N && !(((uintptr_t)q) & 15) && nrows >= 32 &&
         nrows / 32 <= 0x7fffffffLL / 2) {
         const int nfull = (int)(nrows / 32);
         auto launch_fast = [&](auto kern, size_t fsmem) -> int {
@@ -1015,8 +909,8 @@ int fkj_launch_n(const b2k_chain_s *c, int mode, const real *q, long long nrows,
         nrows -= done;
     }
     if (wje) {
-        if (c->dh_like) return wt ? launch_b(k_fkj_backward<real, N, true, 1>) : launch_b(k_fkj_backward<real, N, false, 1>);
-        return wt ? launch_b(k_fkj_backward<real, N, true, 0>) : launch_b(k_fkj_backward<real, N, false, 0>);
+        if (c->dh_like) return wt ? launch(k_fkj_backward<real, N, true, 1>) : launch(k_fkj_backward<real, N, false, 1>);
+        return wt ? launch(k_fkj_backward<real, N, true, 0>) : launch(k_fkj_backward<real, N, false, 0>);
     }
     if (c->dh_like) {
         if (wt && wj0) return launch(k_fkj_forward<real, N, true, true, 1>);

@@ -862,12 +862,10 @@ int ik_launch_n(const b2k_chain_s *c, const real *Tep, long long nprob, const re
     // first search of every problem (one lane each); phase B runs the restarts of the problems that
     // failed it with B2K_IK_GROUP lanes per problem.  Scratch (hard list + counter) is stream-ordered.
     constexpr int G = 8;
-    const bool two_phase = slimit > 1 && nprob >= 1024 && b2k_get_variant() != 4;
-    // first-search scheduling (B2K_IK_MODE, default 2): 0 = persistent lanes pulling problems, 1 = one problem per lane,
-    // 2 = one problem per lane in two segments (IK_SEG1 evaluations, then the rest for the problems still running)
-    static const int mode_env = getenv("B2K_IK_MODE") ? atoi(getenv("B2K_IK_MODE")) : 2;
-    const int mode = two_phase ? mode_env : 0;
-    static const int IK_SEG1 = getenv("B2K_IK_SEG1") ? atoi(getenv("B2K_IK_SEG1")) : 10; // evaluations in the first segment
+    const bool two_phase = slimit > 1 && nprob >= 1024;
+    // first search: with two phases, one problem per lane in two segments (IK_SEG1 evaluations, then the rest for the
+    // problems still running); otherwise persistent lanes pulling problems
+    constexpr int IK_SEG1 = 10;
     int *scratch = nullptr;
     if (two_phase) {
         b2k_keep_mempool(); // do not hand the pool's memory back to the OS at every synchronisation
@@ -885,9 +883,9 @@ int ik_launch_n(const b2k_chain_s *c, const real *Tep, long long nprob, const re
         if (per_sm < 1) return per_sm < 0 ? per_sm : (b2k_set_error("ik kernel does not fit on an SM"), B2K_ERR_INVALID);
         long long grid = (long long)b2k_num_sms() * per_sm;
         long long need = (nprob + B2K_THREADS - 1) / B2K_THREADS;
-        if (grid > need || mode >= 1) grid = need;
+        if (grid > need || two_phase) grid = need;
         if (grid < 1) grid = 1;
-        const bool seg = mode == 2 && ilimit > IK_SEG1 + 2;
+        const bool seg = two_phase && ilimit > IK_SEG1 + 2;
         go(kern, grid, P, K, Tep, q0, nprob, q_out, success, iterations, searches, residual, two_phase ? 1 : 0, hard_idx,
            hard_count, seg ? IK_SEG1 : 0, (const int *)nullptr, (const int *)nullptr, cont_idx, park_count);
         b2k_count_launch();
@@ -917,16 +915,15 @@ int ik_launch_n(const b2k_chain_s *c, const real *Tep, long long nprob, const re
     };
     int rc = c->dh_like ? launch_a(ik_kernel_a<real, N, 1, STEP, NS>()) : launch_a(ik_kernel_a<real, N, 0, STEP, NS>());
     if (rc == B2K_OK && two_phase) {
-        // B2K_IK_ROUNDS: 1 = a single round of 8-lane groups; 2 = 4 lanes for searches 1-4, then 8 lanes to the end;
-        // 3 (default) = 4 lanes, ONE batch of 8 lanes (searches 5-12), then whole warps (32 searches per batch) for the
-        // handful of problems still unsolved -- a protocol whose hardest problem needs 50 (or all 100) searches otherwise
-        // runs 6 (12) serial batches of 30 evaluations for a few dozen problems.
-        static const int rounds_env = getenv("B2K_IK_ROUNDS") ? atoi(getenv("B2K_IK_ROUNDS")) : 3;
+        // Restart rounds: 4 lanes (searches 1-4), ONE batch of 8 lanes (searches 5-12), then whole warps (32 searches
+        // per batch) for the handful of problems still unsolved -- a protocol whose hardest problem needs 50 (or all
+        // 100) searches otherwise runs 6 (12) serial batches of 30 evaluations for a few dozen problems.  A search
+        // limit too small for the earlier rounds starts with 8-lane groups, or keeps them to the end.
         constexpr int G1 = 4, G3 = 32;
-        if (rounds_env >= 2 && slimit > 1 + G1) {
+        if (slimit > 1 + G1) {
             rc = c->dh_like ? launch_b(ik_kernel_b<real, N, 1, G1, STEP, NS>(), G1, hard_idx, hard_count, 1, 1, cont_idx, cont_count)
                             : launch_b(ik_kernel_b<real, N, 0, G1, STEP, NS>(), G1, hard_idx, hard_count, 1, 1, cont_idx, cont_count);
-            if (rc == B2K_OK && rounds_env >= 3 && slimit > 1 + G1 + G) {
+            if (rc == B2K_OK && slimit > 1 + G1 + G) {
                 rc = c->dh_like ? launch_b(ik_kernel_b<real, N, 1, G, STEP, NS>(), G, cont_idx, cont_count, 1 + G1, 1, hard_idx, third_count)
                                 : launch_b(ik_kernel_b<real, N, 0, G, STEP, NS>(), G, cont_idx, cont_count, 1 + G1, 1, hard_idx, third_count);
                 if (rc == B2K_OK)

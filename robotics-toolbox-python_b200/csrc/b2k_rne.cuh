@@ -754,10 +754,6 @@ int rne_launch_n(const b2k_rne_s *r, const real *q, const real *qd, const real *
         int per_sm = b2k_blocks_per_sm((const void *)kern, B2K_THREADS, smem);
         if (per_sm < 1) return per_sm < 0 ? per_sm : (b2k_set_error("rne kernel does not fit on an SM"), B2K_ERR_INVALID);
         long long grid = nblk_needed; // one tile per warp, one-shot grid (see b2k_fkj.cuh launcher)
-        if (b2k_get_variant() == 4) {
-            grid = (long long)b2k_num_sms() * per_sm;
-            if (grid > nblk_needed) grid = nblk_needed;
-        }
         if (grid < 1) grid = 1;
         if constexpr (WRENCH) kern<<<(unsigned)grid, B2K_THREADS, smem, st>>>(P, q, qd, qdd, nrows, tau, wbase, (int)wsm, (int)inb, qmode);
         else kern<<<(unsigned)grid, B2K_THREADS, smem, st>>>(P, q, qd, qdd, nrows, tau, (int)wsm, (int)inb, qmode);

@@ -600,8 +600,7 @@ std::string build_source(const GenFn &gen, int n, int mode, int dtype, Program &
     // pipe for two cycles and the kernel is not bound by issue at this size) and a persistent grid-stride loop with
     // double-buffered tiles (fp32 equal, fp64 slower: the second buffer's registers spill).
     const bool light = mode == B2K_GEN_RNE || mode == B2K_GEN_GRAVLOAD || mode == B2K_GEN_ITORQUE || mode == B2K_GEN_RNE_WRENCH;
-    int tpw = (dtype == B2K_F32 && light) ? 2 : 1;
-    if (const char *e = getenv("B2K_RNE_SPEC_TPW")) tpw = atoi(e) > 0 ? atoi(e) : tpw;
+    const int tpw = (dtype == B2K_F32 && light) ? 2 : 1;
     p.tpw = tpw;
     p.smem = 4 * ((tpw > 1 ? 2 : 1) * p.nin * in_bytes + (size_t)32 * (p.nout + p.nout2) * es);
     if (p.smem > 220 * 1024) { p.why = "a tile of this operation does not fit the shared memory of an SM (" + std::to_string(p.smem) + " B)"; return std::string(); }
@@ -610,7 +609,6 @@ std::string build_source(const GenFn &gen, int n, int mode, int dtype, Program &
     const int want = light ? (es == 8 ? 5 : 8) : (es == 8 ? 2 : 3);
     if (minb > want) minb = want;
     if (minb < 1) minb = 1;
-    if (const char *e = getenv("B2K_RNE_SPEC_MINB")) minb = atoi(e) > 0 ? atoi(e) : minb;
     auto D = [&](const char *k, long long v) { defs.push_back(std::string("-D") + k + "=" + std::to_string(v)); };
     defs.push_back(std::string("-DREAL=") + (es == 8 ? "double" : "float"));
     D("REAL_IS_F64", es == 8);

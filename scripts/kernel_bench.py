@@ -23,7 +23,6 @@ ap.add_argument("--ik-rows", type=int, default=100_000)
 ap.add_argument("--steps", type=int, default=50)
 ap.add_argument("--warmup", type=int, default=10)
 ap.add_argument("--only", default="")
-ap.add_argument("--variant", type=int, default=0)
 args = ap.parse_args()
 try:
     PEAK = float(json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"])
@@ -31,8 +30,6 @@ except Exception:
     PEAK = 3350.0  # H100 SXM data sheet
 dev = torch.device("cuda", 0)
 torch.cuda.set_device(0)
-if args.variant:
-    rtb.set_variant(args.variant)
 
 
 def timeit(fn, nbuf):
@@ -97,6 +94,35 @@ for robot_name, robot in (("panda", rtb.models.Panda()), ("ur10", rtb.models.UR1
             report(f"jacob0_{tag}", timeit(lambda i: L.b2k_jacob0(ch, code, qs[i].data_ptr(), N, n, None, J.data_ptr(), st), nbuf), N, (n + 6 * n) * es)
         if want(f"jacobe_{tag}") and robot_name == "panda":
             report(f"jacobe_{tag}", timeit(lambda i: L.b2k_jacobe(ch, code, qs[i].data_ptr(), N, n, None, J.data_ptr(), st), nbuf), N, (n + 6 * n) * es)
+        del qs, T, J
+
+# The general kernels (k_fkj_forward / k_fkj_backward), which the cases above do not reach: Panda with q rows one wider
+# than the chain (the DH-like profile), and a 7-joint chain with Rx / Ry / prismatic joints (the generic profile).
+E = rtb.ET
+gen7 = rtb.ETS([E.tz(0.3), E.Rx(), E.ty(0.1), E.Ry(), E.tz(), E.tx(0.2), E.Rz(), E.Ry(), E.tx(), E.tz(0.1), E.Rx(),
+                E.tx(0.05)])
+rngg = np.random.default_rng(1)
+for fam, ets, ldq in (("panda_ldq8", rtb.models.Panda().ets(), 8), ("generic7", gen7, 7)):
+    n = ets.n
+    for dt in (np.float64, np.float32):
+        es = np.dtype(dt).itemsize
+        tag = f"{fam}_{'f64' if dt == np.float64 else 'f32'}"
+        if not (want(f"fkine_jacob0_{tag}") or want(f"jacobe_{tag}")):
+            continue
+        nbuf = min(8, max(2, int(np.ceil(300e6 / (N * ldq * es)))))
+        qs = [torch.from_numpy(rngg.uniform(-np.pi, np.pi, (N, ldq)).astype(dt)).to(dev) for _ in range(nbuf)]
+        T = torch.empty((N, 4, 4), dtype=tdt[dt], device=dev)
+        J = torch.empty((N, 6, n), dtype=tdt[dt], device=dev)
+        L = rtb._lib.lib()
+        ch = ets._chain
+        st = torch.cuda.current_stream().cuda_stream
+        code = rtb._lib.F64 if dt == np.float64 else rtb._lib.F32
+        if want(f"fkine_jacob0_{tag}"):
+            report(f"fkine_jacob0_{tag}", timeit(lambda i: rtb._lib.check(L.b2k_fkine_jacob0(ch, code, qs[i].data_ptr(), N, ldq, None, None, T.data_ptr(), J.data_ptr(), st)), nbuf),
+                   N, (ldq + 16 + 6 * n) * es)
+        if want(f"jacobe_{tag}"):
+            report(f"jacobe_{tag}", timeit(lambda i: rtb._lib.check(L.b2k_jacobe(ch, code, qs[i].data_ptr(), N, ldq, None, J.data_ptr(), st)), nbuf),
+                   N, (ldq + 6 * n) * es)
         del qs, T, J
 
 puma = rtb.models.Puma560()
@@ -310,16 +336,8 @@ if want("extra_"):
         ("extra_mtraj_trapezoidal_f64", lambda i: rtb.mtraj(rtb.trapezoidal, np.zeros(7), np.ones(7), NX, device=True), 21 * 8),
         ("extra_ctraj_f64", lambda i: rtb.ctraj(Tx[0].cpu().numpy(), Tx[1].cpu().numpy(), NX, device=True), 16 * 8),
         ("extra_fkine_all_panda_f64", lambda i: PD.fkine_all(Qx), (7 + 8 * 16) * 8),
-        ("extra_fkine_all_panda_f64_per_frame_launches", lambda i: fkine_all_per_frame(PD, Qx), (7 + 8 * 16) * 8),
     ]
     PD = rtb.models.DH.Panda()
-
-    def fkine_all_per_frame(robot, Q):  # the earlier route: one pose launch per frame over the prefix chains
-        rtb.ETS.frames_single_walk = False
-        try:
-            return robot.fkine_all(Q)
-        finally:
-            rtb.ETS.frames_single_walk = True
 
     for name, fn, bpr in cases:
         if not want(name):

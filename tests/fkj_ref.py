@@ -70,17 +70,16 @@ def compile_chain(desc):
                 q_width=max(jidx) + 1)
 
 
-def lean_eligible(c, ldq, q_ptr, nrows, variant=0):
+def lean_eligible(c, ldq, q_ptr, nrows):
     """fkj_launch_n's condition for the lean kernels (k_fkj_fast / k_fkj_back_fast) on the full tiles of a call."""
-    return bool(c["dh_like"] and c["dense_jindex"] and ldq == c["n"] and variant == 0 and q_ptr % 16 == 0
-                and nrows >= 32)
+    return bool(c["dh_like"] and c["dense_jindex"] and ldq == c["n"] and q_ptr % 16 == 0 and nrows >= 32)
 
 
-def expected_launches(c, ldq, q_ptr, nrows, variant=0):
+def expected_launches(c, ldq, q_ptr, nrows):
     """Kernel launches of one fkj call: the lean kernel plus the general kernel on a ragged tail, or one kernel."""
     if nrows == 0:
         return 0
-    if lean_eligible(c, ldq, q_ptr, nrows, variant):
+    if lean_eligible(c, ldq, q_ptr, nrows):
         return 1 + (nrows % 32 != 0)
     return 1
 
@@ -112,22 +111,19 @@ def _joint(axis, eta):
     return T
 
 
-def evaluate(desc, q, base=None, tool=None, batch_trig=None):
+def evaluate(desc, q, base=None, tool=None):
     """The five entry points' results on q (N, ldq), fp32 or fp64, exactly as the kernel reads it.
 
     Returns a dict of long-double arrays T (base @ pose @ tool), Tnb (without base), J0 (base-frame Jacobian, tool
     included, base not: RobotKinematics.py:158), Je (end-effector frame), and per row: L, angle (largest |sincos
-    argument|) and path (PATH_*: the sincos branch the kernel takes for the row).  batch_trig: the chain walk evaluates
-    its n sincos as one batch (b2k_sincos_batch: the DH-like profile of the FK kernels), default from the chain's
-    classification; False for kernels that call the scalar b2k_sincos per joint."""
+    argument|) and path (PATH_*: the sincos branch the kernel takes for the row).  The chain walk of a DH-like chain
+    evaluates its n sincos as one batch (b2k_sincos_batch); any other chain calls the scalar b2k_sincos per joint."""
     c = compile_chain(desc)
     n = c["n"]
     q = np.asarray(q)
     assert q.ndim == 2 and q.dtype in (np.float32, np.float64)
     N = q.shape[0]
     ql = q.astype(LD)
-    if batch_trig is None:
-        batch_trig = c["dh_like"]
     # constants folded in long double from the description's fp64 matrices
     consts, acc = [], np.eye(4, dtype=LD)
     for i in range(len(desc["isjoint"])):
@@ -167,7 +163,7 @@ def evaluate(desc, q, base=None, tool=None, batch_trig=None):
             J0[:, :3, j] = z[:, :, j]
     Rt = np.swapaxes(T[:, :3, :3], 1, 2)
     Je = np.concatenate([Rt @ J0[:, :3], Rt @ J0[:, 3:]], axis=1)
-    path, angle = sincos_path(np.stack(angles, 1) if angles else np.zeros((N, 0), LD), q.dtype, batch_trig)
+    path, angle = sincos_path(np.stack(angles, 1) if angles else np.zeros((N, 0), LD), q.dtype, c["dh_like"])
     return dict(T=B @ T, Tnb=T, J0=J0, Je=Je, L=L, path=path, angle=angle, chain=c)
 
 

@@ -8,9 +8,6 @@ guards untouched and no sentinel left in the outputs.  The largest error of each
 fraction of its bar, is printed at the end of the module (run with -s to see it).
 """
 import math
-import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -24,7 +21,6 @@ from oracle import chains as ch  # noqa: E402
 
 import fkj_ref as R  # noqa: E402
 
-ROOT = os.path.abspath(os.path.join(os.path.dirname(__file__), ".."))
 SENTINEL = {np.float64: (torch.int64, 0x7FF4DEADBEEF0BAD), np.float32: (torch.int32, 0x7FA0DEAD)}  # signalling NaNs
 GUARD = 64  # bytes of guard before and after every output
 ENTRIES = ("fkine", "jacob0", "jacobe", "fkine_jacob0", "fkine_jacobe")
@@ -90,7 +86,7 @@ def device_q(Q, qoff=0):
     return flat[qoff:qoff + Q.size]
 
 
-def call(chain, entry, Q, base=None, tool=None, qoff=0, joff=0, variant=0):
+def call(chain, entry, Q, base=None, tool=None, qoff=0, joff=0):
     """One C-ABI call; returns (T or None, J or None) on the host after checking the guards and the launch count."""
     L = rtb._lib.lib()
     dt = Q.dtype.type
@@ -117,9 +113,8 @@ def call(chain, entry, Q, base=None, tool=None, qoff=0, joff=0, variant=0):
     rtb._lib.check(rc)
     torch.cuda.synchronize()
     launches = rtb.launch_count() - n0
-    if variant == 0:
-        want = R.expected_launches(chain.c, ldq, qd.data_ptr(), N, variant)
-        assert launches == want, (entry, n, N, ldq, launches, want)
+    want = R.expected_launches(chain.c, ldq, qd.data_ptr(), N)
+    assert launches == want, (entry, n, N, ldq, launches, want)
     T = J = None
     if wt:
         check_guards(Tb[0], Tb[2], N * 16, dt, entry + " T")
@@ -410,75 +405,6 @@ def test_lean_and_general_kernels_agree(n):
             same = all(np.array_equal(x, y) for x, y in zip(lean, gen) if x is not None)
             REPORT[(np.dtype(dt).name, "lean==general", e)] = max(REPORT.get((np.dtype(dt).name, "lean==general", e), 0.0),
                                                                  0.0 if same else 1.0)
-
-
-# ------------------------------------------------------------------ several tiles per warp, measurement variants
-def _persistent_tpw(nrows):
-    """An upper bound of the grid of variant 4 (launch_impl: as many blocks as fit, each warp a contiguous share) and
-    the tiles per warp it gives: at most max-threads-per-SM / 128 blocks of 128 threads per SM."""
-    p = torch.cuda.get_device_properties(0)
-    g = p.multi_processor_count * (p.max_threads_per_multi_processor // 128)
-    ntiles = (nrows + 31) // 32
-    return (ntiles + g * 4 - 1) // (g * 4)
-
-
-@pytest.mark.parametrize("n", [1, 4, 7, 10])
-def test_persistent_grid_several_tiles_per_warp(n):
-    """set_variant(4) at 1M + 17 rows: every warp walks several consecutive tiles (next-tile q load, L2 prefetch)."""
-    N = (1 << 20) + 17
-    assert _persistent_tpw(N) > 1
-    rng = np.random.default_rng(130 + n)
-    rows = np.unique(np.r_[0:64, N - 64:N, rng.integers(0, N, 1024)])
-    rtb.set_variant(4)
-    try:
-        for desc, fam in ((R.dh_family(n, rng, "gen"), "v4-dh"), (R.generic_family(n, rng, []), "v4-generic")):
-            chain = Chain(desc)
-            for dt in (np.float64, np.float32):
-                Q = rand_q(rng, N, n, dt)
-                ref = R.evaluate(desc, Q[rows], BASE, TOOL)
-                for e in ("fkine_jacob0", "fkine_jacobe", "fkine"):
-                    T, J = call(chain, e, Q, BASE, TOOL, variant=4)
-                    check_entry((np.dtype(dt).name, fam), e, ref, T[rows], None if J is None else J[rows], dt)
-    finally:
-        rtb.set_variant(0)
-
-
-def tpw3_body():
-    """Run in a process started with B2K_TPW_POSE=3 B2K_TPW_JAC=3 (read once per process)."""
-    rng = np.random.default_rng(5)
-    for n in (2, 7, 10):
-        for desc, fam in ((R.generic_family(n, rng, []), "tpw3-generic"), (R.dh_family(n, rng, "gen"), "tpw3-tail")):
-            chain = Chain(desc)
-            for dt in (np.float64, np.float32):
-                for N in (32 * 4 * 3 * 5 + 17, 1000 + n):
-                    run_all(chain, fam, rand_q(rng, N, n, dt), BASE, TOOL)
-    print("TPW3_OK")
-
-
-def test_three_tiles_per_warp_in_the_default_variant():
-    env = dict(os.environ, B2K_TPW_POSE="3", B2K_TPW_JAC="3")
-    code = ("import sys; sys.path[:0] = [%r, %r]; import test_gpu_fkj_dispatch as t; t.tpw3_body()"
-            % (ROOT, os.path.join(ROOT, "tests")))
-    r = subprocess.run([sys.executable, "-c", code], env=env, capture_output=True, text=True, cwd=ROOT, timeout=600)
-    assert r.returncode == 0 and "TPW3_OK" in r.stdout, r.stdout[-3000:] + r.stderr[-3000:]
-
-
-@pytest.mark.parametrize("n", [6, 7])
-def test_warp_per_configuration_variant(n):
-    """set_variant(1): the warp-per-configuration walk (b2k_fkw.cu, built for n = 6 and 7 only) on a DH-like chain;
-    it calls the scalar sincos."""
-    rng = np.random.default_rng(150 + n)
-    chain = Chain(R.dh_family(n, rng, "gen"))
-    rtb.set_variant(1)
-    try:
-        for dt in (np.float64, np.float32):
-            Q = rand_q(rng, 77, n, dt)
-            for e, base in (("fkine", BASE), ("jacob0", None), ("fkine_jacob0", BASE)):
-                ref = R.evaluate(chain.desc, Q, base, TOOL, batch_trig=False)
-                T, J = call(chain, e, Q, base, TOOL, variant=1)
-                check_entry((np.dtype(dt).name, "variant1"), e, ref, T, J, dt)
-    finally:
-        rtb.set_variant(0)
 
 
 def test_public_ets_methods():

@@ -750,28 +750,6 @@ def test_full_size_ur10_fp32():
     np.testing.assert_allclose(host(J[idx]), C.jacob0(Qr), rtol=1e-4, atol=1e-5)
 
 
-def test_measurement_variants_are_correct():
-    """Variant 1 (literal warp-per-configuration walk) and variant 4 (persistent grid) compute the
-    same results as the default kernel; they exist so the design choices can be measured."""
-    e = rtb.models.Panda().ets()
-    C = orc.Chain(e.describe())
-    Q = np.random.default_rng(8).uniform(-np.pi, np.pi, (5003, 7))
-    base = ch.trotz(0.3) @ ch.transl(0.1, 0.2, 0.3)
-    tool = ch.trotx(-0.4) @ ch.transl(0.0, 0.1, 0.05)
-    try:
-        for v in (1, 4):
-            rtb.set_variant(v)
-            for dt in (np.float64, np.float32):
-                Qr = ref_inputs(Q, dt)
-                T, J = e.fkine_jacob0(dev(Q, dt), base=base, tool=tool)
-                np.testing.assert_allclose(host(T), C.fkine(Qr, base, tool), **TOL[dt])
-                np.testing.assert_allclose(host(J), C.jacob0(Qr, tool), **TOL[dt])
-                np.testing.assert_allclose(host(e.eval(dev(Q, dt), base=base)), C.fkine(Qr, base), **TOL[dt])
-                np.testing.assert_allclose(host(e.jacob0(dev(Q, dt))), C.jacob0(Qr), **TOL[dt])
-    finally:
-        rtb.set_variant(0)
-
-
 def test_launch_counter_moves():
     e = rtb.models.Panda().ets()
     n0 = rtb.launch_count()

@@ -234,13 +234,10 @@ def test_fdyn_device_integrator_follows_scipy_rk45():
         puma.fdyn(0.1, q0, solver="Radau")
 
 
-@pytest.mark.parametrize("single_walk", [True, False])
-def test_fkine_all_reference_literals_and_dh_link_products(single_walk, monkeypatch):
+def test_fkine_all_reference_literals_and_dh_link_products():
     """DHRobot.fkine_all (DHRobot.py:1018-1064): the literal frames of the reference's own test (tests/test_DHRobot.py:
     638-710, DH Panda at q = 1..7, 4 decimals) and, for batches, the running product base * A1 ... Ak of the DH link
     transforms restated independently in oracle/chains.py."""
-    # both routes: all frames from one walk (b2k_fkine_frames) / one pose launch per frame over prefix chains
-    monkeypatch.setattr(rtb.ETS, "frames_single_walk", single_walk)
     panda = rtb.models.DH.Panda()
     q = np.arange(1.0, 8.0)
     T = panda.fkine_all(q)
@@ -280,12 +277,9 @@ def test_fkine_all_reference_literals_and_dh_link_products(single_walk, monkeypa
         robot.base = None
 
 
-@pytest.mark.parametrize("single_walk", [True, False])
-def test_fkine_all_of_a_branched_urdf_robot(single_walk, monkeypatch):
+def test_fkine_all_of_a_branched_urdf_robot():
     """Robot.fkine_all (Robot.py:638-700): frame i = pose of link number i, every branch, static links included; each
     frame against the product of link.A(q) from the base link down (the reference's recursion)."""
-    # both routes: all frames from one walk (b2k_fkine_frames) / one pose launch per frame over prefix chains
-    monkeypatch.setattr(rtb.ETS, "frames_single_walk", single_walk)
     import os
 
     rob = rtb.Robot.URDF(os.path.join(os.path.dirname(__file__), "golden", "urdf", "two_arm.urdf"))
