@@ -192,6 +192,29 @@ int b2k_ikine_null(b2k_chain_t chain, int dtype, const void *Tep, int64_t N, con
                    const double *pi, void *q_out, int32_t *success, int32_t *iterations,
                    int32_t *searches, void *residual, void *stream);
 
+/* The Python solver loop of b2k_ik_lm (always B2K_IK_SEM_PYTHON) with the quadratic-programming step of the
+ * reference's IK_QP (ETS.ikine_QP), for 1 <= n <= 10.  Arguments as b2k_ik_lm without lambda, method and semantics
+ * (we weighs only the cost E), plus:
+ *   kj, ks  joint-velocity and slack gains (> 0)
+ *   kq      velocity-damper gain; > 0 turns the damper on
+ *   km      manipulability gain; > 0 turns the term on (needs n >= 6)
+ *   ps      scalar; pi  host n-vector, the influence distance of each joint's limits (read only when kq > 0)
+ * Every step, at the pre-step q with the unweighted angle-axis error e and the base-frame J, dq is the exact minimiser of
+ *   1/2 kj |dq|^2 + 1/2 w |s|^2 + c^T dq   subject to  J dq + s = e,   w = ks / sum|e|,  c = -[km > 0] jacobm(q) / km
+ * (jacobm as b2k_jacobm with all six axes) and, when kq > 0, one damper row per joint within pi_i of a limit:
+ *   -dq_i <= ((q_i - l_i) - ps) / ((pi_i - ps) kq)  if q_i - l_i <= pi_i
+ *    dq_i <= ((h_i - q_i) - ps) / ((pi_i - ps) kq)  if h_i - q_i <= pi_i (this row wins when both hold)
+ * with l, h the chain's joint limits in chain order; q <- q + dq.  A row with sum|e| = 0 steps by 0 (its E is 0).  A QP
+ * whose factorisation fails or that is not solved within 2n + 2 active-set rounds abandons the search.  Rejected
+ * before any CUDA call: what b2k_ik_lm rejects, non-finite kj, ks, kq, km or ps, kj <= 0 or ks <= 0, with kq > 0 a
+ * NULL or non-finite pi or ps == pi[i], and km > 0 with n < 6 (J J^T is singular there).
+ */
+int b2k_ikine_qp(b2k_chain_t chain, int dtype, const void *Tep, int64_t N, const void *q0,
+                 int ilimit, int slimit, double tol, int reject_jl, const double *we, uint64_t seed,
+                 int rng_per_row, double kj, double ks, double kq, double km, double ps, const double *pi,
+                 void *q_out, int32_t *success, int32_t *iterations, int32_t *searches, void *residual,
+                 void *stream);
+
 /* ---------------------------------------------------------------- inverse dynamics (DH RNE)
  * b2k_rne_create replaces frne.init (frne.c:233-299): n links, mdh = 0 standard / 1 modified
  * DH, L = 24 doubles per link packed as reference DHRobot.py:1340-1358

@@ -286,6 +286,15 @@ class DHRobot:
     def ik_GN(self, Tep, **kwargs):
         return self.ets().ik_GN(Tep, **kwargs)
 
+    def ikine_NR(self, Tep, **kwargs):
+        return self.ets().ikine_NR(Tep, **kwargs)
+
+    def ikine_GN(self, Tep, **kwargs):
+        return self.ets().ikine_GN(Tep, **kwargs)
+
+    def ikine_QP(self, Tep, **kwargs):
+        return self.ets().ikine_QP(Tep, **kwargs)
+
     # reference DHRobot.py:1923-2452: positional wrappers over the C++ solvers.  (In the reference they
     # forward to ETS methods of the same lower-case names, which ETS does not define; here they work.)
     def ik_lm_chan(self, Tep, q0=None, ilimit=30, slimit=100, tol=1e-6, reject_jl=True, we=None, λ=1.0):

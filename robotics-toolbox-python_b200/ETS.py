@@ -644,7 +644,7 @@ class ETS:
 
     # ------------------------------------------------------------------ inverse kinematics
     def _ik(self, Tep, q0, ilimit, slimit, tol, mask, joint_limits, k, method, seed, semantics, rng_per_row, dtype,
-            null=None):
+            null=None, qp=None):
         Tep = getattr(Tep, "A", Tep)
         B.check_numeric(Tep, "Tep")
         host = not B.is_tensor(Tep)
@@ -682,7 +682,13 @@ class ETS:
         E = B.empty((N,), dt, like=Td)
         if seed is None:
             seed = int(np.random.default_rng().integers(0, 2**63 - 1))
-        if null is None:
+        if qp is not None:  # the Python loop with the quadratic-programming step (semantics is SEM_PYTHON)
+            kj, ks, kq, km, ps, pi = qp
+            _lib.check(_lib.lib().b2k_ikine_qp(
+                self._chain, B.code(dt), B.ptr(Td), N, B.ptr(q0d), int(ilimit), int(slimit), float(tol),
+                int(bool(joint_limits)), _lib.dptr(we), int(seed) & (2**64 - 1), int(bool(rng_per_row)), kj, ks, kq, km,
+                ps, _lib.dptr(pi), B.ptr(q), B.ptr(succ), B.ptr(its), B.ptr(srch), B.ptr(E), B.stream_ptr(Td)))
+        elif null is None:
             _lib.check(_lib.lib().b2k_ik_lm(
                 self._chain, B.code(dt), B.ptr(Td), N, B.ptr(q0d), int(ilimit), int(slimit), float(tol),
                 int(bool(joint_limits)), _lib.dptr(we), float(k), meth, int(seed) & (2**64 - 1), semantics,
@@ -760,8 +766,12 @@ class ETS:
 
     def _ikine(self, meth, Tep, q0, ilimit, slimit, tol, mask, joint_limits, seed, k, kq, km, dtype, ps=0.0,
                pi=0.3) -> IKSolution:
-        q, s, it, sr, E, single = self._ik(Tep, q0, ilimit, slimit, tol, mask, joint_limits, k, meth, seed,
-                                           _lib.SEM_PYTHON, False, dtype, null=self._null_args(kq, km, ps, pi))
+        return self._ik_solution(self._ik(Tep, q0, ilimit, slimit, tol, mask, joint_limits, k, meth, seed,
+                                          _lib.SEM_PYTHON, False, dtype, null=self._null_args(kq, km, ps, pi)))
+
+    def _ik_solution(self, r) -> IKSolution:
+        """IKSolution of the Python solver loop from _ik's per-row results (IK.py:263-290)"""
+        q, s, it, sr, E, single = r
         if B.is_tensor(q):
             q, s, it, sr, E = (B.to_host(x) for x in (q, s, it, sr, E))
         fail = "iteration and search limit reached"
@@ -797,3 +807,37 @@ class ETS:
         :class:`IKSolution`; for an (N,4,4) trajectory q is (N,n), success is the conjunction,
         iterations / searches are summed and residual is the minimum (IK.py:263-290)."""
         return self._ikine(method, Tep, q0, ilimit, slimit, tol, mask, joint_limits, seed, k, kq, km, dtype, ps, pi)
+
+    def _qp_args(self, kj, ks, kq, km, ps, pi):
+        """(kj, ks, kq, km, ps, pi as an n-vector) for b2k_ikine_qp, after the checks DESIGN (f-11) lists"""
+        kj, ks, kq, km, ps = (float(x) for x in (kj, ks, kq, km, ps))
+        n = self.n
+        pa = np.asarray(pi, dtype=np.float64)
+        if pa.ndim == 0:
+            pa = np.full(n, float(pa))
+        elif pa.shape != (n,):
+            raise ValueError(f"pi must be a scalar or have {n} elements, got shape {pa.shape}")
+        pa = np.ascontiguousarray(pa)
+        if not all(np.isfinite(x) for x in (kj, ks, kq, km, ps)) or not np.isfinite(pa).all():
+            raise ValueError("kj, ks, kq, km, ps and pi must be finite")
+        if not (kj > 0 and ks > 0):
+            raise ValueError("kj and ks must be > 0: the step's quadratic form is not positive definite otherwise")
+        if kq > 0 and (pa == ps).any():
+            raise ValueError(f"ps == pi at joint {int(np.argmax(pa == ps))}: the velocity damper divides by pi - ps")
+        if km > 0 and n < 6:
+            raise ValueError(f"km > 0 needs at least 6 joints (n = {n}): J J^T is singular for fewer")
+        return kj, ks, kq, km, ps, pa
+
+    def ikine_QP(self, Tep, q0=None, ilimit: int = 30, slimit: int = 100, tol: float = 1e-6, mask=None,
+                 joint_limits: bool = True, seed: Optional[int] = None, kj: float = 1.0, ks: float = 1.0,
+                 kq: float = 0.0, km: float = 0.0, ps: float = 0.0, pi=0.3, dtype=None, **kwargs) -> IKSolution:
+        """Quadratic-programming IK with the semantics of the reference's Python solver class (ETS.ikine_QP ->
+        IK_QP): each step minimises 1/2 kj |dq|^2 + 1/2 w |s|^2 - [km > 0] jacobm(q)^T dq / km subject to
+        J dq + s = e, w = ks / sum|e|, and, with kq > 0, a velocity damper on every joint within pi of a limit:
+        dq_i <= ((h_i - q_i) - ps) / ((pi_i - ps) kq) or -dq_i <= ((q_i - l_i) - ps) / ((pi_i - ps) kq).  The QP is
+        solved exactly on the device (no qpsolvers / quadprog).  Same return convention as :meth:`ikine_LM`;
+        DESIGN (f-11) lists the deviations (bad gains raise ValueError, a QP the kernel cannot finish abandons the
+        search instead of ending the solve)."""
+        qp = self._qp_args(kj, ks, kq, km, ps, pi)
+        return self._ik_solution(self._ik(Tep, q0, ilimit, slimit, tol, mask, joint_limits, 0.0, 0, seed,
+                                          _lib.SEM_PYTHON, False, dtype, qp=qp))

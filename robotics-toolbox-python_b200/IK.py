@@ -93,3 +93,26 @@ class IK_GN(_IK_pinv):
     def solve(self, ets, Tep, q0=None) -> IKSolution:
         ets = ets.ets() if hasattr(ets, "ets") and callable(ets.ets) else ets
         return ets.ikine_GN(Tep, q0=q0, **self._args())
+
+
+class IK_QP:
+    """Quadratic-programming solver object (reference IK_QP, IK.py); ``solve`` runs the fused GPU kernel, each step's
+    QP solved exactly on the device (DESIGN (f-11))."""
+
+    def __init__(self, name: str = "IK Solver", ilimit: int = 30, slimit: int = 100, tol: float = 1e-6,
+                 mask=None, joint_limits: bool = True, seed: Optional[int] = None, kj: float = 1.0, ks: float = 1.0,
+                 kq: float = 0.0, km: float = 0.0, ps: float = 0.0, pi=0.3, **kwargs):
+        self.ilimit, self.slimit, self.tol = ilimit, slimit, tol
+        self.mask = mask
+        self.We = np.diag(np.ones(6) if mask is None else np.asarray(mask, dtype=float))
+        self.joint_limits = joint_limits
+        self.seed = seed
+        self.kj, self.ks = kj, ks
+        self.kq, self.km, self.ps, self.pi = kq, km, ps, pi
+        self.name = f"QP (kj={kj}, ks={ks})"
+
+    def solve(self, ets, Tep, q0=None) -> IKSolution:
+        ets = ets.ets() if hasattr(ets, "ets") and callable(ets.ets) else ets
+        return ets.ikine_QP(Tep, q0=q0, ilimit=self.ilimit, slimit=self.slimit, tol=self.tol, mask=self.mask,
+                            joint_limits=self.joint_limits, seed=self.seed, kj=self.kj, ks=self.ks, kq=self.kq,
+                            km=self.km, ps=self.ps, pi=self.pi)

@@ -387,6 +387,9 @@ class Robot:
     def ikine_GN(self, Tep, end=None, start=None, **kw):
         return self.ets(start, end).ikine_GN(Tep, **kw)
 
+    def ikine_QP(self, Tep, end=None, start=None, **kw):
+        return self.ets(start, end).ikine_QP(Tep, **kw)
+
     # ---- inverse dynamics of the tree (reference Robot.rne, Robot.py:1704-1903)
     def tree_description(self) -> dict:
         """The tree as Robot.rne walks it: links grouped so that static links travel with the next joint link in

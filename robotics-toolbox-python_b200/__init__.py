@@ -14,7 +14,7 @@ from . import _lib  # noqa: F401
 from ._lib import B2KError, launch_count, pinned_empty  # noqa: F401
 from ._se3 import SE3  # noqa: F401
 from .ET import ET  # noqa: F401
-from .IK import IK_GN, IK_LM, IK_NR, IKSolution  # noqa: F401
+from .IK import IK_GN, IK_LM, IK_NR, IK_QP, IKSolution  # noqa: F401
 from .ETS import ETS  # noqa: F401
 from .DHLink import DHLink, PrismaticDH, PrismaticMDH, RevoluteDH, RevoluteMDH  # noqa: F401
 from .DHRobot import DHRobot  # noqa: F401

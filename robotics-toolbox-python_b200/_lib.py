@@ -47,6 +47,8 @@ _PROTOS = {
     "b2k_ikine_null": (C.c_int, [vp, C.c_int, vp, i64, vp, C.c_int, C.c_int, C.c_double, C.c_int, dp, C.c_double,
                                  C.c_int, C.c_uint64, C.c_int, C.c_double, C.c_double, C.c_double, dp, vp, vp, vp, vp, vp,
                                  vp]),
+    "b2k_ikine_qp": (C.c_int, [vp, C.c_int, vp, i64, vp, C.c_int, C.c_int, C.c_double, C.c_int, dp, C.c_uint64, C.c_int,
+                               C.c_double, C.c_double, C.c_double, C.c_double, C.c_double, dp, vp, vp, vp, vp, vp, vp]),
     "b2k_rne_create": (C.c_int, [C.c_int, C.c_int, dp, C.POINTER(vp)]),
     "b2k_rne_destroy": (C.c_int, [vp]),
     "b2k_rne": (C.c_int, [vp, C.c_int, vp, vp, vp, i64, dp, dp, vp, vp]),

@@ -560,6 +560,58 @@ extern "C" int b2k_ikine_null(b2k_chain_t c, int dtype, const void *Tep, int64_t
                   rng_per_row, q_out, success, iterations, searches, residual, ns, (cudaStream_t)stream);
 }
 
+int b2k_ik_qp_launch_f32(const b2k_chain_s *, const void *, long long, const void *, int, int, double, int, const double *,
+                         unsigned long long, int, void *, int *, int *, int *, void *, const IkQpArgs &, cudaStream_t);
+int b2k_ik_qp_launch_f64(const b2k_chain_s *, const void *, long long, const void *, int, int, double, int, const double *,
+                         unsigned long long, int, void *, int *, int *, int *, void *, const IkQpArgs &, cudaStream_t);
+
+extern "C" int b2k_ikine_qp(b2k_chain_t c, int dtype, const void *Tep, int64_t N, const void *q0, int ilimit,
+                            int slimit, double tol, int reject_jl, const double *we, uint64_t seed, int rng_per_row,
+                            double kj, double ks, double kq, double km, double ps, const double *pi, void *q_out,
+                            int32_t *success, int32_t *iterations, int32_t *searches, void *residual, void *stream)
+{
+    const char *fn = "b2k_ikine_qp";
+    if (!c) { b2k_set_error("%s: chain handle is NULL", fn); return B2K_ERR_INVALID; }
+    if (dtype != B2K_F32 && dtype != B2K_F64) { b2k_set_error("%s: dtype must be B2K_F32 or B2K_F64", fn); return B2K_ERR_INVALID; }
+    if (N < 0) { b2k_set_error("%s: N is negative", fn); return B2K_ERR_INVALID; }
+    if (!c->distinct_jindex) {
+        b2k_set_error("%s: two joints of the chain share a jindex (coupled joints are outside the solver's model)", fn);
+        return B2K_ERR_INVALID;
+    }
+    if (c->n < 1 || c->n > B2K_MAX_JOINTS) { b2k_set_error("%s: unsupported joint count %d", fn, c->n); return B2K_ERR_INVALID; }
+    if (ilimit < 1 || slimit < 1) { b2k_set_error("%s: ilimit and slimit must be >= 1", fn); return B2K_ERR_INVALID; }
+    if (!isfinite(kj) || !isfinite(ks) || !isfinite(kq) || !isfinite(km) || !isfinite(ps)) {
+        b2k_set_error("%s: kj, ks, kq, km and ps must be finite", fn);
+        return B2K_ERR_INVALID;
+    }
+    if (!(kj > 0) || !(ks > 0)) {
+        b2k_set_error("%s: kj and ks must be > 0 (the step's quadratic form is not positive definite otherwise)", fn);
+        return B2K_ERR_INVALID;
+    }
+    if (kq > 0) {
+        if (!pi) { b2k_set_error("%s: pi is NULL", fn); return B2K_ERR_INVALID; }
+        for (int i = 0; i < c->n; i++) {
+            if (!isfinite(pi[i])) { b2k_set_error("%s: pi[%d] is not finite", fn, i); return B2K_ERR_INVALID; }
+            if (ps == pi[i]) { b2k_set_error("%s: ps == pi[%d] divides by zero in the velocity damper", fn, i); return B2K_ERR_INVALID; }
+        }
+    }
+    if (km > 0 && c->n < 6) {
+        b2k_set_error("%s: km > 0 needs at least 6 joints (n = %d): J J^T is singular for fewer", fn, c->n);
+        return B2K_ERR_INVALID;
+    }
+    int rc;
+    if ((rc = check_out(fn, "Tep", Tep, N)) || (rc = check_out(fn, "q_out", q_out, N)) ||
+        (rc = check_out(fn, "success", success, N)) || (rc = check_out(fn, "iterations", iterations, N)) ||
+        (rc = check_out(fn, "searches", searches, N)) || (rc = check_out(fn, "residual", residual, N)))
+        return rc;
+    if (N == 0) return B2K_OK;
+    B2K_ON_DEVICE_OF(Tep);
+    const IkQpArgs qp{kj, ks, kq, km, ps, pi};
+    auto launch = dtype == B2K_F64 ? b2k_ik_qp_launch_f64 : b2k_ik_qp_launch_f32;
+    return launch(c, Tep, N, q0, ilimit, slimit, tol, reject_jl, we, seed, rng_per_row, q_out, success, iterations,
+                  searches, residual, qp, (cudaStream_t)stream);
+}
+
 // ------------------------------------------------------------------ dynamics fan-outs
 int b2k_rne_fan_launch_f32(const b2k_rne_s *, int, const void *, const void *, const void *, long long, const double *, void *, cudaStream_t);
 int b2k_rne_fan_launch_f64(const b2k_rne_s *, int, const void *, const void *, const void *, long long, const double *, void *, cudaStream_t);

@@ -103,6 +103,12 @@ struct IkNullArgs {
     const double *pi; // host, n
 };
 
+// gains and damper band of b2k_ikine_qp, as the host passes them (validated there; b2k_ik.cuh)
+struct IkQpArgs {
+    double kj, ks, kq, km, ps;
+    const double *pi; // host, n; read only when kq > 0
+};
+
 struct b2k_rne_s {
     int n, mdh;
     double L[B2K_MAX_JOINTS][24];

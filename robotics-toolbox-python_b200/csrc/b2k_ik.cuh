@@ -228,6 +228,29 @@ __device__ __forceinline__ real b2k_hess_term(JX jx, int i, int r, int k)
     return fma(u1, w2, -(u2 * w1));
 }
 
+// acc[i] = sum_{b,k} H_i[b,k] G[b,k] for the factor A of J J^T that b2k_gram_chol6 left (jacobm[i] = m * acc[i]), from
+// the unweighted base-frame J (J[k][a]).  G is streamed one column at a time (x = A^-1 J[:, k]) into the N sums instead
+// of being held whole.
+template <typename real, int N>
+__device__ __forceinline__ void ik_jacobm_sums(const real (*J)[6], const real *A, real *acc)
+{
+    auto jx = [&](int a, int k) { return J[k][a]; };
+#pragma unroll
+    for (int i = 0; i < N; i++) acc[i] = 0;
+#pragma unroll
+    for (int k = 0; k < N; k++) {
+        real x[6];
+#pragma unroll
+        for (int a = 0; a < 6; a++) x[a] = J[k][a];
+        ik_chol_subst<real, 6>(A, x);
+#pragma unroll
+        for (int i = 0; i < N; i++)
+#pragma unroll
+            for (int r = 0; r < 6; r++)
+                if (k >= i || r < 3) acc[i] = fma(b2k_hess_term<real>(jx, i, r, k), x[r], acc[i]);
+    }
+}
+
 // ------------------------------------------------------------------ null-space motion of the Python solver loop
 // Reference IKSolver._calc_qnull / _null_Σ (restated in DESIGN (f-7)); host side: b2k_ikine_null.
 //   qnull = (I - J^T (J J^T)^-1 J) g,   g = inv_kq sigma(q) + inv_km jacobm(q)
@@ -268,22 +291,8 @@ __device__ __forceinline__ bool ik_null_motion(const IkP<real, N> &K, const IkNs
         qn[i] = s;
     }
     if (S.use_m) {
-        // G is streamed one column at a time (x = A^-1 J[:, k]) into the N sums instead of being held whole
         real acc[N];
-#pragma unroll
-        for (int i = 0; i < N; i++) acc[i] = 0;
-#pragma unroll
-        for (int k = 0; k < N; k++) {
-            real x[6];
-#pragma unroll
-            for (int a = 0; a < 6; a++) x[a] = J[k][a];
-            ik_chol_subst<real, 6>(A, x);
-#pragma unroll
-            for (int i = 0; i < N; i++)
-#pragma unroll
-                for (int r = 0; r < 6; r++)
-                    if (k >= i || r < 3) acc[i] = fma(b2k_hess_term<real>(jx, i, r, k), x[r], acc[i]);
-        }
+        ik_jacobm_sums<real, N>(J, A, acc);
         const real c = S.inv_km * m;
 #pragma unroll
         for (int i = 0; i < N; i++) qn[i] = fma(c, acc[i], qn[i]);
@@ -305,6 +314,136 @@ __device__ __forceinline__ bool ik_null_motion(const IkP<real, N> &K, const IkNs
         qn[k] = s;
     }
     return ok;
+}
+
+// ------------------------------------------------------------------ quadratic-programming step of the Python solver loop
+// Reference IK_QP.step (restated in DESIGN (f-11)); host side: b2k_ikine_qp.  With x = (dq, s):
+//   min 1/2 kj |dq|^2 + 1/2 w |s|^2 + c^T dq   s.t.  J dq + s = e,   w = ks / sum|e|,   c = -[km > 0] jacobm(q) / km
+// and, with kq > 0, at most one velocity-damper row per joint (the upper one wins when both hold):
+//   -dq_i <= inv_kq ((q_i - l_i) - ps) / (pi_i - ps)  if q_i - l_i <= pi_i
+//    dq_i <= inv_kq ((h_i - q_i) - ps) / (pi_i - ps)  if h_i - q_i <= pi_i
+// Eliminating s and dividing by w (w grows as e shrinks; fp32 needs the scaled form):
+//   min 1/2 dq^T (lam I + J^T J) dq - r^T dq,   lam = (kj / ks) sum|e|,   r = J^T e + sum|e| / (km ks) jacobm(q)
+// under one-sided bounds on single coordinates.  kj_ks = kj / ks, inv_kmks = 1 / (km ks), inv_kq = 1 / kq.
+template <typename real, int N>
+struct IkQp {
+    real kj_ks, inv_kmks, inv_kq, ps;
+    real pi[N];
+    int use_q, use_m;
+};
+
+// dq of the step in g.  The bounded QP is a linear complementarity problem with the SPD matrix lam I + J^T J, solved by
+// principal pivoting with the least-index rule (Murty), which terminates for such matrices: each round solves the
+// equality problem with the current set of fixed coordinates -- their rows and columns replaced by identity rows, so
+// every index stays static -- then frees the lowest-indexed fixed coordinate whose multiplier is negative, or fixes the
+// lowest-indexed free one past its bound.  Without a damper row that is one Cholesky solve, the cost of an LM step.
+// False (the search is abandoned) when a factorisation fails or the rounds run out; sum|e| = 0 gives dq = 0.
+template <typename real, int N>
+__device__ __forceinline__ bool ik_qp_step(const IkP<real, N> &K, const IkQp<real, N> &S, const real (*J)[6],
+                                           const real *e, const real *q, real *g)
+{
+    real se = 0;
+#pragma unroll
+    for (int k = 0; k < 6; k++) se += fabs(e[k]);
+    if (se == (real)0) {
+#pragma unroll
+        for (int i = 0; i < N; i++) g[i] = 0;
+        return true;
+    }
+    const real lam = S.kj_ks * se;
+    real r[N];
+#pragma unroll
+    for (int i = 0; i < N; i++) {
+        real s = 0;
+#pragma unroll
+        for (int k = 0; k < 6; k++) s = fma(J[i][k], e[k], s);
+        r[i] = s;
+    }
+    if constexpr (N >= 6) { // the host rejects km > 0 for fewer joints: J J^T is singular there
+        if (S.use_m) {
+            auto jx = [&](int a, int k) { return J[k][a]; };
+            real A[21], m, acc[N];
+            if (!b2k_gram_chol6<real, N>(jx, A, m)) return false;
+            ik_jacobm_sums<real, N>(J, A, acc);
+            const real cm = m * se * S.inv_kmks;
+#pragma unroll
+            for (int i = 0; i < N; i++) r[i] = fma(cm, acc[i], r[i]);
+        }
+    }
+    // damper rows: bit i of `up` (dq_i <= bnd_i) or `lo` (dq_i >= bnd_i)
+    unsigned up = 0, lo = 0;
+    real bnd[N];
+#pragma unroll
+    for (int i = 0; i < N; i++) {
+        bnd[i] = 0;
+        if (S.use_q) {
+            const real dl = q[i] - K.qlim_l[i], dh = K.qlim_h[i] - q[i], d = S.inv_kq / (S.pi[i] - S.ps);
+            if (dh <= S.pi[i]) {
+                up |= 1u << i;
+                bnd[i] = (dh - S.ps) * d;
+            } else if (dl <= S.pi[i]) {
+                lo |= 1u << i;
+                bnd[i] = -((dl - S.ps) * d);
+            }
+        }
+    }
+    const unsigned rows = up | lo;
+    const real tol = (real)64 * (sizeof(real) == 8 ? (real)2.220446049250313e-16 : (real)1.1920929e-07);
+    unsigned fixed = 0;
+    for (int round = 0; round < 2 * N + 2; round++) {
+        real A[N * (N + 1) / 2];
+#pragma unroll
+        for (int i = 0; i < N; i++) g[i] = ((fixed >> i) & 1u) ? bnd[i] : r[i];
+#pragma unroll
+        for (int i = 0; i < N; i++) {
+            const bool fi = (fixed >> i) & 1u;
+#pragma unroll
+            for (int j = 0; j <= i; j++) {
+                const bool fj = (fixed >> j) & 1u;
+                real h = 0;
+#pragma unroll
+                for (int k = 0; k < 6; k++) h = fma(J[i][k], J[j][k], h);
+                if (i == j) {
+                    A[i * (i + 1) / 2 + j] = fi ? (real)1 : h + lam;
+                } else {
+                    A[i * (i + 1) / 2 + j] = (fi || fj) ? (real)0 : h;
+                    if (fi && !fj) g[j] = fma(-h, bnd[i], g[j]);
+                    if (fj && !fi) g[i] = fma(-h, bnd[j], g[i]);
+                }
+            }
+        }
+        if (!ik_chol_solve<real, N>(A, g)) return false;
+        if (!rows) return true;
+#pragma unroll
+        for (int i = 0; i < N; i++)
+            if ((fixed >> i) & 1u) g[i] = bnd[i];
+        real Jx[6];
+#pragma unroll
+        for (int k = 0; k < 6; k++) {
+            real s = 0;
+#pragma unroll
+            for (int j = 0; j < N; j++) s = fma(J[j][k], g[j], s);
+            Jx[k] = s;
+        }
+        int pick = -1;
+#pragma unroll
+        for (int i = N - 1; i >= 0; i--) { // downwards: the lowest index that breaks a condition is picked
+            if (!((rows >> i) & 1u)) continue;
+            const real sg = ((up >> i) & 1u) ? (real)1 : (real)-1;
+            if ((fixed >> i) & 1u) { // multiplier -sg * gradient must be >= 0
+                real jj = 0;
+#pragma unroll
+                for (int k = 0; k < 6; k++) jj = fma(J[i][k], Jx[k], jj);
+                const real lx = lam * g[i], grad = lx + jj - r[i];
+                if (sg * grad > tol * (fabs(lx) + fabs(jj) + fabs(r[i]))) pick = i;
+            } else if (sg * (g[i] - bnd[i]) > tol * (fabs(g[i]) + fabs(bnd[i]))) {
+                pick = i;
+            }
+        }
+        if (pick < 0) return true;
+        fixed ^= 1u << pick;
+    }
+    return false;
 }
 
 // ------------------------------------------------------------------ one LM evaluation (+ update) in registers
@@ -372,10 +511,11 @@ __device__ __forceinline__ bool ik_pinv_step(const IkP<real, N> &K, real (*J)[6]
 }
 
 // NS: add the null-space motion of IkNs S (Python semantics, N >= 7 only) to the update; S is unused otherwise.
-template <typename real, int N, int PROF, int STEP = 0, bool NS = false>
+// STEP = 2: the quadratic-programming step of IkQp S (Python semantics) instead of the LM step.
+template <typename real, int N, int PROF, int STEP = 0, bool NS = false, typename XP = IkNs<real, N>>
 __device__ __forceinline__ bool ik_eval(const ChainP<real, N> &P, const IkP<real, N> &K, const real *Tp, const real *q,
                                         real &Ecur, real *g, bool skip_step_if_converged,
-                                        const IkNs<real, N> *S = nullptr)
+                                        const XP *S = nullptr)
 {
     Pose<real> Te;
     real zj[N][3], pj[N][3], e[6];
@@ -408,6 +548,7 @@ __device__ __forceinline__ bool ik_eval(const ChainP<real, N> &P, const IkP<real
             J[j][3] = 0; J[j][4] = 0; J[j][5] = 0;
         }
     }
+    if constexpr (STEP == 2) return ik_qp_step<real, N>(K, *S, J, e, q, g);
     real qn[N];
     bool nok = true;
     if constexpr (NS) nok = ik_null_motion<real, N>(K, *S, J, q, qn); // before ik_pinv_step weighs J in place
@@ -494,11 +635,16 @@ template <typename real> constexpr int ik_min_blocks() { return sizeof(real) == 
 // at N = 10; fp64 at 255 (2 blocks) spills less than the plain fp64 k_ik_lm does at 168 (DESIGN (f-7) has the table).
 template <typename real, int N> constexpr int ik_ns_min_blocks() { return sizeof(real) == 4 && N <= 9 ? 3 : 2; }
 
-// The bodies of the two kernels are shared by the plain kernels (k_ik_lm, k_ik_restarts) and their null-space
-// variants (k_ik_lm_ns, k_ik_restarts_ns, NS = true, S = their IkNs parameter); S is unused when NS is false.
-template <typename real, int N, int PROF, int STEP, bool NS>
+// The kernels with the quadratic-programming step (k_ik_lm_qp, k_ik_restarts_qp) hold J, the factor of the bounded
+// system and, from N = 6, the Gram factor and the N Hessian sums.  Chosen from -Xptxas -v (DESIGN (f-11) has the table).
+template <typename real, int N> constexpr int ik_qp_min_blocks() { return sizeof(real) == 4 && N <= 7 ? 3 : 2; }
+
+// The bodies of the two kernels are shared by the plain kernels (k_ik_lm, k_ik_restarts), their null-space
+// variants (k_ik_lm_ns, k_ik_restarts_ns, NS = true, S = their IkNs parameter) and the QP kernels (STEP = 2, S = their
+// IkQp parameter); S is unused otherwise.
+template <typename real, int N, int PROF, int STEP, bool NS, typename XP = IkNs<real, N>>
 __device__ __forceinline__ void
-ik_lm_body(const ChainP<real, N> &P, const IkP<real, N> &K, const IkNs<real, N> *S,
+ik_lm_body(const ChainP<real, N> &P, const IkP<real, N> &K, const std::enable_if_t<true, XP> *S,
            const real *__restrict__ Tep, const real *__restrict__ q0, long long nprob, real *__restrict__ q_out,
            int *__restrict__ success, int *__restrict__ iterations, int *__restrict__ searches,
            real *__restrict__ residual, int two_phase, int *__restrict__ hard_idx, int *__restrict__ hard_count,
@@ -594,7 +740,7 @@ ik_lm_body(const ChainP<real, N> &P, const IkP<real, N> &K, const IkNs<real, N> 
         real g[N], Ecur;
         // one call site for both loop orders (the evaluation is ~600 instructions; two inlined copies only cost
         // instruction-cache misses): the C++ order skips the step when the test before it has already passed
-        const bool ok = ik_eval<real, N, PROF, STEP, NS>(P, K, Tp, q, Ecur, g, cpp, S);
+        const bool ok = ik_eval<real, N, PROF, STEP, NS, XP>(P, K, Tp, q, Ecur, g, cpp, S);
         E = Ecur;
         if (cpp) {
             // test before stepping (ik.cpp:44-58)
@@ -658,6 +804,20 @@ k_ik_lm_ns(const __grid_constant__ ChainP<real, N> P, const __grid_constant__ Ik
                                           cont_count);
 }
 
+template <typename real, int N, int PROF>
+__global__ void __launch_bounds__(B2K_THREADS, ik_qp_min_blocks<real, N>())
+k_ik_lm_qp(const __grid_constant__ ChainP<real, N> P, const __grid_constant__ IkP<real, N> K,
+           const real *__restrict__ Tep, const real *__restrict__ q0, long long nprob, real *__restrict__ q_out,
+           int *__restrict__ success, int *__restrict__ iterations, int *__restrict__ searches,
+           real *__restrict__ residual, int two_phase, int *__restrict__ hard_idx, int *__restrict__ hard_count,
+           int iter_cap, const int *__restrict__ in_list, const int *__restrict__ in_count, int *__restrict__ cont_idx,
+           int *__restrict__ cont_count, const __grid_constant__ IkQp<real, N> S)
+{
+    ik_lm_body<real, N, PROF, 2, false, IkQp<real, N>>(P, K, &S, Tep, q0, nprob, q_out, success, iterations, searches, residual,
+                                        two_phase, hard_idx, hard_count, iter_cap, in_list, in_count, cont_idx,
+                                        cont_count);
+}
+
 // ------------------------------------------------------------------ phase B: G lanes per hard problem, searches in parallel
 // The restart draws are counter-based (seed, row, search, joint), so search s of a problem does not
 // depend on searches 0..s-1.  A group of G lanes therefore runs G consecutive searches of one hard
@@ -665,9 +825,9 @@ k_ik_lm_ns(const __grid_constant__ ChainP<real, N> P, const __grid_constant__ Ik
 // is the sum of the contributions of all lower-numbered searches plus its own -- exactly what
 // the sequential loop reports, but the latency of a problem needing k restarts drops from
 // k x ilimit LM iterations to ceil(k / G) x ilimit.
-template <typename real, int N, int PROF, int G, int STEP, bool NS>
+template <typename real, int N, int PROF, int G, int STEP, bool NS, typename XP = IkNs<real, N>>
 __device__ __forceinline__ void
-ik_restarts_body(const ChainP<real, N> &P, const IkP<real, N> &K, const IkNs<real, N> *S,
+ik_restarts_body(const ChainP<real, N> &P, const IkP<real, N> &K, const std::enable_if_t<true, XP> *S,
                  const real *__restrict__ Tep, real *__restrict__ q_out, int *__restrict__ success,
                  int *__restrict__ iterations, int *__restrict__ searches, real *__restrict__ residual,
                  const int *__restrict__ hard_idx, const int *__restrict__ hard_count, int s_first, int max_batches,
@@ -709,7 +869,7 @@ ik_restarts_body(const ChainP<real, N> &P, const IkP<real, N> &K, const IkNs<rea
             while (__any_sync(FULL, going)) {
                 if (going) {
                     real g[N], Ecur;
-                    const bool ok = ik_eval<real, N, PROF, STEP, NS>(P, K, Tp, q, Ecur, g, cpp, S);
+                    const bool ok = ik_eval<real, N, PROF, STEP, NS, XP>(P, K, Tp, q, Ecur, g, cpp, S);
                     E = Ecur;
                     if (cpp) {
                         if (Ecur < K.tol) {
@@ -810,17 +970,31 @@ k_ik_restarts_ns(const __grid_constant__ ChainP<real, N> P, const __grid_constan
                                                    hard_idx, hard_count, s_first, max_batches, out_idx, out_count);
 }
 
-// kernel selection for ik_launch_n: the plain kernels, or (NS) their null-space variants
+template <typename real, int N, int PROF, int G>
+__global__ void __launch_bounds__(B2K_THREADS, ik_qp_min_blocks<real, N>())
+k_ik_restarts_qp(const __grid_constant__ ChainP<real, N> P, const __grid_constant__ IkP<real, N> K,
+                 const real *__restrict__ Tep, real *__restrict__ q_out, int *__restrict__ success,
+                 int *__restrict__ iterations, int *__restrict__ searches, real *__restrict__ residual,
+                 const int *__restrict__ hard_idx, const int *__restrict__ hard_count, int s_first, int max_batches,
+                 int *__restrict__ out_idx, int *__restrict__ out_count, const __grid_constant__ IkQp<real, N> S)
+{
+    ik_restarts_body<real, N, PROF, G, 2, false, IkQp<real, N>>(P, K, &S, Tep, q_out, success, iterations, searches, residual,
+                                                 hard_idx, hard_count, s_first, max_batches, out_idx, out_count);
+}
+
+// kernel selection for ik_launch_n: the plain kernels, (NS) their null-space variants, or (STEP = 2) the QP kernels
 template <typename real, int N, int PROF, int STEP, bool NS>
 constexpr auto ik_kernel_a()
 {
-    if constexpr (NS) return &k_ik_lm_ns<real, N, PROF, STEP>;
+    if constexpr (STEP == 2) return &k_ik_lm_qp<real, N, PROF>;
+    else if constexpr (NS) return &k_ik_lm_ns<real, N, PROF, STEP>;
     else return &k_ik_lm<real, N, PROF, STEP>;
 }
 template <typename real, int N, int PROF, int G, int STEP, bool NS>
 constexpr auto ik_kernel_b()
 {
-    if constexpr (NS) return &k_ik_restarts_ns<real, N, PROF, G, STEP>;
+    if constexpr (STEP == 2) return &k_ik_restarts_qp<real, N, PROF, G>;
+    else if constexpr (NS) return &k_ik_restarts_ns<real, N, PROF, G, STEP>;
     else return &k_ik_restarts<real, N, PROF, G, STEP>;
 }
 
@@ -828,7 +1002,7 @@ template <typename real, int N, int STEP, bool NS = false>
 int ik_launch_n(const b2k_chain_s *c, const real *Tep, long long nprob, const real *q0, int ilimit, int slimit,
                 double tol, int reject_jl, const double *we, double lambda, int method, unsigned long long seed,
                 int semantics, int rng_per_row, real *q_out, int *success, int *iterations, int *searches,
-                real *residual, cudaStream_t st, const IkNullArgs *ns = nullptr)
+                real *residual, cudaStream_t st, const IkNullArgs *ns = nullptr, const IkQpArgs *qp = nullptr)
 {
     ChainP<real, N> P;
     b2k_fill_chain<real, N>(c, nullptr, nullptr, true, P);
@@ -844,8 +1018,16 @@ int ik_launch_n(const b2k_chain_s *c, const real *Tep, long long nprob, const re
     K.lambda = (real)lambda; K.tol = (real)tol;
     K.ilimit = ilimit; K.slimit = slimit; K.method = method; K.reject_jl = reject_jl ? 1 : 0;
     K.semantics = semantics; K.rng_per_row = rng_per_row ? 1 : 0; K.has_q0 = q0 ? 1 : 0; K.seed = seed;
-    IkNs<real, N> S{};
-    if constexpr (NS) {
+    std::conditional_t<STEP == 2, IkQp<real, N>, IkNs<real, N>> S{};
+    if constexpr (STEP == 2) {
+        S.use_q = qp->kq > 0 ? 1 : 0;
+        S.use_m = qp->km > 0 ? 1 : 0;
+        S.kj_ks = (real)(qp->kj / qp->ks);
+        S.inv_kmks = S.use_m ? (real)(1.0 / (qp->km * qp->ks)) : (real)0;
+        S.inv_kq = S.use_q ? (real)(1.0 / qp->kq) : (real)0;
+        S.ps = (real)qp->ps;
+        for (int i = 0; i < N; i++) S.pi[i] = S.use_q ? (real)qp->pi[i] : (real)0;
+    } else if constexpr (NS) {
         S.use_q = ns->kq > 0 ? 1 : 0;
         S.use_m = ns->km > 0 ? 1 : 0;
         S.inv_kq = S.use_q ? (real)(1.0 / ns->kq) : (real)0; // the reference scales by 1.0 / λ (IK.py _calc_qnull)
@@ -853,9 +1035,9 @@ int ik_launch_n(const b2k_chain_s *c, const real *Tep, long long nprob, const re
         S.ps = (real)ns->ps;
         for (int i = 0; i < N; i++) S.pi[i] = (real)ns->pi[i];
     }
-    // one launch of kern (NS: with S appended as its last argument)
+    // one launch of kern (NS, STEP = 2: with S appended as its last argument)
     auto go = [&](auto kern, long long grid, auto... a) {
-        if constexpr (NS) kern<<<(unsigned)grid, B2K_THREADS, 0, st>>>(a..., S);
+        if constexpr (NS || STEP == 2) kern<<<(unsigned)grid, B2K_THREADS, 0, st>>>(a..., S);
         else kern<<<(unsigned)grid, B2K_THREADS, 0, st>>>(a...);
     };
     // Two phases when restarts are allowed and the batch is large enough to matter: phase A runs the
@@ -988,6 +1170,28 @@ int ik_ns_launch(const b2k_chain_s *c, const void *Tep, long long nprob, const v
         B2K_CASE(7) B2K_CASE(8) B2K_CASE(9) B2K_CASE(10)
     default:
         b2k_set_error("ikine_null: unsupported joint count %d (7..10)", c->n);
+        return B2K_ERR_INVALID;
+    }
+#undef B2K_CASE
+}
+
+// b2k_ikine_qp: the Python solver loop with the quadratic-programming step, for 1..10 joints
+template <typename real>
+int ik_qp_launch(const b2k_chain_s *c, const void *Tep, long long nprob, const void *q0, int ilimit, int slimit, double tol,
+                 int reject_jl, const double *we, unsigned long long seed, int rng_per_row, void *q_out, int *success,
+                 int *iterations, int *searches, void *residual, const IkQpArgs &qp, cudaStream_t st)
+{
+#define B2K_CASE(NN)                                                                                                   \
+    case NN:                                                                                                           \
+        return ik_launch_n<real, NN, 2, false>(c, (const real *)Tep, nprob, (const real *)q0, ilimit, slimit, tol,     \
+                                               reject_jl, we, 0.0, 0, seed, B2K_IK_SEM_PYTHON, rng_per_row,          \
+                                               (real *)q_out, success, iterations, searches, (real *)residual, st,    \
+                                               nullptr, &qp);
+    switch (c->n) {
+        B2K_CASE(1) B2K_CASE(2) B2K_CASE(3) B2K_CASE(4) B2K_CASE(5)
+        B2K_CASE(6) B2K_CASE(7) B2K_CASE(8) B2K_CASE(9) B2K_CASE(10)
+    default:
+        b2k_set_error("ikine_qp: unsupported joint count %d", c->n);
         return B2K_ERR_INVALID;
     }
 #undef B2K_CASE

@@ -527,3 +527,56 @@ if want("ikine_null_"):
                         mean_searches=float(ro.float().mean())))
             del qo, so, io, ro, Eo
         del Td
+
+# IK with the quadratic-programming step (b2k_ikine_qp) against the LM loop: config 4's targets (Panda, reachable,
+# seed 2), the Python solver loop (joint limits checked, restarts shared by all rows), kj = ks = 1, ps = 0, pi = 0.3,
+# kq / km = 1.0 where on.  "lm" is b2k_ik_lm in the same semantics (chan k = 1.0).  The card's name and power limit are
+# read in the same run.
+if want("ikine_qp_"):
+    import subprocess
+
+    try:
+        plim = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True,
+                              text=True, timeout=30).stdout.strip()
+    except Exception as e:  # the figure is context, the timing does not depend on it
+        plim = f"unavailable ({type(e).__name__})"
+    card = {"gpu": torch.cuda.get_device_name(0), "power_limit": plim}
+    panda = rtb.models.Panda().ets()
+    M = args.ik_rows
+    Tep = panda.eval(np.random.default_rng(2).uniform(-np.pi, np.pi, (M, 7)))
+    Lb = rtb._lib.lib()
+    chn = panda._chain
+    stp = torch.cuda.current_stream().cuda_stream
+    pi = np.full(7, 0.3)
+    for dt in (np.float32, np.float64):
+        tag = "f64" if dt == np.float64 else "f32"
+        Td = torch.from_numpy(Tep.astype(dt)).to(dev)
+        codei = rtb._lib.F64 if dt == np.float64 else rtb._lib.F32
+        for var, kq, km in (("lm", 0.0, 0.0), ("off", 0.0, 0.0), ("kq", 1.0, 0.0), ("km", 0.0, 1.0), ("both", 1.0, 1.0)):
+            name = f"ikine_qp_panda_{tag}_{var}"
+            if not want(name):
+                continue
+            qo = torch.empty((M, 7), dtype=Td.dtype, device=dev)
+            so, io, ro = (torch.empty(M, dtype=torch.int32, device=dev) for _ in range(3))
+            Eo = torch.empty(M, dtype=Td.dtype, device=dev)
+
+            def run(i):
+                if var == "lm":
+                    rc = Lb.b2k_ik_lm(chn, codei, Td.data_ptr(), M, None, 30, 100, 1e-6, 1, None, 1.0, 0, 5 + i,
+                                      rtb._lib.SEM_PYTHON, 0, qo.data_ptr(), so.data_ptr(), io.data_ptr(), ro.data_ptr(),
+                                      Eo.data_ptr(), stp)
+                else:
+                    rc = Lb.b2k_ikine_qp(chn, codei, Td.data_ptr(), M, None, 30, 100, 1e-6, 1, None, 5 + i, 0, 1.0, 1.0,
+                                         kq, km, 0.0, rtb._lib.dptr(pi), qo.data_ptr(), so.data_ptr(), io.data_ptr(),
+                                         ro.data_ptr(), Eo.data_ptr(), stp)
+                rtb._lib.check(rc)
+
+            steps, args.steps = args.steps, 10
+            wu, args.warmup = args.warmup, 2
+            ms = timeit(run, 1 << 30)
+            args.steps, args.warmup = steps, wu
+            report(name, ms, M, (16 + 7 + 4) * np.dtype(dt).itemsize,
+                   dict(card, solves_per_s=M / (ms * 1e-3), success=float(so.float().mean()), mean_it=float(io.float().mean()),
+                        mean_searches=float(ro.float().mean())))
+            del qo, so, io, ro, Eo
+        del Td
