@@ -139,6 +139,19 @@ int b2k_fkine_jacob0(b2k_chain_t chain, int dtype, const void *q, int64_t N, int
 int b2k_fkine_jacobe(b2k_chain_t chain, int dtype, const void *q, int64_t N, int64_t ldq,
                      const double *base, const double *tool, void *T, void *J, void *stream);
 
+/* Planar forward kinematics and Jacobians of an ETS2 chain (reference ETS2.eval / fkine / jacob0 / jacobe, ET.py and
+ * ETS.py; pure Python there).  The chain is created by b2k_chain_create from the ETS2's 3-D embedding (R -> Rz,
+ * tx -> tx, ty -> ty, SE2 -> an SE3 acting in the xy plane); a chain with any other joint axis, or a constant with an
+ * out-of-plane rotation or a z translation, is rejected before any CUDA call with an error naming the first such
+ * transform.  base and tool are row-major 3x3 SE(2) matrices (NULL = identity); the base enters T only.
+ *   T (N,3,3) row-major = base * prod_k ET2_k(q[i, jindex_k]) * tool
+ *   J (N,3,n), rows (vx, vy, w), columns in chain order: frame 0 = jacob0, in the chain's start frame;
+ *     frame 1 = jacobe = blkdiag(R^T, 1) jacob0, R the rotation of the pose (tool in, base out).
+ * T or J may be NULL, not both; both from one pass when both are given.  n = 1..B2K_MAX_JOINTS, fp32 / fp64; q rows
+ * as b2k_fkine.  Every argument is checked before any CUDA call; N = 0 touches no device. */
+int b2k_fkine_planar(b2k_chain_t chain, int dtype, const void *q, int64_t N, int64_t ldq, const double *base,
+                     const double *tool, int frame, void *T, void *J, void *stream);
+
 /* ---------------------------------------------------------------- inverse kinematics
  * Replaces fknm.IK_LM_c (fknm.cpp:394-525 -> _IK_LM_Chan/_Wampler/_Sugihara ik.cpp:157-209
  * -> _IK_loop ik.cpp:19-75) for N targets at once, and -- with semantics =

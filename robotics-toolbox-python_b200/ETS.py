@@ -25,8 +25,8 @@ import numpy as np
 
 from . import _buffers as B
 from . import _lib
-from ._se3 import SE3
-from .ET import AXES, ET
+from ._se3 import SE2, SE3
+from .ET import ET, ET2
 from .IK import IKSolution
 
 
@@ -83,8 +83,8 @@ class ETS:
                 j.jindex = k
             self._auto_jindex = True
 
-    @staticmethod
-    def from_links(link_ets: List["ETS"]) -> "ETS":
+    @classmethod
+    def from_links(cls, link_ets: List["ETS"]) -> "ETS":
         """Concatenate per-link ETSs into a robot chain.  When every link's joint index was only
         auto-assigned (each link numbered its own joint 0), the joints are renumbered 0..n-1 in
         chain order -- what the reference's robot constructor does (BaseRobot.py:336-352)."""
@@ -96,14 +96,14 @@ class ETS:
                 if renumber and c.isjoint:
                     c._jindex = None
                 parts.append(c)
-        return ETS(parts)
+        return cls(parts)
 
     # ---- composition
     def __mul__(self, other):
         if isinstance(other, ET):
-            return ETS([*self._ets, other])
+            return type(self)([*self._ets, other])
         if isinstance(other, ETS):
-            return ETS([*self._ets, *other._ets])
+            return type(self)([*self._ets, *other._ets])
         return NotImplemented
 
     __add__ = __mul__
@@ -111,7 +111,7 @@ class ETS:
     def inv(self) -> "ETS":
         """Inverse of the ETS: the inverses of the individual ETs in reverse order (reference ETS.inv,
         ETS.py:545-576).  Joints keep their jindex, so explicit joint indices are essential."""
-        return ETS([et.inv() for et in reversed(self._ets)])
+        return type(self)([et.inv() for et in reversed(self._ets)])
 
     def __len__(self):
         return len(self._ets)
@@ -121,7 +121,7 @@ class ETS:
 
     def __getitem__(self, i):
         r = self._ets[i]
-        return ETS(r) if isinstance(i, slice) else r
+        return type(self)(r) if isinstance(i, slice) else r
 
     def __repr__(self):
         return " ⊕ ".join(repr(e) for e in self._ets)
@@ -155,6 +155,8 @@ class ETS:
     def structure(self) -> str:
         return "".join("R" if e.isrotation else "P" for e in self.joints())
 
+    _const = staticmethod(ET.SE3)  # the constant transform compile() folds a run into
+
     def compile(self) -> "ETS":
         """Fold runs of constants into single SE(3) constants (reference ETS.py:857-906).  The
         native chain compiler applies the same rule internally; this is for inspection."""
@@ -163,14 +165,14 @@ class ETS:
         for e in self._ets:
             if e.isjoint:
                 if acc is not None:
-                    out.append(ET.SE3(acc))
+                    out.append(self._const(acc))
                     acc = None
                 out.append(e.copy())
             else:
                 acc = e.A() if acc is None else acc @ e.A()
         if acc is not None:
-            out.append(ET.SE3(acc))
-        return ETS(out)
+            out.append(self._const(acc))
+        return type(self)(out)
 
     def describe(self) -> dict:
         """Neutral per-ET description: exactly what the reference marshals into fknm.ET_init
@@ -183,10 +185,10 @@ class ETS:
         }
         for i, e in enumerate(self._ets):
             d["isjoint"][i] = int(e.isjoint)
-            d["axis"][i] = AXES.get(e.axis, 0)
+            d["axis"][i] = e._axis_code()
             d["flip"][i] = int(e.isflip)
             d["jindex"][i] = e.jindex if (e.isjoint and e.jindex is not None) else 0
-            d["T"][i] = e.A() if not e.isjoint else np.eye(4)
+            d["T"][i] = e.A3() if not e.isjoint else np.eye(4)
             d["qlim"][i] = e._qlim_default()
         return d
 
@@ -841,3 +843,72 @@ class ETS:
         qp = self._qp_args(kj, ks, kq, km, ps, pi)
         return self._ik_solution(self._ik(Tep, q0, ilimit, slimit, tol, mask, joint_limits, 0.0, 0, seed,
                                           _lib.SEM_PYTHON, False, dtype, qp=qp))
+
+
+def _mat33(T, name):
+    """None / SE2-like / array -> fp64 (3,3) or None."""
+    if T is None:
+        return None
+    T = getattr(T, "A", T)
+    T = np.ascontiguousarray(np.asarray(T, dtype=np.float64))
+    if T.shape != (3, 3):
+        raise ValueError(f"{name} must be a 3x3 matrix")
+    return T
+
+
+class ETS2(ETS):
+    """A sequence of planar :class:`ET2` (reference ETS2, ETS.py).  Joint numbering, q shapes and the compiled chain
+    are those of :class:`ETS`: the sequence reaches ``b2k_chain_create`` as its 3-D embedding (``describe``), and the
+    planar kernel (``b2k_fkine_planar``) evaluates that chain in the plane.  Poses are (3,3) / (N,3,3) and Jacobians
+    (3,n) / (N,3,n) with rows (vx, vy, w)."""
+
+    _const = staticmethod(ET2.SE2)
+
+    def __init__(self, arg: Union[None, ET2, "ETS2", List] = None):
+        super().__init__(arg)
+        if not all(isinstance(e, ET2) for e in self._ets):
+            raise TypeError("an ETS2 holds ET2 transforms only")
+
+    # ------------------------------------------------------------------ kinematics
+    def _planar(self, q, base, tool, frame, want_t, want_j, dtype):
+        """(T or None, J or None, single) from one b2k_fkine_planar launch; host in -> host out"""
+        q2, single = self._qbatch(q)
+        dt = B.pick_dtype(q2, dtype)
+        base, tool = _mat33(base, "base"), _mat33(tool, "tool")
+        host = not B.is_tensor(q2)
+        qd = B.to_device(q2, dt)
+        N = qd.shape[0]
+        T = B.empty((N, 3, 3), dt, like=qd) if want_t else None
+        J = B.empty((N, 3, self.n), dt, like=qd) if want_j else None
+        _lib.check(_lib.lib().b2k_fkine_planar(self._chain, B.code(dt), B.ptr(qd), N, qd.shape[1], _lib.dptr(base),
+                                               _lib.dptr(tool), frame, None if T is None else B.ptr(T),
+                                               None if J is None else B.ptr(J), B.stream_ptr(qd)))
+        if host:
+            T = None if T is None else B.to_host(T)
+            J = None if J is None else B.to_host(J)
+        if single:
+            T = None if T is None else T[0]
+            J = None if J is None else J[0]
+        return T, J
+
+    def eval(self, q, base=None, tool=None, include_base: bool = True, dtype=None):
+        """Planar forward kinematics as arrays: (3,3) for one q, (N,3,3) for a batch;
+        base * prod A_i(q[jindex_i]) * tool."""
+        return self._planar(q, base if include_base else None, tool, 0, True, False, dtype)[0]
+
+    def fkine(self, q, base=None, tool=None, include_base: bool = True, dtype=None) -> SE2:
+        """Planar forward kinematics as one batched SE2 container."""
+        T = self.eval(q, base, tool, include_base, dtype)
+        return SE2(B.to_host(T) if B.is_tensor(T) else T)
+
+    def jacob0(self, q, tool=None, dtype=None):
+        """Jacobian in the chain's start frame, (3,n) or (N,3,n), rows (vx, vy, w); the tool is included, no base."""
+        return self._planar(q, None, tool, 0, False, True, dtype)[1]
+
+    def jacobe(self, q, tool=None, dtype=None):
+        """Jacobian in the end-effector frame: blkdiag(R^T, 1) jacob0 with R the rotation of the pose (tool in)."""
+        return self._planar(q, None, tool, 1, False, True, dtype)[1]
+
+    def fkine_jacob0(self, q, base=None, tool=None, include_base: bool = True, dtype=None):
+        """Pose and start-frame Jacobian from one pass over q.  Returns (T, J)."""
+        return self._planar(q, base if include_base else None, tool, 0, True, True, dtype)

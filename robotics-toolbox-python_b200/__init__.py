@@ -12,13 +12,14 @@ There is no CPU fallback in this package.
 """
 from . import _lib  # noqa: F401
 from ._lib import B2KError, launch_count, pinned_empty  # noqa: F401
-from ._se3 import SE3  # noqa: F401
-from .ET import ET  # noqa: F401
+from ._se3 import SE2, SE3  # noqa: F401
+from .ET import ET, ET2  # noqa: F401
 from .IK import IK_GN, IK_LM, IK_NR, IK_QP, IKSolution  # noqa: F401
-from .ETS import ETS  # noqa: F401
+from .ETS import ETS, ETS2  # noqa: F401
 from .DHLink import DHLink, PrismaticDH, PrismaticMDH, RevoluteDH, RevoluteMDH  # noqa: F401
 from .DHRobot import DHRobot  # noqa: F401
 from .Robot import ERobot, Link, Robot  # noqa: F401
+from .Robot2 import Link2, Robot2  # noqa: F401
 from . import models  # noqa: F401
 from . import dist  # noqa: F401
 from . import trajectory  # noqa: F401

@@ -188,6 +188,34 @@ extern "C" int b2k_fkine_jacobe(b2k_chain_t c, int dtype, const void *q, int64_t
     return fkj_dispatch("b2k_fkine_jacobe", c, dtype, FKJ_T | FKJ_JE, q, N, ldq, base, tool, T, J, stream);
 }
 
+// ------------------------------------------------------------------ planar chains (b2k_planar.cu)
+int b2k_planar_check(const char *fn, const b2k_chain_s *c, const double *base, const double *tool);
+int b2k_planar_launch(const b2k_chain_s *c, int dtype, const double *base, const double *tool, int frame, const void *q,
+                      long long nrows, long long ldq, void *T, void *J, cudaStream_t st);
+
+// the unit a per-warp output stage of rows of `row_bytes` is copied in (TileStage<real, n>::UB in b2k_fkj.cuh)
+static unsigned stage_unit(unsigned row_bytes) { return row_bytes % 16 == 0 ? 16u : (row_bytes % 8 == 0 ? 8u : 4u); }
+
+extern "C" int b2k_fkine_planar(b2k_chain_t c, int dtype, const void *q, int64_t N, int64_t ldq, const double *base,
+                                const double *tool, int frame, void *T, void *J, void *stream)
+{
+    const char *fn = "b2k_fkine_planar";
+    if (!c) { b2k_set_error("%s: chain handle is NULL", fn); return B2K_ERR_INVALID; }
+    if (dtype != B2K_F32 && dtype != B2K_F64) { b2k_set_error("%s: dtype must be B2K_F32 or B2K_F64", fn); return B2K_ERR_INVALID; }
+    if (c->n < 1 || c->n > B2K_MAX_JOINTS) { b2k_set_error("%s: unsupported joint count %d", fn, c->n); return B2K_ERR_INVALID; }
+    if (frame != 0 && frame != 1) { b2k_set_error("%s: frame must be 0 (jacob0) or 1 (jacobe), got %d", fn, frame); return B2K_ERR_INVALID; }
+    if (!T && !J) { b2k_set_error("%s: T and J are both NULL; nothing to compute", fn); return B2K_ERR_INVALID; }
+    int rc = b2k_planar_check(fn, c, base, tool);
+    if (rc) return rc;
+    if ((rc = check_common(fn, c, dtype, q, N, ldq))) return rc;
+    const unsigned es = dtype == B2K_F64 ? 8u : 4u;
+    if ((T && (rc = check_out(fn, "T", T, N, stage_unit(9 * es)))) || (J && (rc = check_out(fn, "J", J, N, stage_unit(3 * c->n * es)))))
+        return rc;
+    if (N == 0) return B2K_OK;
+    B2K_ON_DEVICE_OF(q);
+    return b2k_planar_launch(c, dtype, base, tool, frame, q, N, ldq, T, J, (cudaStream_t)stream);
+}
+
 // b2k_rne and b2k_rne_wrench (wrench: also the base wrench, wbase (N, 6)); every argument is checked before any CUDA call
 static int rne_run(const char *fn, b2k_rne_t r, int dtype, const void *q, const void *qd, const void *qdd, int64_t N,
                    const double *grav, const double *fext, void *tau, bool wrench, void *wbase, void *stream)

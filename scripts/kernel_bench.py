@@ -580,3 +580,51 @@ if want("ikine_qp_"):
                         mean_searches=float(ro.float().mean())))
             del qo, so, io, ro, Eo
         del Td
+
+# Planar chains (b2k_fkine_planar, csrc/b2k_planar.cu) through the C ABI: Planar2 (n = 2) and a 7-joint chain with R,
+# tx and ty joints, a flip and constants between joints, 1M rows.  Algorithmic bytes per row, sizeof(real) = es:
+# fkine (n + 9) es, jacob0 (n + 3n) es, fkine_jacob0 (n + 9 + 3n) es.  planar_3d_fkine_jacob0 is the 3-D kernel on the
+# same (embedded) chain, for context: it writes the 16 + 6n reals of the 3-D pose and Jacobian, and its share is stated
+# for the planar call's bytes.  The card's name and power limit are read in the same run.
+if want("planar_"):
+    import subprocess
+
+    try:
+        plim = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True,
+                              text=True, timeout=30).stdout.strip()
+    except Exception as e:  # the figure is context, the timing does not depend on it
+        plim = f"unavailable ({type(e).__name__})"
+    card = {"gpu": torch.cuda.get_device_name(0), "power_limit": plim}
+    E2 = rtb.ET2
+    planar7 = rtb.ETS2([E2.R(), E2.tx(0.4), E2.R(), E2.tx(0.3), E2.ty(), E2.R(), E2.tx(0.25), E2.R(flip=True), E2.tx(),
+                        E2.R(), E2.tx(0.1), E2.ty(0.05)])
+    Lp = rtb._lib.lib()
+    stp = torch.cuda.current_stream().cuda_stream
+    rngp = np.random.default_rng(8)
+    for fam, ets in (("planar2", rtb.models.ETS.Planar2().ets()), ("planar7", planar7)):
+        n = ets.n
+        for dt in (np.float64, np.float32):
+            es = np.dtype(dt).itemsize
+            tag = f"{fam}_{'f64' if dt == np.float64 else 'f32'}"
+            code = rtb._lib.F64 if dt == np.float64 else rtb._lib.F32
+            nbuf = min(8, max(2, int(np.ceil(300e6 / (N * n * es)))))
+            qs = [torch.from_numpy(rngp.uniform(-np.pi, np.pi, (N, n)).astype(dt)).to(dev) for _ in range(nbuf)]
+            T = torch.empty((N, 3, 3), dtype=tdt[dt], device=dev)
+            J = torch.empty((N, 3, n), dtype=tdt[dt], device=dev)
+            ch = ets._chain
+            for case, t, j, bpr in ((f"planar_fkine_{tag}", T, None, n + 9), (f"planar_jacob0_{tag}", None, J, 4 * n),
+                                    (f"planar_fkine_jacob0_{tag}", T, J, 4 * n + 9)):
+                if not want(case):
+                    continue
+                tp, jp = (None if t is None else t.data_ptr()), (None if j is None else j.data_ptr())
+                ms = timeit(lambda i: rtb._lib.check(Lp.b2k_fkine_planar(ch, code, qs[i].data_ptr(), N, n, None, None, 0, tp, jp, stp)), nbuf)
+                report(case, ms, N, bpr * es, dict(card, api="C ABI, q on the device", frac_of_3350=round(bpr * es * N / (ms * 1e-3) / 3.35e12, 4)))
+            case = f"planar_3d_fkine_jacob0_{tag}"
+            if want(case):
+                T3 = torch.empty((N, 4, 4), dtype=tdt[dt], device=dev)
+                J3 = torch.empty((N, 6, n), dtype=tdt[dt], device=dev)
+                ms = timeit(lambda i: rtb._lib.check(Lp.b2k_fkine_jacob0(ch, code, qs[i].data_ptr(), N, n, None, None, T3.data_ptr(), J3.data_ptr(), stp)), nbuf)
+                report(case, ms, N, (4 * n + 9) * es, dict(card, api="C ABI, 3-D kernel on the embedded chain", bytes_written_per_row=(16 + 6 * n) * es,
+                                                          frac_of_3350=round((4 * n + 9) * es * N / (ms * 1e-3) / 3.35e12, 4)))
+                del T3, J3
+            del qs, T, J
