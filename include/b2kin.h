@@ -237,6 +237,9 @@ int b2k_ikine_qp(b2k_chain_t chain, int dtype, const void *Tep, int64_t N, const
  *   grav : host 3-vector handed to the recursion as the base acceleration, i.e. MINUS the
  *          robot's gravity exactly as DHRobot.rne passes it (DHRobot.py:1449); must not be NULL
  *   fext : host 6-vector wrench at the tip or NULL (= zeros)
+ * q, qd, qdd need the alignment of their element type; tau is written in pieces of 16 bytes when a row of tau (n reals)
+ * is a multiple of 16 bytes, else 8 when it is a multiple of 8, else 4, and must be aligned to that piece (an fp64
+ * 6-joint tau: 16 bytes).  A misaligned or NULL (N > 0) array is rejected before any CUDA call.
  */
 int b2k_rne_create(int n, int mdh, const double *L, b2k_rne_t *out);
 int b2k_rne_destroy(b2k_rne_t rne);
@@ -253,7 +256,9 @@ int b2k_rne_wrench(b2k_rne_t rne, int dtype, const void *q, const void *qd, cons
 /* Robot-specialised kernels.  For all-revolute arms b2k_rne (and the dynamics entry points below) run a kernel that is
  * generated for THIS robot's link table and compiled for sm_90a at first use (NVRTC): terms whose link parameter is zero
  * are never emitted, alpha = k pi/2 turns rotations into permutations, constants are folded (csrc/b2k_rne_gen.cpp,
- * b2k_rne_spec.cu).  Results equal the generic kernel's to rounding.  Environment: B2K_RNE_SPEC=0 disables it, =2 makes a
+ * b2k_rne_spec.cu).  Results equal the generic kernel's to rounding.  A modified-DH arm with a prismatic first joint has a
+ * non-symmetric M under the kept reference treatment of that joint, which the specialised accel solve (pivot-free LDL^T)
+ * cannot handle: its accel is served by the generic kernel, and b2k_rne_fdyn refuses it.  Environment: B2K_RNE_SPEC=0 disables it, =2 makes a
  * failure to specialise an error; B2K_NVRTC_PATH names libnvrtc.so.12 when it is not on the loader path.
  *   b2k_rne_spec_info  writes a one-line description of the kernel that serves (mode, dtype, grav pattern, has_fext) for
  *                      this robot into buf -- mode: 0 rne, 1 inertia, 2 gravload, 3 itorque, 4 coriolis, 5 accel,
@@ -312,6 +317,9 @@ int b2k_tree_info(b2k_tree_t tree, int op, int dtype, const double *grav, char *
  *   b2k_rne_itorque   taui (N,n) = rne(q, 0, qdd, g=0)                          Dynamics.py:1407-1465
  *   b2k_rne_coriolis  C (N,n,n), on a friction-free copy of the robot           Dynamics.py:765-861
  *   b2k_rne_accel     qdd (N,n) = M^-1 (torque - rne(q, qd, 0, g)), friction kept  Dynamics.py:424-510
+ * Inputs need the alignment of their element type.  The output is written in pieces of 16 bytes when one of its rows (n
+ * or n*n reals) is a multiple of 16 bytes, else 8 when it is a multiple of 8, else 4, and must be aligned to that piece;
+ * a misaligned or NULL (N > 0) array is rejected before any CUDA call.
  */
 int b2k_rne_inertia(b2k_rne_t rne, int dtype, const void *q, int64_t N, void *M, void *stream);
 int b2k_rne_gravload(b2k_rne_t rne, int dtype, const void *q, int64_t N, const double *grav, void *taug, void *stream);

@@ -226,8 +226,9 @@ static int rne_run(const char *fn, b2k_rne_t r, int dtype, const void *q, const 
     if (!grav) { b2k_set_error("%s: grav is NULL (pass -robot.gravity like DHRobot.rne)", fn); return B2K_ERR_INVALID; }
     int rc;
     const unsigned es = dtype == B2K_F64 ? 8u : 4u;
+    // tau leaves through a per-warp stage of n-element rows, copied in stage_unit(n * es) pieces (b2k_rne.cuh)
     if ((rc = check_out(fn, "q", q, N, es)) || (rc = check_out(fn, "qd", qd, N, es)) || (rc = check_out(fn, "qdd", qdd, N, es)) ||
-        (rc = check_out(fn, "tau", tau, N, es)))
+        (rc = check_out(fn, "tau", tau, N, stage_unit((unsigned)r->n * es))))
         return rc;
     // a row of wbase is 3 pairs of reals: the kernels store it in 2-element units
     if (wrench && (rc = check_out(fn, "wbase", wbase, N, 2 * es))) return rc;
@@ -654,8 +655,10 @@ static int fan_dispatch(const char *fn, b2k_rne_t r, int dtype, int mode, const 
     if (need_grav && !grav) { b2k_set_error("%s: grav is NULL (pass -robot.gravity like DHRobot.rne)", fn); return B2K_ERR_INVALID; }
     int rc;
     const unsigned es = dtype == B2K_F64 ? 8u : 4u;
+    // the output leaves through a per-warp stage of rows of n (or n * n) elements, copied in stage_unit(row bytes) pieces
+    const unsigned out_row = (mode == FAN_INERTIA || mode == FAN_CORIOLIS) ? (unsigned)(r->n * r->n) : (unsigned)r->n;
     if ((rc = check_out(fn, "q", in0, N, es)) || (nin >= 2 && (rc = check_out(fn, "second input", in1, N, es))) ||
-        (nin >= 3 && (rc = check_out(fn, "third input", in2, N, es))) || (rc = check_out(fn, "output", out, N, es)))
+        (nin >= 3 && (rc = check_out(fn, "third input", in2, N, es))) || (rc = check_out(fn, "output", out, N, stage_unit(out_row * es))))
         return rc;
     if (N == 0) return B2K_OK;
     B2K_ON_DEVICE_OF(in0);
@@ -664,11 +667,10 @@ static int fan_dispatch(const char *fn, b2k_rne_t r, int dtype, int mode, const 
     if (done < 0) return (int)done;
     if (done == N) return B2K_OK;
     const size_t off = (size_t)done * r->n * es;
-    const size_t out_per_row = (mode == FAN_INERTIA || mode == FAN_CORIOLIS) ? (size_t)r->n * r->n : (size_t)r->n;
     in0 = (const char *)in0 + off;
     if (in1) in1 = (const char *)in1 + off;
     if (in2) in2 = (const char *)in2 + off;
-    out = (char *)out + (size_t)done * out_per_row * es;
+    out = (char *)out + (size_t)done * out_row * es;
     N -= done;
     if (dtype == B2K_F64) return b2k_rne_fan_launch_f64(r, mode, in0, in1, in2, N, grav, out, st);
     return b2k_rne_fan_launch_f32(r, mode, in0, in1, in2, N, grav, out, st);

@@ -683,6 +683,12 @@ GenFn dh_gen(const b2k_rne_s *r, const Key &key)
     return [r, key](b2k_gen_out &g) {
         b2k_gen_opts o;
         o.mode = std::get<0>(key); o.grav_mask = std::get<2>(key); o.has_fext = std::get<3>(key);
+        if (o.mode % 100 == B2K_GEN_ACCEL && r->mdh && (int)r->L[0][4] != 0) {
+            // the prismatic-first-joint treatment kept for modified DH (ne.c:187-204) makes M non-symmetric, and the
+            // accel kernels here solve with a pivot-free LDL^T that reads only M's lower triangle
+            g.error = "accel of a modified-DH arm with a prismatic first joint needs the pivoted solve of the generic kernel";
+            return -1;
+        }
         return b2k_rne_generate(r, o, g);
     };
 }
