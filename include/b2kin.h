@@ -317,6 +317,11 @@ int b2k_tree_info(b2k_tree_t tree, int op, int dtype, const double *grav, char *
  *   b2k_rne_itorque   taui (N,n) = rne(q, 0, qdd, g=0)                          Dynamics.py:1407-1465
  *   b2k_rne_coriolis  C (N,n,n), on a friction-free copy of the robot           Dynamics.py:765-861
  *   b2k_rne_accel     qdd (N,n) = M^-1 (torque - rne(q, qd, 0, g)), friction kept  Dynamics.py:424-510
+ *   b2k_rne_derivatives        dtau_dq, dtau_dqd (N,n,n), [i,k] = d tau_i / d x_k of tau = rne(q, qd, qdd, g, fext)
+ *                              (viscous friction adds G^2 B to the diagonal of dtau_dqd, Coulomb friction adds 0)
+ *   b2k_rne_accel_derivatives  at qdd* = b2k_rne_accel(q, qd, torque, g), with M = b2k_rne_inertia(q):
+ *                              dqdd_dq = -M^-1 dtau_dq, dqdd_dqd = -M^-1 dtau_dqd (both at qdd*), dqdd_dtau = M^-1
+ *   (no reference counterpart: exact forward-mode tangents of the recursion, one launch each; fext may be NULL)
  * Inputs need the alignment of their element type.  The output is written in pieces of 16 bytes when one of its rows (n
  * or n*n reals) is a multiple of 16 bytes, else 8 when it is a multiple of 8, else 4, and must be aligned to that piece;
  * a misaligned or NULL (N > 0) array is rejected before any CUDA call.
@@ -327,6 +332,10 @@ int b2k_rne_itorque(b2k_rne_t rne, int dtype, const void *q, const void *qdd, in
 int b2k_rne_coriolis(b2k_rne_t rne, int dtype, const void *q, const void *qd, int64_t N, void *C, void *stream);
 int b2k_rne_accel(b2k_rne_t rne, int dtype, const void *q, const void *qd, const void *torque, int64_t N,
                   const double *grav, void *qdd, void *stream);
+int b2k_rne_derivatives(b2k_rne_t rne, int dtype, const void *q, const void *qd, const void *qdd, int64_t N,
+                        const double *grav, const double *fext, void *dtau_dq, void *dtau_dqd, void *stream);
+int b2k_rne_accel_derivatives(b2k_rne_t rne, int dtype, const void *q, const void *qd, const void *torque, int64_t N,
+                              const double *grav, void *dqdd_dq, void *dqdd_dqd, void *dqdd_dtau, void *stream);
 
 /* ---------------------------------------------------------------- static forces (DynamicsMixin, robot/Dynamics.py)
  * One forward walk over a compiled chain per row (base and tool as the chain has them, as for b2k_jacob0); q is (N, ldq)

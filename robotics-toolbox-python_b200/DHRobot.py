@@ -475,10 +475,17 @@ class DHRobot:
 
     _RNE_MODES = {"rne": 0, "inertia": 1, "gravload": 2, "itorque": 3, "coriolis": 4, "accel": 5, "rne_wrench": 6}
 
+    _DERIV_OPS = {"rne_derivatives": "inverse", "accel_derivatives": "forward"}
+
     def rne_kernel_info(self, op="rne", dtype=np.float64, gravity=None, fext=None) -> str:
         """Which kernel serves `op` for this robot: the robot-specialised one (generated from the link table and
         compiled with NVRTC at first use; the line lists its multiply / FMA / add count per row, registers and
         shared memory) or the pre-compiled generic one, with the reason."""
+        if op in self._DERIV_OPS:
+            allrev = all(l.sigma == 0 for l in self.links)
+            return (f"generic k_rne_deriv<{'double' if np.dtype(dtype) == np.float64 else 'float'}, n={self.n}, {'MDH' if self.mdh else 'DH'}, "
+                    f"{'all-revolute' if allrev else 'prismatic'}, {self._DERIV_OPS[op]}> (the robot-specialised path "
+                    "generates no derivative kernels)")
         if self._rne_ob is None or self._dynchanged:
             self.delete_rne()
             self._init_rne()
@@ -490,8 +497,9 @@ class DHRobot:
         return buf.value.decode()
 
     # ---- dynamics built on the recursion (reference DynamicsMixin, Dynamics.py; SURVEY 8f-1)
-    def _dyn(self, fn_name, ins, out_tail, gravity=None, use_gravity=False, dtype=None):
-        """Shared front end of the fan-out kernels: every input (N,n) or (n,), one launch."""
+    def _dyn(self, fn_name, ins, out_tail, gravity=None, use_gravity=False, dtype=None, fext=None, use_fext=False, n_out=1):
+        """Shared front end of the fan-out kernels: every input (N,n) or (n,), one launch.  With n_out > 1 the kernel
+        writes that many outputs of the same shape, returned as a tuple."""
         if self._rne_ob is None or self._dynchanged:
             self.delete_rne()
             self._init_rne()
@@ -510,17 +518,21 @@ class DHRobot:
         for t in dev:
             if t.dim() != 2 or tuple(t.shape) != (N, n):
                 raise ValueError(f"inputs must have shape ({n},) or (N,{n}); got {tuple(t.shape)}")
-        out = B.empty((N,) + out_tail, dt, like=dev[0])
+        outs = [B.empty((N,) + out_tail, dt, like=dev[0]) for _ in range(n_out)]
         args = [self._rne_ob, B.code(dt)] + [B.ptr(t) for t in dev] + [N]
         if use_gravity:
             g = self._gravity if gravity is None else np.asarray(gravity, dtype=np.float64).reshape(3)
             g = np.ascontiguousarray(-(self._base[:3, :3].T @ g))  # as DHRobot.rne: reference 1431-1433, 1449
             args.append(_lib.dptr(g))
-        args += [B.ptr(out), B.stream_ptr(dev[0])]
+        if use_fext:
+            fx = None if fext is None else np.ascontiguousarray(np.asarray(fext, dtype=np.float64).reshape(6))
+            args.append(_lib.dptr(fx))
+        args += [B.ptr(o) for o in outs] + [B.stream_ptr(dev[0])]
         _lib.check(getattr(_lib.lib(), fn_name)(*args))
         if host:
-            out = B.to_host(out)
-        return out[0] if single else out
+            outs = [B.to_host(o) for o in outs]
+        outs = [o[0] if single else o for o in outs]
+        return outs[0] if n_out == 1 else tuple(outs)
 
     def inertia(self, q, dtype=None):
         """Joint-space inertia matrix M(q): (n,n) or (N,n,n) (reference Dynamics.inertia, Dynamics.py:704-763)."""
@@ -542,6 +554,30 @@ class DHRobot:
         """Forward dynamics qdd = M(q)^-1 (torque - rne(q, qd, 0)), joint friction included
         (reference Dynamics.accel, Dynamics.py:424-510)."""
         return self._dyn("b2k_rne_accel", [q, qd, torque], (self.n,), gravity=gravity, use_gravity=True, dtype=dtype)
+
+    def rne_derivatives(self, q, qd, qdd, gravity=None, fext=None, dtype=None):
+        """Exact first derivatives of inverse dynamics: ``(dtau_dq, dtau_dqd)``, each (n,n) for one state or (N,n,n).
+
+        Layout: ``[..., i, k] = d tau_i / d x_k`` -- rows are torques, columns the variable (numpy's Jacobian
+        convention).  tau is exactly what ``rne(q, qd, qdd, gravity, fext)`` computes: gravity rotated by the base, the
+        tip wrench, the armature term G^2 Jm qdd and joint friction.  Viscous friction adds G^2 B to the diagonal of
+        ``dtau_dqd``; Coulomb friction is piecewise constant and adds 0 (also at qd = 0, where rne uses 0).  A
+        prismatic joint is differentiated through d = q + offset.  Where rne keeps a reference quirk (the modified-DH
+        prismatic first joint, ``flip`` ignored) this is the derivative of what the recursion computes.  d tau / d qdd
+        is ``inertia(q)``.  The values are forward-mode tangents through the recursion (no finite differences), one
+        kernel launch for the whole batch."""
+        return self._dyn("b2k_rne_derivatives", [q, qd, qdd], (self.n, self.n), gravity=gravity, use_gravity=True, dtype=dtype,
+                         fext=fext, use_fext=True, n_out=2)
+
+    def accel_derivatives(self, q, qd, torque, gravity=None, dtype=None):
+        """Exact first derivatives of forward dynamics: ``(dqdd_dq, dqdd_dqd, dqdd_dtau)``, each (n,n) or (N,n,n), in
+        the layout of ``rne_derivatives`` (``[..., i, k] = d qdd_i / d x_k``).
+
+        With qdd* = ``accel(q, qd, torque, gravity)`` (friction kept as accel keeps it) and M = ``inertia(q)``:
+        ``dqdd_dq = -M^-1 dtau_dq`` and ``dqdd_dqd = -M^-1 dtau_dqd``, the inverse-dynamics derivatives taken at qdd*,
+        and ``dqdd_dtau = M^-1``.  All three come from one kernel launch."""
+        return self._dyn("b2k_rne_accel_derivatives", [q, qd, torque], (self.n, self.n), gravity=gravity, use_gravity=True,
+                         dtype=dtype, n_out=3)
 
     # ---- static forces (reference DynamicsMixin, Dynamics.py): _static.py, csrc/b2k_static.cu
     def _static_mass_table(self) -> np.ndarray:

@@ -697,3 +697,48 @@ extern "C" int b2k_rne_accel(b2k_rne_t r, int dtype, const void *q, const void *
 {
     return fan_dispatch("b2k_rne_accel", r, dtype, FAN_ACCEL, q, qd, torque, 3, N, grav, true, qdd, stream);
 }
+
+// ------------------------------------------------------------------ analytical derivatives of the recursion (b2k_rne.cuh)
+int b2k_rne_deriv_launch_f32(const b2k_rne_s *, int, const void *, const void *, const void *, long long, const double *,
+                             const double *, void *, void *, void *, cudaStream_t);
+int b2k_rne_deriv_launch_f64(const b2k_rne_s *, int, const void *, const void *, const void *, long long, const double *,
+                             const double *, void *, void *, void *, cudaStream_t);
+enum { DERIV_INVERSE = 0, DERIV_FORWARD = 1 };
+
+// the generic kernel serves every row: the robot-specialised path has no derivative kernels
+static int deriv_dispatch(const char *fn, b2k_rne_t r, int dtype, int mode, const void *in0, const void *in1, const void *in2,
+                          int64_t N, const double *grav, const double *fext, void *out0, void *out1, void *out2, void *stream)
+{
+    if (!r) { b2k_set_error("%s: rne handle is NULL", fn); return B2K_ERR_INVALID; }
+    if (dtype != B2K_F32 && dtype != B2K_F64) { b2k_set_error("%s: dtype must be B2K_F32 or B2K_F64", fn); return B2K_ERR_INVALID; }
+    if (N < 0) { b2k_set_error("%s: N is negative", fn); return B2K_ERR_INVALID; }
+    if (r->n < 1 || r->n > B2K_MAX_JOINTS) { b2k_set_error("%s: unsupported joint count %d", fn, r->n); return B2K_ERR_INVALID; }
+    if (!grav) { b2k_set_error("%s: grav is NULL (pass -robot.gravity like DHRobot.rne)", fn); return B2K_ERR_INVALID; }
+    int rc;
+    const unsigned es = dtype == B2K_F64 ? 8u : 4u;
+    // every output leaves through a per-warp stage of n*n-element rows, copied in stage_unit(n * n * es) pieces
+    const unsigned ou = stage_unit((unsigned)(r->n * r->n) * es);
+    const bool fwd = mode == DERIV_FORWARD;
+    if ((rc = check_out(fn, "q", in0, N, es)) || (rc = check_out(fn, "qd", in1, N, es)) ||
+        (rc = check_out(fn, fwd ? "torque" : "qdd", in2, N, es)) || (rc = check_out(fn, fwd ? "dqdd_dq" : "dtau_dq", out0, N, ou)) ||
+        (rc = check_out(fn, fwd ? "dqdd_dqd" : "dtau_dqd", out1, N, ou)) || (fwd && (rc = check_out(fn, "dqdd_dtau", out2, N, ou))))
+        return rc;
+    if (N == 0) return B2K_OK;
+    B2K_ON_DEVICE_OF(in0);
+    auto launch = dtype == B2K_F64 ? b2k_rne_deriv_launch_f64 : b2k_rne_deriv_launch_f32;
+    return launch(r, mode, in0, in1, in2, N, grav, fext, out0, out1, out2, (cudaStream_t)stream);
+}
+
+extern "C" int b2k_rne_derivatives(b2k_rne_t r, int dtype, const void *q, const void *qd, const void *qdd, int64_t N,
+                                   const double *grav, const double *fext, void *dtau_dq, void *dtau_dqd, void *stream)
+{
+    return deriv_dispatch("b2k_rne_derivatives", r, dtype, DERIV_INVERSE, q, qd, qdd, N, grav, fext, dtau_dq, dtau_dqd, nullptr,
+                          stream);
+}
+
+extern "C" int b2k_rne_accel_derivatives(b2k_rne_t r, int dtype, const void *q, const void *qd, const void *torque, int64_t N,
+                                         const double *grav, void *dqdd_dq, void *dqdd_dqd, void *dqdd_dtau, void *stream)
+{
+    return deriv_dispatch("b2k_rne_accel_derivatives", r, dtype, DERIV_FORWARD, q, qd, torque, N, grav, nullptr, dqdd_dq,
+                          dqdd_dqd, dqdd_dtau, stream);
+}

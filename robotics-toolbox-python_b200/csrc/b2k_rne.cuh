@@ -35,28 +35,64 @@ struct RneP {
     TrigC<real> trig;
 };
 
+// Forward-mode dual scalar: value v and tangent d = dv/dx for one seeded input x.  The recursions below are templated on
+// their value type V (real, or Dual<real> for the derivative kernels); link constants stay real, so a product of a
+// constant and a dual costs two multiplies, not the four of a dual-by-dual product.
+template <typename real>
+struct Dual {
+    real v, d;
+    Dual() = default;
+    __device__ __forceinline__ Dual(real x) : v(x), d(0) {}
+    __device__ __forceinline__ Dual(real x, real dx) : v(x), d(dx) {}
+    __device__ __forceinline__ Dual operator-() const { return {-v, -d}; }
+    __device__ __forceinline__ Dual &operator+=(Dual b) { v += b.v; d += b.d; return *this; }
+    __device__ __forceinline__ Dual &operator+=(real b) { v += b; return *this; }
+    friend __device__ __forceinline__ Dual operator+(Dual a, Dual b) { return {a.v + b.v, a.d + b.d}; }
+    friend __device__ __forceinline__ Dual operator+(Dual a, real b) { return {a.v + b, a.d}; }
+    friend __device__ __forceinline__ Dual operator+(real a, Dual b) { return {a + b.v, b.d}; }
+    friend __device__ __forceinline__ Dual operator-(Dual a, Dual b) { return {a.v - b.v, a.d - b.d}; }
+    friend __device__ __forceinline__ Dual operator*(Dual a, Dual b) { return {a.v * b.v, fma(a.v, b.d, a.d * b.v)}; }
+    friend __device__ __forceinline__ Dual operator*(real a, Dual b) { return {a * b.v, a * b.d}; }
+    friend __device__ __forceinline__ Dual operator*(Dual a, real b) { return {a.v * b, a.d * b}; }
+    friend __device__ __forceinline__ Dual fma(Dual a, Dual b, Dual c) { return {fma(a.v, b.v, c.v), fma(a.v, b.d, fma(a.d, b.v, c.d))}; }
+    friend __device__ __forceinline__ Dual fma(real a, Dual b, Dual c) { return {fma(a, b.v, c.v), fma(a, b.d, c.d)}; }
+    friend __device__ __forceinline__ Dual fma(Dual a, real b, Dual c) { return {fma(a.v, b, c.v), fma(a.d, b, c.d)}; }
+    friend __device__ __forceinline__ Dual fma(Dual a, Dual b, real c) { return {fma(a.v, b.v, c), fma(a.v, b.d, a.d * b.v)}; }
+    friend __device__ __forceinline__ Dual fma(real a, Dual b, real c) { return {fma(a, b.v, c), a * b.d}; }
+    friend __device__ __forceinline__ Dual fma(Dual a, real b, real c) { return {fma(a.v, b, c), a.d * b}; }
+    friend __device__ __forceinline__ Dual fma(real a, real b, Dual c) { return {fma(a, b, c.v), c.d}; }
+    // branches (Coulomb friction) follow the value: the tangent of a piecewise-constant term is 0
+    friend __device__ __forceinline__ bool operator>(Dual a, real b) { return a.v > b; }
+    friend __device__ __forceinline__ bool operator<(Dual a, real b) { return a.v < b; }
+};
+
 template <typename real>
 struct V3 {
     real x, y, z;
 };
-template <typename real> __device__ __forceinline__ V3<real> vadd(V3<real> a, V3<real> b) { return {a.x + b.x, a.y + b.y, a.z + b.z}; }
-template <typename real> __device__ __forceinline__ V3<real> vcross(V3<real> a, V3<real> b)
+// Mixed operands (a dual vector and a constant one) give a vector of the wider type; with one type they are the plain ops.
+template <typename A, typename B>
+__device__ __forceinline__ auto vadd(V3<A> a, V3<B> b) -> V3<decltype(a.x + b.x)> { return {a.x + b.x, a.y + b.y, a.z + b.z}; }
+template <typename A, typename B>
+__device__ __forceinline__ auto vcross(V3<A> a, V3<B> b) -> V3<decltype(a.x * b.x)>
 {
     return {a.y * b.z - a.z * b.y, a.z * b.x - a.x * b.z, a.x * b.y - a.y * b.x};
 }
 // a x b + c with the addition folded into the products (2 FMA per component instead of MUL + FMA + ADD)
-template <typename real> __device__ __forceinline__ V3<real> vcross_acc(V3<real> a, V3<real> b, V3<real> c)
+template <typename A, typename B, typename C>
+__device__ __forceinline__ V3<C> vcross_acc(V3<A> a, V3<B> b, V3<C> c)
 {
     return {fma(a.y, b.z, fma(-a.z, b.y, c.x)), fma(a.z, b.x, fma(-a.x, b.z, c.y)), fma(a.x, b.y, fma(-a.y, b.x, c.z))};
 }
-template <typename real> __device__ __forceinline__ V3<real> vscale(V3<real> a, real s) { return {s * a.x, s * a.y, s * a.z}; }
-template <typename real> __device__ __forceinline__ real vdot(V3<real> a, V3<real> b) { return a.x * b.x + a.y * b.y + a.z * b.z; }
+template <typename V, typename real> __device__ __forceinline__ V3<V> vscale(V3<V> a, real s) { return {s * a.x, s * a.y, s * a.z}; }
+template <typename A, typename B>
+__device__ __forceinline__ auto vdot(V3<A> a, V3<B> b) -> decltype(a.x * b.x) { return a.x * b.x + a.y * b.y + a.z * b.z; }
 
 // link rotation R (columns n, o, a) from sin/cos(theta), sin/cos(alpha); frne.c:329-347
-template <typename real, bool MDH>
+template <typename real, bool MDH, typename V = real>
 struct LinkRot {
-    real nx, ny, nz, ox, oy, oz, ax, ay, az;
-    __device__ __forceinline__ LinkRot(real st, real ct, real sa, real ca)
+    V nx, ny, nz, ox, oy, oz, ax, ay, az;
+    __device__ __forceinline__ LinkRot(V st, V ct, real sa, real ca)
     {
         if (!MDH) {
             nx = ct; ox = -ca * st; ax = sa * st;
@@ -68,11 +104,11 @@ struct LinkRot {
             nz = st * sa; oz = ct * sa; az = ca;
         }
     }
-    __device__ __forceinline__ V3<real> mul(V3<real> v) const
+    __device__ __forceinline__ V3<V> mul(V3<V> v) const
     {
         return {nx * v.x + ox * v.y + ax * v.z, ny * v.x + oy * v.y + ay * v.z, nz * v.x + oz * v.y + az * v.z};
     }
-    __device__ __forceinline__ V3<real> tmul(V3<real> v) const
+    __device__ __forceinline__ V3<V> tmul(V3<V> v) const
     {
         return {nx * v.x + ny * v.y + nz * v.z, ox * v.x + oy * v.y + oz * v.z, ax * v.x + ay * v.y + az * v.z};
     }
@@ -84,54 +120,55 @@ struct LinkRot {
 // product with its structural zeros), z-only joint-rate vectors expanded by hand (the compiler
 // may not drop IEEE multiplications by a literal 0), p* taken from the constant bank, and
 // R_{j+1} f_{j+1} computed once per link.  Dropping exact-zero terms does not change any value.
-template <typename real, bool MDH>
+template <typename real, bool MDH, typename V = real>
 struct FRot { // factored link rotation
-    real st, ct, sa, ca;
-    __device__ __forceinline__ V3<real> tmul(V3<real> v) const // R^T v
+    V st, ct;
+    real sa, ca;
+    template <typename X> __device__ __forceinline__ V3<V> tmul(V3<X> v) const // R^T v
     {
         if (!MDH) {
-            const real u = fma(ct, v.x, st * v.y), w = fma(ct, v.y, -(st * v.x));
+            const auto u = fma(ct, v.x, st * v.y), w = fma(ct, v.y, -(st * v.x));
             return {u, fma(ca, w, sa * v.z), fma(ca, v.z, -(sa * w))};
         } else {
-            const real wy = fma(ca, v.y, sa * v.z), wz = fma(ca, v.z, -(sa * v.y));
+            const auto wy = fma(ca, v.y, sa * v.z), wz = fma(ca, v.z, -(sa * v.y));
             return {fma(ct, v.x, st * wy), fma(ct, wy, -(st * v.x)), wz};
         }
     }
-    __device__ __forceinline__ V3<real> mul(V3<real> v) const // R v
+    template <typename X> __device__ __forceinline__ V3<V> mul(V3<X> v) const // R v
     {
         if (!MDH) {
-            const real m = fma(ca, v.y, -(sa * v.z)), z = fma(sa, v.y, ca * v.z);
+            const auto m = fma(ca, v.y, -(sa * v.z)), z = fma(sa, v.y, ca * v.z);
             return {fma(ct, v.x, -(st * m)), fma(st, v.x, ct * m), z};
         } else {
-            const real u = fma(ct, v.x, -(st * v.y)), w = fma(st, v.x, ct * v.y);
+            const auto u = fma(ct, v.x, -(st * v.y)), w = fma(st, v.x, ct * v.y);
             return {u, fma(ca, w, -(sa * v.z)), fma(sa, w, ca * v.z)};
         }
     }
     // R^T v + c and R v + c with c folded into the last stage of FMAs (no separate additions)
-    __device__ __forceinline__ V3<real> tmul_acc(V3<real> v, V3<real> c) const
+    __device__ __forceinline__ V3<V> tmul_acc(V3<V> v, V3<V> c) const
     {
         if (!MDH) {
-            const real w = fma(ct, v.y, -(st * v.x));
+            const auto w = fma(ct, v.y, -(st * v.x));
             return {fma(ct, v.x, fma(st, v.y, c.x)), fma(ca, w, fma(sa, v.z, c.y)), fma(ca, v.z, fma(-sa, w, c.z))};
         } else {
-            const real wy = fma(ca, v.y, sa * v.z);
+            const auto wy = fma(ca, v.y, sa * v.z);
             return {fma(ct, v.x, fma(st, wy, c.x)), fma(ct, wy, fma(-st, v.x, c.y)), fma(ca, v.z, fma(-sa, v.y, c.z))};
         }
     }
-    __device__ __forceinline__ V3<real> mul_acc(V3<real> v, V3<real> c) const
+    __device__ __forceinline__ V3<V> mul_acc(V3<V> v, V3<V> c) const
     {
         if (!MDH) {
-            const real m = fma(ca, v.y, -(sa * v.z));
+            const auto m = fma(ca, v.y, -(sa * v.z));
             return {fma(ct, v.x, fma(-st, m, c.x)), fma(st, v.x, fma(ct, m, c.y)), fma(sa, v.y, fma(ca, v.z, c.z))};
         } else {
-            const real w = fma(st, v.x, ct * v.y);
+            const auto w = fma(st, v.x, ct * v.y);
             return {fma(ct, v.x, fma(-st, v.y, c.x)), fma(ca, w, fma(-sa, v.z, c.y)), fma(sa, w, fma(ca, v.z, c.z))};
         }
     }
 };
 
-template <typename real>
-__device__ __forceinline__ V3<real> imul(const real *I, V3<real> v) // vmath.c mat_vect_mult (column-major read)
+template <typename real, typename V>
+__device__ __forceinline__ V3<V> imul(const real *I, V3<V> v) // vmath.c mat_vect_mult (column-major read)
 {
     return {fma(I[0], v.x, fma(I[3], v.y, I[6] * v.z)), fma(I[1], v.x, fma(I[4], v.y, I[7] * v.z)),
             fma(I[2], v.x, fma(I[5], v.y, I[8] * v.z))};
@@ -164,64 +201,64 @@ __device__ __forceinline__ void rne_put_wrench(V3<real> f0, V3<real> n0, real *w
     wb[3] = n0.x; wb[4] = n0.y; wb[5] = n0.z;
 }
 
-template <typename real, int N, bool MDH, bool WRENCH = false>
-__device__ __forceinline__ void rne_row_allrev(const RneP<real, N> &P, const real *sth, const real *cth, const real *mqd,
-                                               const real *mqdd, V3<real> gravity, real *tq, real *wb = nullptr)
+template <typename real, int N, bool MDH, bool WRENCH = false, typename V = real>
+__device__ __forceinline__ void rne_row_allrev(const RneP<real, N> &P, const V *sth, const V *cth, const V *mqd,
+                                               const V *mqdd, V3<V> gravity, V *tq, V *wb = nullptr)
 {
-    V3<real> Fm[N], Nm[N];
-    V3<real> w = {0, 0, 0}, wd = {0, 0, 0}, acc = {0, 0, 0};
+    V3<V> Fm[N], Nm[N];
+    V3<V> w = {0, 0, 0}, wd = {0, 0, 0}, acc = {0, 0, 0};
 #pragma unroll
     for (int j = 0; j < N; j++) {
-        const FRot<real, MDH> R = {sth[j], cth[j], P.sa[j], P.ca[j]};
+        const FRot<real, MDH, V> R = {sth[j], cth[j], P.sa[j], P.ca[j]};
         const V3<real> ps = {P.ps[j][0], P.ps[j][1], P.ps[j][2]};
-        const real qd = mqd[j], qdd = mqdd[j];
-        V3<real> wn, wdn, accn;
+        const V qd = mqd[j], qdd = mqdd[j];
+        V3<V> wn, wdn, accn;
         if (MDH) { // ne.c:144-181
             if (j == 0) {
                 wn = {0, 0, qd};
                 wdn = {0, 0, qdd};
                 accn = R.tmul(gravity);
             } else {
-                const V3<real> t1 = R.tmul(w);
+                const V3<V> t1 = R.tmul(w);
                 wn = {t1.x, t1.y, t1.z + qd};
-                const V3<real> t3 = R.tmul(wd);
+                const V3<V> t3 = R.tmul(wd);
                 wdn = {fma(t1.y, qd, t3.x), fma(-t1.x, qd, t3.y), t3.z + qdd}; // t1 x (0,0,qd) + t3 + (0,0,qdd)
-                V3<real> a = vcross(w, ps);
+                V3<V> a = vcross(w, ps);
                 a = vcross_acc(w, a, acc);
                 a = vcross_acc(wd, ps, a);
                 accn = R.tmul(a);
             }
         } else { // ne.c:252-288
             if (j == 0) {
-                wn = R.tmul(V3<real>{0, 0, qd});
-                wdn = R.tmul(V3<real>{0, 0, qdd});
+                wn = R.tmul(V3<V>{0, 0, qd});
+                wdn = R.tmul(V3<V>{0, 0, qdd});
             } else {
-                wn = R.tmul(V3<real>{w.x, w.y, w.z + qd});
-                wdn = R.tmul(V3<real>{fma(w.y, qd, wd.x), fma(-w.x, qd, wd.y), wd.z + qdd});
+                wn = R.tmul(V3<V>{w.x, w.y, w.z + qd});
+                wdn = R.tmul(V3<V>{fma(w.y, qd, wd.x), fma(-w.x, qd, wd.y), wd.z + qdd});
             }
-            const V3<real> t2 = vcross(wn, ps);
+            const V3<V> t2 = vcross(wn, ps);
             accn = R.tmul_acc(j == 0 ? gravity : acc, vcross_acc(wdn, ps, vcross(wn, t2)));
         }
         w = wn; wd = wdn; acc = accn;
         const V3<real> rc = {P.r[j][0], P.r[j][1], P.r[j][2]};
-        const V3<real> abar = vcross_acc(wd, rc, vcross_acc(w, vcross(w, rc), acc));
+        const V3<V> abar = vcross_acc(wd, rc, vcross_acc(w, vcross(w, rc), acc));
         Fm[j] = vscale(abar, P.m[j]);
         Nm[j] = vcross_acc(w, imul(P.I[j], w), imul(P.I[j], wd));
     }
-    V3<real> f = {0, 0, 0}, nn = {0, 0, 0};
+    V3<V> f = {0, 0, 0}, nn = {0, 0, 0};
     const V3<real> f_tip = {P.fext[0], P.fext[1], P.fext[2]}, n_tip = {P.fext[3], P.fext[4], P.fext[5]};
 #pragma unroll
     for (int j = N - 1; j >= 0; j--) {
         const V3<real> rc = {P.r[j][0], P.r[j][1], P.r[j][2]};
-        V3<real> fj, nj;
+        V3<V> fj, nj;
         if (MDH) { // ne.c:358-398
             if (j == N - 1) {
                 fj = vadd(f_tip, Fm[j]);
                 nj = vadd(n_tip, Nm[j]);
             } else {
-                const FRot<real, MDH> Rn = {sth[j + 1], cth[j + 1], P.sa[j + 1], P.ca[j + 1]};
+                const FRot<real, MDH, V> Rn = {sth[j + 1], cth[j + 1], P.sa[j + 1], P.ca[j + 1]};
                 const V3<real> psn = {P.ps[j + 1][0], P.ps[j + 1][1], P.ps[j + 1][2]};
-                const V3<real> Rf = Rn.mul(f);
+                const V3<V> Rf = Rn.mul(f);
                 fj = vadd(Rf, Fm[j]);
                 nj = Rn.mul_acc(nn, vcross_acc(psn, Rf, Nm[j]));
             }
@@ -229,11 +266,11 @@ __device__ __forceinline__ void rne_row_allrev(const RneP<real, N> &P, const rea
         } else { // ne.c:409-453
             const V3<real> ps = {P.ps[j][0], P.ps[j][1], P.ps[j][2]};
             const V3<real> psrc = {P.psrc[j][0], P.psrc[j][1], P.psrc[j][2]};
-            V3<real> t1 = vcross_acc(psrc, Fm[j], Nm[j]);
+            V3<V> t1 = vcross_acc(psrc, Fm[j], Nm[j]);
             if (j != N - 1) {
-                const FRot<real, MDH> Rn = {sth[j + 1], cth[j + 1], P.sa[j + 1], P.ca[j + 1]};
+                const FRot<real, MDH, V> Rn = {sth[j + 1], cth[j + 1], P.sa[j + 1], P.ca[j + 1]};
                 fj = Rn.mul_acc(f, Fm[j]);
-                const V3<real> t3 = vcross_acc(Rn.tmul(ps), f, nn);
+                const V3<V> t3 = vcross_acc(Rn.tmul(ps), f, nn);
                 t1 = Rn.mul_acc(t3, t1);
             } else {
                 fj = vadd(Fm[j], f_tip);
@@ -242,16 +279,16 @@ __device__ __forceinline__ void rne_row_allrev(const RneP<real, N> &P, const rea
             nj = t1;
         }
         f = fj; nn = nj;
-        real t = MDH ? nj.z : fma(nj.y, P.sa[j], nj.z * P.ca[j]); // n . (R^T z0)
-        const real qdj = mqd[j];
+        V t = MDH ? nj.z : fma(nj.y, P.sa[j], nj.z * P.ca[j]); // n . (R^T z0)
+        const V qdj = mqd[j];
         t = fma(P.c_jm[j], mqdd[j], t);
         t = fma(P.c_b[j], qdj, t);
         t += (qdj > 0 ? P.c_tcp[j] : (real)0) + (qdj < 0 ? P.c_tcm[j] : (real)0);
         tq[j] = t;
     }
     if constexpr (WRENCH) {
-        const FRot<real, MDH> R = {sth[0], cth[0], P.sa[0], P.ca[0]};
-        const V3<real> f0 = R.mul(f);
+        const FRot<real, MDH, V> R = {sth[0], cth[0], P.sa[0], P.ca[0]};
+        const V3<V> f0 = R.mul(f);
         const V3<real> ps = {P.ps[0][0], P.ps[0][1], P.ps[0][2]};
         rne_put_wrench(f0, MDH ? R.mul_acc(nn, vcross(ps, f0)) : R.mul(nn), wb);
     }
@@ -260,26 +297,26 @@ __device__ __forceinline__ void rne_row_allrev(const RneP<real, N> &P, const rea
 // ------------------------------------------------------------------ generic row (any mix of revolute / prismatic links)
 // Mirrors ne.c operation by operation, including its quirks for a prismatic first joint under
 // modified DH (ne.c:187-204).
-template <typename real, int N, bool MDH, bool WRENCH = false>
-__device__ __forceinline__ void rne_row_generic(const RneP<real, N> &P, const real *mq, const real *sth, const real *cth,
-                                                const real *mqd, const real *mqdd, V3<real> gravity, real *tq,
-                                                real *wb = nullptr)
+template <typename real, int N, bool MDH, bool WRENCH = false, typename V = real>
+__device__ __forceinline__ void rne_row_generic(const RneP<real, N> &P, const V *mq, const V *sth, const V *cth,
+                                                const V *mqd, const V *mqdd, V3<V> gravity, V *tq,
+                                                V *wb = nullptr)
 {
     // stash for the backward recursion
-    V3<real> Fm[N], Nm[N];
+    V3<V> Fm[N], Nm[N];
     // (gravity: base acceleration handed in by the caller)
-    V3<real> w = {0, 0, 0}, wd = {0, 0, 0}, acc = {0, 0, 0}; // of link j-1 on entry
+    V3<V> w = {0, 0, 0}, wd = {0, 0, 0}, acc = {0, 0, 0}; // of link j-1 on entry
 
     // ---------------- forward recursion (ne.c:137-240 MDH, 245-347 DH)
 #pragma unroll
     for (int j = 0; j < N; j++) {
         const bool pris = (P.prismatic[j] != 0);
-        const real st = sth[j], ct = cth[j];
-        const real d = pris ? (mq[j] + P.offset[j]) : P.D[j];
-        const LinkRot<real, MDH> R(st, ct, P.sa[j], P.ca[j]);
-        const V3<real> pstar = MDH ? V3<real>{P.A[j], -d * P.sa[j], d * P.ca[j]} : V3<real>{P.A[j], d * P.sa[j], d * P.ca[j]};
-        const V3<real> qdv = {0, 0, mqd[j]}, qddv = {0, 0, mqdd[j]};
-        V3<real> wn, wdn, accn, t1, t2, t3;
+        const V st = sth[j], ct = cth[j];
+        const V d = pris ? (mq[j] + P.offset[j]) : P.D[j];
+        const LinkRot<real, MDH, V> R(st, ct, P.sa[j], P.ca[j]);
+        const V3<V> pstar = MDH ? V3<V>{P.A[j], -d * P.sa[j], d * P.ca[j]} : V3<V>{P.A[j], d * P.sa[j], d * P.ca[j]};
+        const V3<V> qdv = {0, 0, mqd[j]}, qddv = {0, 0, mqdd[j]};
+        V3<V> wn, wdn, accn, t1, t2, t3;
         if (MDH) {
             if (!pris) {
                 if (j == 0) {
@@ -362,7 +399,7 @@ __device__ __forceinline__ void rne_row_generic(const RneP<real, N> &P, const re
         t1 = vcross(wd, rc);
         t2 = vcross(w, rc);
         t3 = vcross(w, t2);
-        V3<real> abar = vadd(t1, t3);
+        V3<V> abar = vadd(t1, t3);
         abar = vadd(abar, acc);
         Fm[j] = vscale(abar, P.m[j]);
         const real *I = P.I[j]; // read column-major like vmath.c mat_vect_mult
@@ -374,22 +411,22 @@ __device__ __forceinline__ void rne_row_generic(const RneP<real, N> &P, const re
     }
 
     // ---------------- backward recursion (ne.c:358-403 MDH, 409-457 DH) + joint torque (ne.c:464-491)
-    V3<real> f = {0, 0, 0}, nn = {0, 0, 0}; // of link j+1 on entry
+    V3<V> f = {0, 0, 0}, nn = {0, 0, 0}; // of link j+1 on entry
     const V3<real> f_tip = {P.fext[0], P.fext[1], P.fext[2]}, n_tip = {P.fext[3], P.fext[4], P.fext[5]};
 #pragma unroll
     for (int j = N - 1; j >= 0; j--) {
         const bool pris = (P.prismatic[j] != 0);
         const V3<real> rc = {P.r[j][0], P.r[j][1], P.r[j][2]};
-        V3<real> fj, nj, t1, t2, t3, t4;
+        V3<V> fj, nj, t1, t2, t3, t4;
         if (MDH) {
-            const V3<real> F = Fm[j];
+            const V3<V> F = Fm[j];
             if (j == N - 1) {
                 fj = vadd(f_tip, F);
-                t1 = n_tip;
+                t1 = {n_tip.x, n_tip.y, n_tip.z};
             } else {
-                const LinkRot<real, MDH> Rn(sth[j + 1], cth[j + 1], P.sa[j + 1], P.ca[j + 1]);
-                const real dn = P.prismatic[j + 1] ? (mq[j + 1] + P.offset[j + 1]) : P.D[j + 1];
-                const V3<real> pstar_n = {P.A[j + 1], -dn * P.sa[j + 1], dn * P.ca[j + 1]};
+                const LinkRot<real, MDH, V> Rn(sth[j + 1], cth[j + 1], P.sa[j + 1], P.ca[j + 1]);
+                const V dn = P.prismatic[j + 1] ? (mq[j + 1] + P.offset[j + 1]) : P.D[j + 1];
+                const V3<V> pstar_n = {P.A[j + 1], -dn * P.sa[j + 1], dn * P.ca[j + 1]};
                 t1 = Rn.mul(f);
                 fj = vadd(t1, F);
                 t1 = Rn.mul(nn);
@@ -401,13 +438,13 @@ __device__ __forceinline__ void rne_row_generic(const RneP<real, N> &P, const re
             t1 = vadd(t1, t2);
             nj = vadd(t1, Nm[j]);
         } else {
-            const real dj = pris ? (mq[j] + P.offset[j]) : P.D[j];
-            const V3<real> pstar = {P.A[j], dj * P.sa[j], dj * P.ca[j]};
+            const V dj = pris ? (mq[j] + P.offset[j]) : P.D[j];
+            const V3<V> pstar = {P.A[j], dj * P.sa[j], dj * P.ca[j]};
             t4 = Fm[j];
             t2 = vadd(pstar, rc);
             t1 = vcross(t2, t4);
             if (j != N - 1) {
-                const LinkRot<real, MDH> Rn(sth[j + 1], cth[j + 1], P.sa[j + 1], P.ca[j + 1]);
+                const LinkRot<real, MDH, V> Rn(sth[j + 1], cth[j + 1], P.sa[j + 1], P.ca[j + 1]);
                 fj = vadd(t4, Rn.mul(f));
                 t2 = Rn.tmul(pstar);
                 t3 = vcross(t2, f);
@@ -427,20 +464,20 @@ __device__ __forceinline__ void rne_row_generic(const RneP<real, N> &P, const re
         V3<real> zax;
         if (MDH) zax = {0, 0, 1};
         else zax = {0, P.sa[j], P.ca[j]}; // R_j^T z0 = (n.z, o.z, a.z)
-        real t = pris ? vdot(fj, zax) : vdot(nj, zax);
-        const real qdj = mqd[j];
+        V t = pris ? vdot(fj, zax) : vdot(nj, zax);
+        const V qdj = mqd[j];
         t += P.c_jm[j] * mqdd[j];
         t += P.c_b[j] * qdj;
         t += (qdj > 0 ? P.c_tcp[j] : (real)0) + (qdj < 0 ? P.c_tcm[j] : (real)0);
         tq[j] = t;
     }
     if constexpr (WRENCH) { // the MDH prismatic-first-joint quirk above carries over: wb is what that recursion gives
-        const LinkRot<real, MDH> R(sth[0], cth[0], P.sa[0], P.ca[0]);
-        const V3<real> f0 = R.mul(f);
-        V3<real> n0 = R.mul(nn);
+        const LinkRot<real, MDH, V> R(sth[0], cth[0], P.sa[0], P.ca[0]);
+        const V3<V> f0 = R.mul(f);
+        V3<V> n0 = R.mul(nn);
         if (MDH) {
-            const real d = P.prismatic[0] ? (mq[0] + P.offset[0]) : P.D[0];
-            n0 = vadd(n0, vcross(V3<real>{P.A[0], -d * P.sa[0], d * P.ca[0]}, f0));
+            const V d = P.prismatic[0] ? (mq[0] + P.offset[0]) : P.D[0];
+            n0 = vadd(n0, vcross(V3<V>{P.A[0], -d * P.sa[0], d * P.ca[0]}, f0));
         }
         rne_put_wrench(f0, n0, wb);
     }
@@ -537,6 +574,48 @@ struct FanShape {
     static constexpr int NIN = (MODE == FAN_INERTIA || MODE == FAN_GRAVLOAD) ? 1 : (MODE == FAN_ACCEL ? 3 : 2);
     static constexpr int OUT = (MODE == FAN_INERTIA || MODE == FAN_CORIOLIS) ? N * N : N;
 };
+
+// Solves A X = B by Gaussian elimination with partial pivoting (numpy.linalg.solve = LAPACK gesv), A = M (N x N,
+// row-major, destroyed), B = rhs (N x NRHS, row-major, destroyed), X into x (N x NRHS)
+template <typename real, int N, int NRHS>
+__device__ __forceinline__ void rne_lu_solve(real *M, real *rhs, real *x)
+{
+#pragma unroll 1
+    for (int c = 0; c < N; c++) {
+        int p = c;
+        real best = fabs(M[c * N + c]);
+#pragma unroll 1
+        for (int r = c + 1; r < N; r++) {
+            const real v = fabs(M[r * N + c]);
+            if (v > best) { best = v; p = r; }
+        }
+        if (p != c) {
+#pragma unroll 1
+            for (int k = 0; k < N; k++) { const real t = M[c * N + k]; M[c * N + k] = M[p * N + k]; M[p * N + k] = t; }
+#pragma unroll
+            for (int s = 0; s < NRHS; s++) { const real t = rhs[c * NRHS + s]; rhs[c * NRHS + s] = rhs[p * NRHS + s]; rhs[p * NRHS + s] = t; }
+        }
+        const real inv = (real)1 / M[c * N + c];
+#pragma unroll 1
+        for (int r = c + 1; r < N; r++) {
+            const real f = M[r * N + c] * inv;
+#pragma unroll 1
+            for (int k = c; k < N; k++) M[r * N + k] -= f * M[c * N + k];
+#pragma unroll
+            for (int s = 0; s < NRHS; s++) rhs[r * NRHS + s] -= f * rhs[c * NRHS + s];
+        }
+    }
+#pragma unroll 1
+    for (int r = N - 1; r >= 0; r--) {
+#pragma unroll
+        for (int s = 0; s < NRHS; s++) {
+            real acc = rhs[r * NRHS + s];
+#pragma unroll 1
+            for (int k = r + 1; k < N; k++) acc -= M[r * N + k] * x[k * NRHS + s];
+            x[r * NRHS + s] = acc / M[r * N + r];
+        }
+    }
+}
 
 template <typename real, int N, bool MDH, bool ALLREV, int MODE>
 __global__ void __launch_bounds__(B2K_THREADS, (sizeof(real) == 4) ? 3 : 2)
@@ -657,37 +736,7 @@ k_rne_fan(const __grid_constant__ RneP<real, N> P, const real *__restrict__ in0,
 #pragma unroll
             for (int k = 0; k < N; k++) M[i * N + k] = tq[k];
         }
-        // Gaussian elimination with partial pivoting (numpy.linalg.solve = LAPACK gesv)
-#pragma unroll 1
-        for (int c = 0; c < N; c++) {
-            int p = c;
-            real best = fabs(M[c * N + c]);
-#pragma unroll 1
-            for (int r = c + 1; r < N; r++) {
-                const real v = fabs(M[r * N + c]);
-                if (v > best) { best = v; p = r; }
-            }
-            if (p != c) {
-#pragma unroll 1
-                for (int k = 0; k < N; k++) { const real t = M[c * N + k]; M[c * N + k] = M[p * N + k]; M[p * N + k] = t; }
-                const real t = rhs[c]; rhs[c] = rhs[p]; rhs[p] = t;
-            }
-            const real inv = (real)1 / M[c * N + c];
-#pragma unroll 1
-            for (int r = c + 1; r < N; r++) {
-                const real f = M[r * N + c] * inv;
-#pragma unroll 1
-                for (int k = c; k < N; k++) M[r * N + k] -= f * M[c * N + k];
-                rhs[r] -= f * rhs[c];
-            }
-        }
-#pragma unroll 1
-        for (int r = N - 1; r >= 0; r--) {
-            real acc = rhs[r];
-#pragma unroll 1
-            for (int k = r + 1; k < N; k++) acc -= M[r * N + k] * res[k];
-            res[r] = acc / M[r * N + r];
-        }
+        rne_lu_solve<real, N, 1>(M, rhs, res);
     }
     OS::put_row(sout, lane, res);
     if (!OS::drain_async(sout, out + row0 * SH::OUT, rows_here, lane)) {
@@ -844,6 +893,191 @@ int rne_fan_launch(const b2k_rne_s *r, int mode, const void *in0, const void *in
         B2K_CASE(6) B2K_CASE(7) B2K_CASE(8) B2K_CASE(9) B2K_CASE(10)
     default:
         b2k_set_error("rne fan-out: unsupported joint count %d", r->n);
+        return B2K_ERR_INVALID;
+    }
+#undef B2K_CASE
+}
+
+// ------------------------------------------------------------------ analytical derivatives of the recursion (DESIGN f-13)
+// DERIV_INVERSE: in = (q, qd, qdd); out0 = dtau/dq, out1 = dtau/dqd (N, n, n), [i, k] = dtau_i / dx_k, tau exactly what
+//                k_rne computes with the same gravity and tip wrench.
+// DERIV_FORWARD: in = (q, qd, torque); with M = inertia(q) (the FAN_INERTIA layout) and qdd* = M^-1 (torque - rne(q, qd, 0))
+//                as FAN_ACCEL computes them: out0 = -M^-1 dtau/dq, out1 = -M^-1 dtau/dqd (both at qdd*), out2 = M^-1.
+// Column k of each Jacobian is one evaluation of the recursion on Dual<real>, seeded with the tangent of q_k (of
+// sin / cos theta_k for a revolute joint, of d_k = q_k + offset_k for a prismatic one) or of qd_k.  Like the fan-outs,
+// the loops over columns are runtime loops (code size of one dual recursion) and the n x n results live in local memory.
+enum { DERIV_INVERSE = 0, DERIV_FORWARD = 1 };
+
+template <typename real, int N, bool MDH, bool ALLREV, int MODE>
+__global__ void __launch_bounds__(B2K_THREADS, (sizeof(real) == 4) ? 3 : 2)
+k_rne_deriv(const __grid_constant__ RneP<real, N> P, const real *__restrict__ in0, const real *__restrict__ in1,
+            const real *__restrict__ in2, long long nrows, real *__restrict__ out0, real *__restrict__ out1,
+            real *__restrict__ out2, int warp_smem_bytes, int in_bytes, int qmode)
+{
+    typedef TileStage<real, N * N> OS;
+    typedef Dual<real> D;
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    const int lane = threadIdx.x & 31;
+    const int warp = threadIdx.x >> 5;
+    unsigned char *wbase = smem_raw + (size_t)warp * warp_smem_bytes;
+    real *s0 = reinterpret_cast<real *>(wbase);
+    real *s1 = reinterpret_cast<real *>(wbase + in_bytes);
+    real *s2 = reinterpret_cast<real *>(wbase + 2 * in_bytes);
+    unsigned char *sout = wbase + 3 * in_bytes;
+    const int lds = qmode ? N : (N | 1);
+    const long long ntiles = (nrows + 31) >> 5;
+    const float inv_n = 1.0f / (float)N;
+    const long long tile = (long long)blockIdx.x * B2K_WARPS_PER_BLOCK + warp; // one tile per warp, one-shot grid
+    if (tile >= ntiles) return;
+    const long long row0 = tile << 5;
+    const int rows_here = (int)((nrows - row0) < 32 ? (nrows - row0) : 32);
+    load_q_tile<real>(s0, in0 + row0 * N, rows_here, N, inv_n, qmode, lane);
+    load_q_tile<real>(s1, in1 + row0 * N, rows_here, N, inv_n, qmode, lane);
+    load_q_tile<real>(s2, in2 + row0 * N, rows_here, N, inv_n, qmode, lane);
+    cp_async_wait_all();
+    __syncwarp();
+    const int myrow = (lane < rows_here ? lane : 0) * lds;
+    const real *mq = s0 + myrow;
+
+    real sth[N], cth[N], qd[N], qdd[N];
+    rne_sincos<real, N, ALLREV>(P, mq, sth, cth);
+#pragma unroll
+    for (int k = 0; k < N; k++) qd[k] = s1[myrow + k];
+    const V3<real> gvec = {P.grav[0], P.grav[1], P.grav[2]};
+    // one n x n output: staged, copied out, and the stage free again before the next one is put
+    auto emit = [&](const real *res, real *out) {
+        OS::put_row(sout, lane, res);
+        if (!OS::drain_async(sout, out + row0 * (N * N), rows_here, lane)) {
+            __syncwarp();
+            OS::drain(sout, out + row0 * (N * N), rows_here, lane);
+        }
+        OS::wait_all();
+        __syncwarp();
+    };
+
+    real Minv[MODE == DERIV_FORWARD ? N * N : 1];
+    if constexpr (MODE == DERIV_FORWARD) { // qdd* and M^-1 from one pivoted solve of M [X0 | X] = [torque - rne(q, qd, 0) | I]
+        real M[N * N], B[N * (N + 1)], X[N * (N + 1)], zero[N];
+#pragma unroll
+        for (int k = 0; k < N; k++) zero[k] = 0;
+        {
+            real tq[N];
+            if constexpr (ALLREV) rne_row_allrev<real, N, MDH>(P, sth, cth, qd, zero, gvec, tq);
+            else rne_row_generic<real, N, MDH>(P, mq, sth, cth, qd, zero, gvec, tq);
+#pragma unroll
+            for (int k = 0; k < N; k++) {
+                B[k * (N + 1)] = s2[myrow + k] - tq[k];
+#pragma unroll
+                for (int i = 0; i < N; i++) B[k * (N + 1) + 1 + i] = (k == i) ? (real)1 : (real)0;
+            }
+        }
+#pragma unroll 1
+        for (int i = 0; i < N; i++) { // inertia rows: unit accelerations, no velocity, no gravity (as FAN_ACCEL)
+            real a[N], tq[N];
+#pragma unroll
+            for (int k = 0; k < N; k++) a[k] = (k == i) ? (real)1 : (real)0;
+            if constexpr (ALLREV) rne_row_allrev<real, N, MDH>(P, sth, cth, zero, a, V3<real>{0, 0, 0}, tq);
+            else rne_row_generic<real, N, MDH>(P, mq, sth, cth, zero, a, V3<real>{0, 0, 0}, tq);
+#pragma unroll
+            for (int k = 0; k < N; k++) M[i * N + k] = tq[k];
+        }
+        rne_lu_solve<real, N, N + 1>(M, B, X);
+#pragma unroll
+        for (int k = 0; k < N; k++) {
+            qdd[k] = X[k * (N + 1)];
+#pragma unroll
+            for (int i = 0; i < N; i++) Minv[k * N + i] = X[k * (N + 1) + 1 + i];
+        }
+        emit(Minv, out2);
+    } else {
+#pragma unroll
+        for (int k = 0; k < N; k++) qdd[k] = s2[myrow + k];
+    }
+
+    const V3<D> gdual = {gvec.x, gvec.y, gvec.z};
+#pragma unroll 1
+    for (int pass = 0; pass < 2; pass++) { // 0: columns of q, 1: columns of qd
+        real res[N * N];
+#pragma unroll 1
+        for (int k = 0; k < N; k++) {
+            D S[N], Cs[N], Q[N], QD[N], QDD[N], tq[N];
+#pragma unroll
+            for (int j = 0; j < N; j++) {
+                const bool sq = pass == 0 && j == k;
+                const bool rev = ALLREV || !P.prismatic[j];
+                S[j] = D(sth[j], (sq && rev) ? cth[j] : (real)0);
+                Cs[j] = D(cth[j], (sq && rev) ? -sth[j] : (real)0);
+                Q[j] = D(mq[j], (sq && !rev) ? (real)1 : (real)0);
+                QD[j] = D(qd[j], (pass == 1 && j == k) ? (real)1 : (real)0);
+                QDD[j] = D(qdd[j]);
+            }
+            if constexpr (ALLREV) rne_row_allrev<real, N, MDH, false, D>(P, S, Cs, QD, QDD, gdual, tq);
+            else rne_row_generic<real, N, MDH, false, D>(P, Q, S, Cs, QD, QDD, gdual, tq);
+            if constexpr (MODE == DERIV_FORWARD) {
+#pragma unroll
+                for (int i = 0; i < N; i++) {
+                    real acc = 0;
+#pragma unroll
+                    for (int j = 0; j < N; j++) acc = fma(Minv[i * N + j], tq[j].d, acc);
+                    res[i * N + k] = -acc;
+                }
+            } else {
+#pragma unroll
+                for (int i = 0; i < N; i++) res[i * N + k] = tq[i].d;
+            }
+        }
+        emit(res, pass == 0 ? out0 : out1);
+    }
+}
+
+template <typename real, int N, int MODE>
+int rne_deriv_launch_mode(const b2k_rne_s *r, const real *in0, const real *in1, const real *in2, long long nrows,
+                          const double *grav, const double *fext, real *out0, real *out1, real *out2, cudaStream_t st)
+{
+    typedef TileStage<real, N * N> OS;
+    RneP<real, N> P;
+    rne_fill_params<real, N>(r, grav, MODE == DERIV_INVERSE ? fext : nullptr, P);
+    const size_t inb = fkj_q_bytes<real>(N);
+    const size_t wsm = (3 * inb + (size_t)OS::BYTES + 15) & ~(size_t)15;
+    const size_t smem = wsm * B2K_WARPS_PER_BLOCK;
+    const int qmode = (fkj_qmode<real>(in0, N) && fkj_qmode<real>(in1, N) && fkj_qmode<real>(in2, N)) ? 1 : 0;
+    for (real *o : {out0, out1, out2})
+        if (o && ((uintptr_t)o) % OS::UB) { b2k_set_error("rne derivatives: outputs must be %d-byte aligned", OS::UB); return B2K_ERR_INVALID; }
+    const long long ntiles = (nrows + 31) / 32;
+    const long long grid = (ntiles + B2K_WARPS_PER_BLOCK - 1) / B2K_WARPS_PER_BLOCK;
+    bool allrev = true;
+    for (int j = 0; j < N; j++) allrev = allrev && !P.prismatic[j];
+    auto launch = [&](auto kern) -> int {
+        int per_sm = b2k_blocks_per_sm((const void *)kern, B2K_THREADS, smem);
+        if (per_sm < 1) return per_sm < 0 ? per_sm : (b2k_set_error("rne derivative kernel does not fit on an SM"), B2K_ERR_INVALID);
+        kern<<<(unsigned)grid, B2K_THREADS, smem, st>>>(P, in0, in1, in2, nrows, out0, out1, out2, (int)wsm, (int)inb, qmode);
+        b2k_count_launch();
+        B2K_CUDA(cudaGetLastError());
+        return B2K_OK;
+    };
+    if (r->mdh) return allrev ? launch(k_rne_deriv<real, N, true, true, MODE>) : launch(k_rne_deriv<real, N, true, false, MODE>);
+    return allrev ? launch(k_rne_deriv<real, N, false, true, MODE>) : launch(k_rne_deriv<real, N, false, false, MODE>);
+}
+
+// mode DERIV_INVERSE or DERIV_FORWARD (fext and out2 unused by the inverse / forward mode respectively)
+template <typename real>
+int rne_deriv_launch(const b2k_rne_s *r, int mode, const void *in0, const void *in1, const void *in2, long long nrows,
+                     const double *grav, const double *fext, void *out0, void *out1, void *out2, cudaStream_t st)
+{
+#define B2K_CASE(NN)                                                                                                        \
+    case NN:                                                                                                                \
+        return mode == DERIV_FORWARD                                                                                        \
+                   ? rne_deriv_launch_mode<real, NN, DERIV_FORWARD>(r, (const real *)in0, (const real *)in1,               \
+                                                                    (const real *)in2, nrows, grav, fext, (real *)out0,     \
+                                                                    (real *)out1, (real *)out2, st)                        \
+                   : rne_deriv_launch_mode<real, NN, DERIV_INVERSE>(r, (const real *)in0, (const real *)in1,               \
+                                                                    (const real *)in2, nrows, grav, fext, (real *)out0,     \
+                                                                    (real *)out1, nullptr, st);
+    switch (r->n) {
+        B2K_CASE(1) B2K_CASE(2) B2K_CASE(3) B2K_CASE(4) B2K_CASE(5)
+        B2K_CASE(6) B2K_CASE(7) B2K_CASE(8) B2K_CASE(9) B2K_CASE(10)
+    default:
+        b2k_set_error("rne derivatives: unsupported joint count %d", r->n);
         return B2K_ERR_INVALID;
     }
 #undef B2K_CASE

@@ -628,3 +628,65 @@ if want("planar_"):
                                                           frac_of_3350=round((4 * n + 9) * es * N / (ms * 1e-3) / 3.35e12, 4)))
                 del T3, J3
             del qs, T, J
+
+# Analytical derivatives of the DH recursion (k_rne_deriv, csrc/b2k_rne.cuh) through the C ABI, Puma560, 1M rows.
+# Algorithmic bytes per row, sizeof(real) = es: rne_derivatives (3n + 2n^2) es, accel_derivatives (3n + 3n^2) es.  The
+# kernel does 2n dual-number recursions per row (plus n + 1 plain ones and an n x n solve for accel_derivatives), so it is
+# expected to be compute-bound; frac_of_hbm is stated for context only.  fd_route is what a user has without it: the
+# 2n + 1 b2k_rne launches of a one-sided finite difference (q and qd perturbed one joint at a time), timed in the same
+# call on the same rows.  The card's name and power limit are read in the same run.
+DERIV_CASES = [f"dyn_{op}_derivs_puma_{t}" for op in ("rne", "accel") for t in ("f64", "f32")]
+if any(want(c) for c in DERIV_CASES):
+    import subprocess
+
+    try:
+        plim = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True,
+                              text=True, timeout=30).stdout.strip()
+    except Exception as e:  # the figure is context, the timing does not depend on it
+        plim = f"unavailable ({type(e).__name__})"
+    card = {"gpu": torch.cuda.get_device_name(0), "power_limit": plim}
+    Ld = rtb._lib.lib()
+    std = torch.cuda.current_stream().cuda_stream
+    pz = rtb.models.Puma560()
+    pz.rne(np.zeros(6), np.zeros(6), np.zeros(6))  # creates the handle
+    hd, n = pz._rne_ob, 6
+    gd = np.ascontiguousarray(-pz.gravity)
+    rngd = np.random.default_rng(13)
+    for dt in (np.float64, np.float32):
+        tag = "f64" if dt == np.float64 else "f32"
+        es = np.dtype(dt).itemsize
+        code = rtb._lib.F64 if dt == np.float64 else rtb._lib.F32
+        tt = torch.float64 if dt == np.float64 else torch.float32
+        q0, qd0, x0 = (torch.from_numpy(rngd.uniform(-2, 2, (N, n)).astype(dt)).to(dev) for _ in range(3))
+        o = [torch.empty((N, n, n), dtype=tt, device=dev) for _ in range(3)]
+        c_rne, c_acc = f"dyn_rne_derivs_puma_{tag}", f"dyn_accel_derivs_puma_{tag}"
+        fd = {}
+        if want(c_rne) or want(c_acc):
+            hstep = 1e-6 if dt == np.float64 else 1e-2
+            pert = []
+            for k in range(n):
+                e = torch.zeros(n, dtype=tt, device=dev)
+                e[k] = hstep
+                pert.append((q0 + e, qd0))
+                pert.append((q0, qd0 + e))
+            pert.append((q0, qd0))
+            tau = [torch.empty((N, n), dtype=tt, device=dev) for _ in pert]
+
+            def fd_route(i):
+                for (a, b), t in zip(pert, tau):
+                    rtb._lib.check(Ld.b2k_rne(hd, code, a.data_ptr(), b.data_ptr(), x0.data_ptr(), N, rtb._lib.dptr(gd), None, t.data_ptr(), std))
+
+            ms_fd = timeit(fd_route, 1)
+            fd = {"fd_route_ms": round(ms_fd, 4), "fd_route_launches": 2 * n + 1}
+            del pert, tau
+        if want(c_rne):
+            ms = timeit(lambda i: rtb._lib.check(Ld.b2k_rne_derivatives(hd, code, q0.data_ptr(), qd0.data_ptr(), x0.data_ptr(), N, rtb._lib.dptr(gd),
+                                                                       None, o[0].data_ptr(), o[1].data_ptr(), std)), 1)
+            report(c_rne, ms, N, (3 * n + 2 * n * n) * es, dict(card, **fd, bound="compute (expected, not measured)",
+                                                                 speedup_vs_fd_route=round(fd["fd_route_ms"] / ms, 2)))
+        if want(c_acc):
+            ms = timeit(lambda i: rtb._lib.check(Ld.b2k_rne_accel_derivatives(hd, code, q0.data_ptr(), qd0.data_ptr(), x0.data_ptr(), N,
+                                                                             rtb._lib.dptr(gd), o[0].data_ptr(), o[1].data_ptr(), o[2].data_ptr(), std)), 1)
+            report(c_acc, ms, N, (3 * n + 3 * n * n) * es, dict(card, **fd, bound="compute (expected, not measured)",
+                                                                 speedup_vs_fd_route=round(fd["fd_route_ms"] / ms, 2)))
+        del q0, qd0, x0, o
