@@ -361,6 +361,19 @@ class DHRobot:
     def __del__(self):
         self.delete_rne()
 
+    def _rne_handle(self):
+        """The RNE handle of the current link parameters, rebuilt if they changed (reference @_check_rne, DHLink.py:24-51)."""
+        if self._rne_ob is None or self._dynchanged:
+            self.delete_rne()
+            self._init_rne()
+        return self._rne_ob
+
+    def _kernel_gravity(self, gravity):
+        """The gravity vector the kernels take: the recursion has no base, so gravity is rotated into the base frame
+        instead (reference 1431-1433) and handed over negated (1449)."""
+        g = self._gravity if gravity is None else np.asarray(gravity, dtype=np.float64).reshape(3)
+        return np.ascontiguousarray(-(self._base[:3, :3].T @ g))
+
     def rne(self, q, qd=None, qdd=None, gravity=None, fext=None, base_wrench=False, dtype=None):
         """Inverse dynamics tau = RNE(q, qd, qdd): (n,) for one state, (N,n) for a trajectory
         (reference DHRobot.rne 1373-1456 -> frne.frne per row).
@@ -368,9 +381,7 @@ class DHRobot:
         ``base_wrench=True`` returns ``(tau, wbase)``: tau as above and wbase (6,) / (N,6) = [fx, fy, fz, mx, my, mz],
         the wrench the base exerts on link 1, expressed in frame 0 (the chain's base frame, after ``robot.base``) with
         the moment about its origin.  Both come from the same recursion (one kernel launch)."""
-        if self._rne_ob is None or self._dynchanged:  # @_check_rne, DHLink.py:24-51
-            self.delete_rne()
-            self._init_rne()
+        h = self._rne_handle()
         n = self.n
         for x, nm in ((q, "q"), (qd, "qd"), (qdd, "qdd")):
             if x is None:
@@ -391,10 +402,7 @@ class DHRobot:
         for x, nm in ((q2, "q"), (qd2, "qd"), (qdd2, "qdd")):
             if x.ndim != 2 or tuple(x.shape) != (N, n):
                 raise ValueError(f"{nm} must have shape ({n},) or (N,{n}); got {tuple(x.shape)}")
-        g = self._gravity if gravity is None else np.asarray(gravity, dtype=np.float64).reshape(3)
-        # the recursion has no base: rotate gravity instead (reference 1431-1433), and hand it over negated (1449)
-        g = self._base[:3, :3].T @ g
-        ng = np.ascontiguousarray(-g)
+        ng = self._kernel_gravity(gravity)
         fx = None if fext is None else np.ascontiguousarray(np.asarray(fext, dtype=np.float64).reshape(6))
         L = _lib.lib()
         if host:
@@ -403,21 +411,21 @@ class DHRobot:
             tau = _lib.host_result((N, n), dt)
             if base_wrench:
                 wb = _lib.host_result((N, 6), dt)
-                _lib.check(L.b2k_rne_wrench_host(self._rne_ob, B.code(dt), qh.ctypes.data, qdh.ctypes.data, qddh.ctypes.data, N,
+                _lib.check(L.b2k_rne_wrench_host(h, B.code(dt), qh.ctypes.data, qdh.ctypes.data, qddh.ctypes.data, N,
                                                  _lib.dptr(ng), _lib.dptr(fx), tau.ctypes.data, wb.ctypes.data,
                                                  t.cuda.current_device()))
             else:
-                _lib.check(L.b2k_rne_host(self._rne_ob, B.code(dt), qh.ctypes.data, qdh.ctypes.data, qddh.ctypes.data, N,
+                _lib.check(L.b2k_rne_host(h, B.code(dt), qh.ctypes.data, qdh.ctypes.data, qddh.ctypes.data, N,
                                           _lib.dptr(ng), _lib.dptr(fx), tau.ctypes.data, t.cuda.current_device()))
         else:
             qt, qdt, qddt = (B.to_device(x, dt) for x in (q2, qd2, qdd2))
             tau = B.empty((N, n), dt, like=qt)
             if base_wrench:
                 wb = B.empty((N, 6), dt, like=qt)
-                _lib.check(L.b2k_rne_wrench(self._rne_ob, B.code(dt), B.ptr(qt), B.ptr(qdt), B.ptr(qddt), N, _lib.dptr(ng),
+                _lib.check(L.b2k_rne_wrench(h, B.code(dt), B.ptr(qt), B.ptr(qdt), B.ptr(qddt), N, _lib.dptr(ng),
                                             _lib.dptr(fx), B.ptr(tau), B.ptr(wb), B.stream_ptr(qt)))
             else:
-                _lib.check(L.b2k_rne(self._rne_ob, B.code(dt), B.ptr(qt), B.ptr(qdt), B.ptr(qddt), N, _lib.dptr(ng),
+                _lib.check(L.b2k_rne(h, B.code(dt), B.ptr(qt), B.ptr(qdt), B.ptr(qddt), N, _lib.dptr(ng),
                                      _lib.dptr(fx), B.ptr(tau), B.stream_ptr(qt)))
         if base_wrench:
             return (tau[0], wb[0]) if single else (tau, wb)
@@ -462,15 +470,8 @@ class DHRobot:
         right-hand side (any scipy solver; one trajectory)."""
         from ._fdyn import fdyn as _fdyn
 
-        if not callable(Q) and (self._rne_ob is None or self._dynchanged):
-            self.delete_rne()
-            self._init_rne()
-
-        def kernel_gravity(gravity):
-            g = self._gravity if gravity is None else np.asarray(gravity, dtype=np.float64).reshape(3)
-            return -(self._base[:3, :3].T @ g)
-
-        return _fdyn(self, _lib.lib().b2k_rne_fdyn if not callable(Q) else None, self._rne_ob, kernel_gravity, T, q0, Q=Q, Q_args=Q_args,
+        h = self._rne_ob if callable(Q) else self._rne_handle()
+        return _fdyn(self, _lib.lib().b2k_rne_fdyn if not callable(Q) else None, h, self._kernel_gravity, T, q0, Q=Q, Q_args=Q_args,
                      qd0=qd0, solver=solver, solver_args=solver_args, dt=dt, gravity=gravity, max_steps=max_steps, dtype=dtype)
 
     _RNE_MODES = {"rne": 0, "inertia": 1, "gravload": 2, "itorque": 3, "coriolis": 4, "accel": 5, "rne_wrench": 6}
@@ -486,13 +487,10 @@ class DHRobot:
             return (f"generic k_rne_deriv<{'double' if np.dtype(dtype) == np.float64 else 'float'}, n={self.n}, {'MDH' if self.mdh else 'DH'}, "
                     f"{'all-revolute' if allrev else 'prismatic'}, {self._DERIV_OPS[op]}> (the robot-specialised path "
                     "generates no derivative kernels)")
-        if self._rne_ob is None or self._dynchanged:
-            self.delete_rne()
-            self._init_rne()
-        g = self._gravity if gravity is None else np.asarray(gravity, dtype=np.float64).reshape(3)
-        g = np.ascontiguousarray(-(self._base[:3, :3].T @ g))
+        h = self._rne_handle()
+        g = self._kernel_gravity(gravity)
         buf = C.create_string_buffer(2048)
-        _lib.check(_lib.lib().b2k_rne_spec_info(self._rne_ob, self._RNE_MODES[op], B.code(np.dtype(dtype)), _lib.dptr(g),
+        _lib.check(_lib.lib().b2k_rne_spec_info(h, self._RNE_MODES[op], B.code(np.dtype(dtype)), _lib.dptr(g),
                                                 int(fext is not None and np.any(np.asarray(fext) != 0)), buf, 2048))
         return buf.value.decode()
 
@@ -500,9 +498,7 @@ class DHRobot:
     def _dyn(self, fn_name, ins, out_tail, gravity=None, use_gravity=False, dtype=None, fext=None, use_fext=False, n_out=1):
         """Shared front end of the fan-out kernels: every input (N,n) or (n,), one launch.  With n_out > 1 the kernel
         writes that many outputs of the same shape, returned as a tuple."""
-        if self._rne_ob is None or self._dynchanged:
-            self.delete_rne()
-            self._init_rne()
+        h = self._rne_handle()
         n = self.n
         for x in ins:
             B.check_numeric(x)
@@ -519,10 +515,9 @@ class DHRobot:
             if t.dim() != 2 or tuple(t.shape) != (N, n):
                 raise ValueError(f"inputs must have shape ({n},) or (N,{n}); got {tuple(t.shape)}")
         outs = [B.empty((N,) + out_tail, dt, like=dev[0]) for _ in range(n_out)]
-        args = [self._rne_ob, B.code(dt)] + [B.ptr(t) for t in dev] + [N]
+        args = [h, B.code(dt)] + [B.ptr(t) for t in dev] + [N]
         if use_gravity:
-            g = self._gravity if gravity is None else np.asarray(gravity, dtype=np.float64).reshape(3)
-            g = np.ascontiguousarray(-(self._base[:3, :3].T @ g))  # as DHRobot.rne: reference 1431-1433, 1449
+            g = self._kernel_gravity(gravity)
             args.append(_lib.dptr(g))
         if use_fext:
             fx = None if fext is None else np.ascontiguousarray(np.asarray(fext, dtype=np.float64).reshape(6))

@@ -13,15 +13,11 @@
 
 #include "b2k_common.cuh"
 
-// per-dtype launchers (b2k_fkj_f32.cu / b2k_fkj_f64.cu / b2k_rne.cu / b2k_ik_*.cu)
+// per-dtype launchers (b2k_fkj_f32.cu / b2k_fkj_f64.cu / b2k_ik_*.cu)
 int b2k_fkj_launch_f32(const b2k_chain_s *, int, const void *, long long, long long, const double *, const double *,
                        void *, void *, cudaStream_t);
 int b2k_fkj_launch_f64(const b2k_chain_s *, int, const void *, long long, long long, const double *, const double *,
                        void *, void *, cudaStream_t);
-int b2k_rne_launch(const b2k_rne_s *, int dtype, const void *, const void *, const void *, long long, const double *,
-                   const double *, void *, cudaStream_t);
-int b2k_rne_wrench_launch(const b2k_rne_s *, int dtype, const void *, const void *, const void *, long long, const double *,
-                          const double *, void *, void *, cudaStream_t);
 
 enum { FKJ_T = 1, FKJ_J0 = 2, FKJ_JE = 4 };
 
@@ -144,10 +140,9 @@ static int fkj_dispatch(const char *fn, b2k_chain_t c, int dtype, int mode, cons
 {
     int rc = check_common(fn, c, dtype, q, N, ldq);
     if (rc) return rc;
-    // T is stored in 32-byte pieces; J leaves through a shared-memory stage whose copy unit (TileStage<real, 6n>::UB in
-    // b2k_fkj.cuh) is 16 bytes when a 6n-element row is a whole number of 16-byte units, else 8
+    // T is stored in 32-byte pieces; J leaves through a shared-memory stage of 6n-element rows (TileStage in b2k_fkj.cuh)
     const unsigned es = dtype == B2K_F64 ? 8u : 4u;
-    const unsigned jub = (6u * (unsigned)c->n * es) % 16u == 0 ? 16u : 8u;
+    const unsigned jub = b2k_stage_unit(6 * c->n * (int)es);
     if ((mode & FKJ_T) && (rc = check_out(fn, "T", T, N, 32))) return rc;
     if ((mode & (FKJ_J0 | FKJ_JE)) && (rc = check_out(fn, "J", J, N, jub))) return rc;
     if ((rc = check_affine(fn, "base", base)) || (rc = check_affine(fn, "tool", tool))) return rc;
@@ -193,9 +188,6 @@ int b2k_planar_check(const char *fn, const b2k_chain_s *c, const double *base, c
 int b2k_planar_launch(const b2k_chain_s *c, int dtype, const double *base, const double *tool, int frame, const void *q,
                       long long nrows, long long ldq, void *T, void *J, cudaStream_t st);
 
-// the unit a per-warp output stage of rows of `row_bytes` is copied in (TileStage<real, n>::UB in b2k_fkj.cuh)
-static unsigned stage_unit(unsigned row_bytes) { return row_bytes % 16 == 0 ? 16u : (row_bytes % 8 == 0 ? 8u : 4u); }
-
 extern "C" int b2k_fkine_planar(b2k_chain_t c, int dtype, const void *q, int64_t N, int64_t ldq, const double *base,
                                 const double *tool, int frame, void *T, void *J, void *stream)
 {
@@ -209,54 +201,64 @@ extern "C" int b2k_fkine_planar(b2k_chain_t c, int dtype, const void *q, int64_t
     if (rc) return rc;
     if ((rc = check_common(fn, c, dtype, q, N, ldq))) return rc;
     const unsigned es = dtype == B2K_F64 ? 8u : 4u;
-    if ((T && (rc = check_out(fn, "T", T, N, stage_unit(9 * es)))) || (J && (rc = check_out(fn, "J", J, N, stage_unit(3 * c->n * es)))))
+    if ((T && (rc = check_out(fn, "T", T, N, b2k_stage_unit(9 * es)))) || (J && (rc = check_out(fn, "J", J, N, b2k_stage_unit(3 * c->n * es)))))
         return rc;
     if (N == 0) return B2K_OK;
     B2K_ON_DEVICE_OF(q);
     return b2k_planar_launch(c, dtype, base, tool, frame, q, N, ldq, T, J, (cudaStream_t)stream);
 }
 
-// b2k_rne and b2k_rne_wrench (wrench: also the base wrench, wbase (N, 6)); every argument is checked before any CUDA call
-static int rne_run(const char *fn, b2k_rne_t r, int dtype, const void *q, const void *qd, const void *qdd, int64_t N,
-                   const double *grav, const double *fext, void *tau, bool wrench, void *wbase, void *stream)
+// ------------------------------------------------------------------ operations on an rne handle
+// the generic kernels (b2k_rne.cuh), one translation unit per family of operations and dtype
+typedef int RneGenericFn(const b2k_rne_s *, int op, int dtype, const b2k_rne_args &, cudaStream_t);
+RneGenericFn b2k_rne_generic_rne, b2k_rne_generic_wrench, b2k_rne_generic_fan_f32, b2k_rne_generic_fan_f64,
+    b2k_rne_generic_deriv_f32, b2k_rne_generic_deriv_f64;
+
+// Every argument is checked against the operation's row of B2K_RNE_OPS before any CUDA call; then the robot-specialised
+// kernel (b2k_rne_spec.cu) serves the full 32-row tiles of the operations it has, and the generic kernel the rest.
+static int rne_dispatch(const char *fn, int op, b2k_rne_t r, int dtype, b2k_rne_args a, void *stream)
 {
+    const b2k_rne_op_s &d = B2K_RNE_OPS[op];
     if (!r) { b2k_set_error("%s: rne handle is NULL", fn); return B2K_ERR_INVALID; }
     if (dtype != B2K_F32 && dtype != B2K_F64) { b2k_set_error("%s: dtype must be B2K_F32 or B2K_F64", fn); return B2K_ERR_INVALID; }
-    if (N < 0) { b2k_set_error("%s: N is negative", fn); return B2K_ERR_INVALID; }
-    if (!grav) { b2k_set_error("%s: grav is NULL (pass -robot.gravity like DHRobot.rne)", fn); return B2K_ERR_INVALID; }
+    if (a.nrows < 0) { b2k_set_error("%s: N is negative", fn); return B2K_ERR_INVALID; }
+    if (r->n < 1 || r->n > B2K_MAX_JOINTS) { b2k_set_error("%s: unsupported joint count %d", fn, r->n); return B2K_ERR_INVALID; }
+    if (d.grav && !a.grav) { b2k_set_error("%s: grav is NULL (pass -robot.gravity like DHRobot.rne)", fn); return B2K_ERR_INVALID; }
     int rc;
-    const unsigned es = dtype == B2K_F64 ? 8u : 4u;
-    // tau leaves through a per-warp stage of n-element rows, copied in stage_unit(n * es) pieces (b2k_rne.cuh)
-    if ((rc = check_out(fn, "q", q, N, es)) || (rc = check_out(fn, "qd", qd, N, es)) || (rc = check_out(fn, "qdd", qdd, N, es)) ||
-        (rc = check_out(fn, "tau", tau, N, stage_unit((unsigned)r->n * es))))
-        return rc;
-    // a row of wbase is 3 pairs of reals: the kernels store it in 2-element units
-    if (wrench && (rc = check_out(fn, "wbase", wbase, N, 2 * es))) return rc;
-    if (N == 0) return B2K_OK;
-    B2K_ON_DEVICE_OF(q);
-    // the robot-specialised kernel (b2k_rne_spec.cu) serves the full 32-row tiles, the generic one the ragged tail
-    const long long done = b2k_rne_spec_launch(r, wrench ? 6 /* B2K_GEN_RNE_WRENCH */ : 0 /* B2K_GEN_RNE */, dtype, q, qd, qdd, N, grav,
-                                               fext, tau, wrench ? wbase : nullptr, (cudaStream_t)stream);
-    if (done < 0) return (int)done;
-    if (done == N) return B2K_OK;
-    const size_t off = (size_t)done * r->n * es;
-    if (wrench)
-        return b2k_rne_wrench_launch(r, dtype, (const char *)q + off, (const char *)qd + off, (const char *)qdd + off, N - done, grav,
-                                     fext, (char *)tau + off, (char *)wbase + (size_t)done * 6 * es, (cudaStream_t)stream);
-    return b2k_rne_launch(r, dtype, (const char *)q + off, (const char *)qd + off, (const char *)qdd + off, N - done, grav, fext,
-                          (char *)tau + off, (cudaStream_t)stream);
+    const int es = dtype == B2K_F64 ? 8 : 4;
+    for (int i = 0; i < d.nin; i++)
+        if ((rc = check_out(fn, d.in[i], a.in[i], a.nrows, es))) return rc;
+    // each output leaves through a per-warp stage of its rows, copied in b2k_stage_unit(row bytes) pieces (b2k_rne.cuh)
+    for (int o = 0; o < d.nout; o++)
+        if ((rc = check_out(fn, d.out[o], a.out[o], a.nrows, b2k_stage_unit(d.out_row(o, r->n) * es)))) return rc;
+    if (a.nrows == 0) return B2K_OK;
+    B2K_ON_DEVICE_OF(a.in[0]);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (op <= B2K_GEN_RNE_WRENCH) {
+        const long long done = b2k_rne_spec_launch(r, op, dtype, a.in[0], a.in[1], a.in[2], a.nrows, a.grav, a.fext, a.out[0], a.out[1], st);
+        if (done < 0) return (int)done;
+        if (done == a.nrows) return B2K_OK;
+        for (int i = 0; i < d.nin; i++) a.in[i] = (const char *)a.in[i] + (size_t)done * r->n * es;
+        for (int o = 0; o < d.nout; o++) a.out[o] = (char *)a.out[o] + (size_t)done * d.out_row(o, r->n) * es;
+        a.nrows -= done;
+    }
+    RneGenericFn *generic = op == B2K_GEN_RNE          ? b2k_rne_generic_rne
+                            : op == B2K_GEN_RNE_WRENCH ? b2k_rne_generic_wrench
+                            : op >= B2K_GEN_RNE_DERIV  ? (dtype == B2K_F64 ? b2k_rne_generic_deriv_f64 : b2k_rne_generic_deriv_f32)
+                                                       : (dtype == B2K_F64 ? b2k_rne_generic_fan_f64 : b2k_rne_generic_fan_f32);
+    return generic(r, op, dtype, a, st);
 }
 
 extern "C" int b2k_rne(b2k_rne_t r, int dtype, const void *q, const void *qd, const void *qdd, int64_t N,
                        const double *grav, const double *fext, void *tau, void *stream)
 {
-    return rne_run("b2k_rne", r, dtype, q, qd, qdd, N, grav, fext, tau, false, nullptr, stream);
+    return rne_dispatch("b2k_rne", B2K_GEN_RNE, r, dtype, {{q, qd, qdd}, {tau}, N, grav, fext}, stream);
 }
 
 extern "C" int b2k_rne_wrench(b2k_rne_t r, int dtype, const void *q, const void *qd, const void *qdd, int64_t N,
                               const double *grav, const double *fext, void *tau, void *wbase, void *stream)
 {
-    return rne_run("b2k_rne_wrench", r, dtype, q, qd, qdd, N, grav, fext, tau, true, wbase, stream);
+    return rne_dispatch("b2k_rne_wrench", B2K_GEN_RNE_WRENCH, r, dtype, {{q, qd, qdd}, {tau, wbase}, N, grav, fext}, stream);
 }
 
 // ------------------------------------------------------------------ host-buffer front ends
@@ -451,42 +453,37 @@ extern "C" int b2k_fkine_host(b2k_chain_t c, int dtype, const void *q, int64_t N
     });
 }
 
-extern "C" int b2k_rne_host(b2k_rne_t r, int dtype, const void *q, const void *qd, const void *qdd, int64_t N,
-                            const double *grav, const double *fext, void *tau, int device)
+// b2k_rne_host and b2k_rne_wrench_host (wrench: also the base wrench wbase (N, 6))
+static int rne_host(const char *fn, b2k_rne_t r, int dtype, const void *q, const void *qd, const void *qdd, int64_t N,
+                    const double *grav, const double *fext, void *tau, bool wrench, void *wbase, int device)
 {
-    const char *fn = "b2k_rne_host";
-    if (!r) { b2k_set_error("%s: rne handle is NULL", fn); return B2K_ERR_INVALID; }
-    if (dtype != B2K_F32 && dtype != B2K_F64) { b2k_set_error("%s: bad dtype", fn); return B2K_ERR_INVALID; }
-    if (N < 0 || (N > 0 && (!q || !qd || !qdd || !tau || !grav))) { b2k_set_error("%s: NULL argument", fn); return B2K_ERR_INVALID; }
-    if (N == 0) return B2K_OK;
-    const size_t es = dtype == B2K_F64 ? 8 : 4;
-    const void *h_in[3] = {q, qd, qdd};
-    size_t in_b[3] = {r->n * es, r->n * es, r->n * es};
-    void *h_out[1] = {tau};
-    size_t out_b[1] = {r->n * es};
-    return run_pipeline(device, N, 3, h_in, in_b, 1, h_out, out_b, [&](Slot &s, long long rows) {
-        return b2k_rne(r, dtype, s.d_in[0], s.d_in[1], s.d_in[2], rows, grav, fext, s.d_out[0], s.st);
-    });
-}
-
-extern "C" int b2k_rne_wrench_host(b2k_rne_t r, int dtype, const void *q, const void *qd, const void *qdd, int64_t N,
-                                   const double *grav, const double *fext, void *tau, void *wbase, int device)
-{
-    const char *fn = "b2k_rne_wrench_host";
     if (!r) { b2k_set_error("%s: rne handle is NULL", fn); return B2K_ERR_INVALID; }
     if (dtype != B2K_F32 && dtype != B2K_F64) { b2k_set_error("%s: bad dtype", fn); return B2K_ERR_INVALID; }
     if (N < 0 || (N > 0 && (!q || !qd || !qdd || !tau || !grav))) { b2k_set_error("%s: NULL argument", fn); return B2K_ERR_INVALID; }
     const size_t es = dtype == B2K_F64 ? 8 : 4;
     int rc;
-    if ((rc = check_out(fn, "wbase", wbase, N, (unsigned)es))) return rc;
+    if (wrench && (rc = check_out(fn, "wbase", wbase, N, (unsigned)es))) return rc;
     if (N == 0) return B2K_OK;
     const void *h_in[3] = {q, qd, qdd};
     size_t in_b[3] = {r->n * es, r->n * es, r->n * es};
     void *h_out[2] = {tau, wbase};
     size_t out_b[2] = {r->n * es, 6 * es};
-    return run_pipeline(device, N, 3, h_in, in_b, 2, h_out, out_b, [&](Slot &s, long long rows) {
-        return b2k_rne_wrench(r, dtype, s.d_in[0], s.d_in[1], s.d_in[2], rows, grav, fext, s.d_out[0], s.d_out[1], s.st);
+    return run_pipeline(device, N, 3, h_in, in_b, wrench ? 2 : 1, h_out, out_b, [&](Slot &s, long long rows) {
+        if (wrench) return b2k_rne_wrench(r, dtype, s.d_in[0], s.d_in[1], s.d_in[2], rows, grav, fext, s.d_out[0], s.d_out[1], s.st);
+        return b2k_rne(r, dtype, s.d_in[0], s.d_in[1], s.d_in[2], rows, grav, fext, s.d_out[0], s.st);
     });
+}
+
+extern "C" int b2k_rne_host(b2k_rne_t r, int dtype, const void *q, const void *qd, const void *qdd, int64_t N,
+                            const double *grav, const double *fext, void *tau, int device)
+{
+    return rne_host("b2k_rne_host", r, dtype, q, qd, qdd, N, grav, fext, tau, false, nullptr, device);
+}
+
+extern "C" int b2k_rne_wrench_host(b2k_rne_t r, int dtype, const void *q, const void *qd, const void *qdd, int64_t N,
+                                   const double *grav, const double *fext, void *tau, void *wbase, int device)
+{
+    return rne_host("b2k_rne_wrench_host", r, dtype, q, qd, qdd, N, grav, fext, tau, true, wbase, device);
 }
 
 // ------------------------------------------------------------------ inverse kinematics
@@ -642,103 +639,39 @@ extern "C" int b2k_ikine_qp(b2k_chain_t c, int dtype, const void *Tep, int64_t N
 }
 
 // ------------------------------------------------------------------ dynamics fan-outs
-int b2k_rne_fan_launch_f32(const b2k_rne_s *, int, const void *, const void *, const void *, long long, const double *, void *, cudaStream_t);
-int b2k_rne_fan_launch_f64(const b2k_rne_s *, int, const void *, const void *, const void *, long long, const double *, void *, cudaStream_t);
-enum { FAN_INERTIA = 0, FAN_GRAVLOAD = 1, FAN_ITORQUE = 2, FAN_CORIOLIS = 3, FAN_ACCEL = 4 };
-
-static int fan_dispatch(const char *fn, b2k_rne_t r, int dtype, int mode, const void *in0, const void *in1, const void *in2,
-                        int nin, int64_t N, const double *grav, bool need_grav, void *out, void *stream)
-{
-    if (!r) { b2k_set_error("%s: rne handle is NULL", fn); return B2K_ERR_INVALID; }
-    if (dtype != B2K_F32 && dtype != B2K_F64) { b2k_set_error("%s: dtype must be B2K_F32 or B2K_F64", fn); return B2K_ERR_INVALID; }
-    if (N < 0) { b2k_set_error("%s: N is negative", fn); return B2K_ERR_INVALID; }
-    if (need_grav && !grav) { b2k_set_error("%s: grav is NULL (pass -robot.gravity like DHRobot.rne)", fn); return B2K_ERR_INVALID; }
-    int rc;
-    const unsigned es = dtype == B2K_F64 ? 8u : 4u;
-    // the output leaves through a per-warp stage of rows of n (or n * n) elements, copied in stage_unit(row bytes) pieces
-    const unsigned out_row = (mode == FAN_INERTIA || mode == FAN_CORIOLIS) ? (unsigned)(r->n * r->n) : (unsigned)r->n;
-    if ((rc = check_out(fn, "q", in0, N, es)) || (nin >= 2 && (rc = check_out(fn, "second input", in1, N, es))) ||
-        (nin >= 3 && (rc = check_out(fn, "third input", in2, N, es))) || (rc = check_out(fn, "output", out, N, stage_unit(out_row * es))))
-        return rc;
-    if (N == 0) return B2K_OK;
-    B2K_ON_DEVICE_OF(in0);
-    cudaStream_t st = (cudaStream_t)stream;
-    const long long done = b2k_rne_spec_launch(r, mode + 1 /* FAN_* -> B2K_GEN_* */, dtype, in0, in1, in2, N, grav, nullptr, out, nullptr, st);
-    if (done < 0) return (int)done;
-    if (done == N) return B2K_OK;
-    const size_t off = (size_t)done * r->n * es;
-    in0 = (const char *)in0 + off;
-    if (in1) in1 = (const char *)in1 + off;
-    if (in2) in2 = (const char *)in2 + off;
-    out = (char *)out + (size_t)done * out_row * es;
-    N -= done;
-    if (dtype == B2K_F64) return b2k_rne_fan_launch_f64(r, mode, in0, in1, in2, N, grav, out, st);
-    return b2k_rne_fan_launch_f32(r, mode, in0, in1, in2, N, grav, out, st);
-}
-
 extern "C" int b2k_rne_inertia(b2k_rne_t r, int dtype, const void *q, int64_t N, void *M, void *stream)
 {
-    return fan_dispatch("b2k_rne_inertia", r, dtype, FAN_INERTIA, q, nullptr, nullptr, 1, N, nullptr, false, M, stream);
+    return rne_dispatch("b2k_rne_inertia", B2K_GEN_INERTIA, r, dtype, {{q}, {M}, N, nullptr, nullptr}, stream);
 }
 extern "C" int b2k_rne_gravload(b2k_rne_t r, int dtype, const void *q, int64_t N, const double *grav, void *taug, void *stream)
 {
-    return fan_dispatch("b2k_rne_gravload", r, dtype, FAN_GRAVLOAD, q, nullptr, nullptr, 1, N, grav, true, taug, stream);
+    return rne_dispatch("b2k_rne_gravload", B2K_GEN_GRAVLOAD, r, dtype, {{q}, {taug}, N, grav, nullptr}, stream);
 }
 extern "C" int b2k_rne_itorque(b2k_rne_t r, int dtype, const void *q, const void *qdd, int64_t N, void *taui, void *stream)
 {
-    return fan_dispatch("b2k_rne_itorque", r, dtype, FAN_ITORQUE, q, qdd, nullptr, 2, N, nullptr, false, taui, stream);
+    return rne_dispatch("b2k_rne_itorque", B2K_GEN_ITORQUE, r, dtype, {{q, qdd}, {taui}, N, nullptr, nullptr}, stream);
 }
 extern "C" int b2k_rne_coriolis(b2k_rne_t r, int dtype, const void *q, const void *qd, int64_t N, void *Cm, void *stream)
 {
-    return fan_dispatch("b2k_rne_coriolis", r, dtype, FAN_CORIOLIS, q, qd, nullptr, 2, N, nullptr, false, Cm, stream);
+    return rne_dispatch("b2k_rne_coriolis", B2K_GEN_CORIOLIS, r, dtype, {{q, qd}, {Cm}, N, nullptr, nullptr}, stream);
 }
 extern "C" int b2k_rne_accel(b2k_rne_t r, int dtype, const void *q, const void *qd, const void *torque, int64_t N,
                              const double *grav, void *qdd, void *stream)
 {
-    return fan_dispatch("b2k_rne_accel", r, dtype, FAN_ACCEL, q, qd, torque, 3, N, grav, true, qdd, stream);
+    return rne_dispatch("b2k_rne_accel", B2K_GEN_ACCEL, r, dtype, {{q, qd, torque}, {qdd}, N, grav, nullptr}, stream);
 }
 
 // ------------------------------------------------------------------ analytical derivatives of the recursion (b2k_rne.cuh)
-int b2k_rne_deriv_launch_f32(const b2k_rne_s *, int, const void *, const void *, const void *, long long, const double *,
-                             const double *, void *, void *, void *, cudaStream_t);
-int b2k_rne_deriv_launch_f64(const b2k_rne_s *, int, const void *, const void *, const void *, long long, const double *,
-                             const double *, void *, void *, void *, cudaStream_t);
-enum { DERIV_INVERSE = 0, DERIV_FORWARD = 1 };
-
-// the generic kernel serves every row: the robot-specialised path has no derivative kernels
-static int deriv_dispatch(const char *fn, b2k_rne_t r, int dtype, int mode, const void *in0, const void *in1, const void *in2,
-                          int64_t N, const double *grav, const double *fext, void *out0, void *out1, void *out2, void *stream)
-{
-    if (!r) { b2k_set_error("%s: rne handle is NULL", fn); return B2K_ERR_INVALID; }
-    if (dtype != B2K_F32 && dtype != B2K_F64) { b2k_set_error("%s: dtype must be B2K_F32 or B2K_F64", fn); return B2K_ERR_INVALID; }
-    if (N < 0) { b2k_set_error("%s: N is negative", fn); return B2K_ERR_INVALID; }
-    if (r->n < 1 || r->n > B2K_MAX_JOINTS) { b2k_set_error("%s: unsupported joint count %d", fn, r->n); return B2K_ERR_INVALID; }
-    if (!grav) { b2k_set_error("%s: grav is NULL (pass -robot.gravity like DHRobot.rne)", fn); return B2K_ERR_INVALID; }
-    int rc;
-    const unsigned es = dtype == B2K_F64 ? 8u : 4u;
-    // every output leaves through a per-warp stage of n*n-element rows, copied in stage_unit(n * n * es) pieces
-    const unsigned ou = stage_unit((unsigned)(r->n * r->n) * es);
-    const bool fwd = mode == DERIV_FORWARD;
-    if ((rc = check_out(fn, "q", in0, N, es)) || (rc = check_out(fn, "qd", in1, N, es)) ||
-        (rc = check_out(fn, fwd ? "torque" : "qdd", in2, N, es)) || (rc = check_out(fn, fwd ? "dqdd_dq" : "dtau_dq", out0, N, ou)) ||
-        (rc = check_out(fn, fwd ? "dqdd_dqd" : "dtau_dqd", out1, N, ou)) || (fwd && (rc = check_out(fn, "dqdd_dtau", out2, N, ou))))
-        return rc;
-    if (N == 0) return B2K_OK;
-    B2K_ON_DEVICE_OF(in0);
-    auto launch = dtype == B2K_F64 ? b2k_rne_deriv_launch_f64 : b2k_rne_deriv_launch_f32;
-    return launch(r, mode, in0, in1, in2, N, grav, fext, out0, out1, out2, (cudaStream_t)stream);
-}
-
 extern "C" int b2k_rne_derivatives(b2k_rne_t r, int dtype, const void *q, const void *qd, const void *qdd, int64_t N,
                                    const double *grav, const double *fext, void *dtau_dq, void *dtau_dqd, void *stream)
 {
-    return deriv_dispatch("b2k_rne_derivatives", r, dtype, DERIV_INVERSE, q, qd, qdd, N, grav, fext, dtau_dq, dtau_dqd, nullptr,
-                          stream);
+    return rne_dispatch("b2k_rne_derivatives", B2K_GEN_RNE_DERIV, r, dtype, {{q, qd, qdd}, {dtau_dq, dtau_dqd}, N, grav, fext},
+                        stream);
 }
 
 extern "C" int b2k_rne_accel_derivatives(b2k_rne_t r, int dtype, const void *q, const void *qd, const void *torque, int64_t N,
                                          const double *grav, void *dqdd_dq, void *dqdd_dqd, void *dqdd_dtau, void *stream)
 {
-    return deriv_dispatch("b2k_rne_accel_derivatives", r, dtype, DERIV_FORWARD, q, qd, torque, N, grav, nullptr, dqdd_dq,
-                          dqdd_dqd, dqdd_dtau, stream);
+    return rne_dispatch("b2k_rne_accel_derivatives", B2K_GEN_ACCEL_DERIV, r, dtype,
+                        {{q, qd, torque}, {dqdd_dq, dqdd_dqd, dqdd_dtau}, N, grav, nullptr}, stream);
 }

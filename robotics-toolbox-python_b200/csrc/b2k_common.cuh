@@ -109,14 +109,58 @@ struct IkQpArgs {
     const double *pi; // host, n; read only when kq > 0
 };
 
+// the unit a per-warp output stage of rows of `row_bytes` is copied in (TileStage<real, n>::UB in b2k_fkj.cuh): 16 bytes
+// when a row is a whole number of 16-byte units, else 8, else 4.  An output array must be aligned to it.
+constexpr int b2k_stage_unit(int row_bytes) { return row_bytes % 16 == 0 ? 16 : (row_bytes % 8 == 0 ? 8 : 4); }
+
 struct b2k_rne_s {
     int n, mdh;
     double L[B2K_MAX_JOINTS][24];
     void *spec; // cache of run-time compiled, robot-specialised kernels (b2k_rne_spec.cu)
 };
+
+// Operations on an rne handle.  B2K_GEN_RNE..B2K_GEN_RNE_WRENCH are served by the robot-specialised kernels
+// (b2k_rne_gen.cpp, b2k_rne_spec.cu) on the full 32-row tiles and by the generic ones (b2k_rne.cuh) on the rest; the
+// derivatives only by the generic ones.  RNE..ACCEL are also the public B2K_DYN_* codes of the tree entry points.
+enum { B2K_GEN_RNE = 0, B2K_GEN_INERTIA = 1, B2K_GEN_GRAVLOAD = 2, B2K_GEN_ITORQUE = 3, B2K_GEN_CORIOLIS = 4, B2K_GEN_ACCEL = 5,
+       B2K_GEN_RNE_WRENCH = 6, B2K_GEN_RNE_DERIV = 7, B2K_GEN_ACCEL_DERIV = 8, B2K_GEN_NOPS = 9 };
+static_assert(B2K_GEN_RNE == B2K_DYN_RNE && B2K_GEN_INERTIA == B2K_DYN_INERTIA && B2K_GEN_GRAVLOAD == B2K_DYN_GRAVLOAD &&
+                  B2K_GEN_ITORQUE == B2K_DYN_ITORQUE && B2K_GEN_CORIOLIS == B2K_DYN_CORIOLIS && B2K_GEN_ACCEL == B2K_DYN_ACCEL,
+              "B2K_DYN_* (b2kin.h) are the B2K_GEN_* codes of the tree operations");
+
+// What an operation reads and writes.  Every input is an (N, n) array; every output has rows of n or n * n reals, except
+// the base wrench, the (N, 6) second output of B2K_GEN_RNE_WRENCH.
+struct b2k_rne_op_s {
+    int nin, nout;          // input / output arrays
+    bool square;            // output rows of n * n reals
+    bool wrench;            // the second output is the base wrench
+    bool grav, fext;        // reads the gravity vector / the tip wrench
+    const char *in[3], *out[3]; // argument names, as the error messages print them
+    constexpr int out_row(int o, int n) const { return wrench && o == 1 ? 6 : (square ? n * n : n); }
+};
+inline constexpr b2k_rne_op_s B2K_RNE_OPS[B2K_GEN_NOPS] = {
+    {3, 1, false, false, true, true, {"q", "qd", "qdd"}, {"tau"}},                                     // RNE
+    {1, 1, true, false, false, false, {"q"}, {"output"}},                                             // INERTIA
+    {1, 1, false, false, true, false, {"q"}, {"output"}},                                             // GRAVLOAD
+    {2, 1, false, false, false, false, {"q", "second input"}, {"output"}},                            // ITORQUE
+    {2, 1, true, false, false, false, {"q", "second input"}, {"output"}},                             // CORIOLIS
+    {3, 1, false, false, true, false, {"q", "second input", "third input"}, {"output"}},              // ACCEL
+    {3, 2, false, true, true, true, {"q", "qd", "qdd"}, {"tau", "wbase"}},                            // RNE_WRENCH
+    {3, 2, true, false, true, true, {"q", "qd", "qdd"}, {"dtau_dq", "dtau_dqd"}},                     // RNE_DERIV
+    {3, 3, true, false, true, false, {"q", "qd", "torque"}, {"dqdd_dq", "dqdd_dqd", "dqdd_dtau"}},    // ACCEL_DERIV
+};
+
+// The arrays of one launch of an operation, device pointers: unused entries are NULL
+struct b2k_rne_args {
+    const void *in[3];
+    void *out[3];
+    long long nrows;
+    const double *grav, *fext;
+};
+
 void b2k_rne_spec_attach(b2k_rne_s *r);
 void b2k_rne_spec_detach(b2k_rne_s *r);
-// mode = B2K_GEN_* (b2k_rne_gen.h); returns the rows served by the specialised kernel (a multiple of 32, possibly 0)
+// mode = B2K_GEN_RNE..B2K_GEN_RNE_WRENCH; returns the rows served by the specialised kernel (a multiple of 32, possibly 0)
 // or a negative b2k_status.  out2: the base wrench (nrows, 6) of B2K_GEN_RNE_WRENCH, NULL for every other mode.
 long long b2k_rne_spec_launch(const b2k_rne_s *r, int mode, int dtype, const void *in0, const void *in1, const void *in2,
                               long long nrows, const double *grav, const double *fext, void *out, void *out2, cudaStream_t st);

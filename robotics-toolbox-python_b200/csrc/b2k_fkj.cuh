@@ -344,15 +344,15 @@ __device__ __forceinline__ void jacob0_row(const ChainP<real, N> &P, const Pose<
 }
 
 // ------------------------------------------------------------------ per-warp staging of output tiles
-// A tile of 32 rows x ROW_ELEMS reals is staged in units of UB bytes (16 when a row is a whole
-// number of 16-byte units, else 8) with a row stride of S units, S odd and >= units per row, so
+// A tile of 32 rows x ROW_ELEMS reals is staged in units of UB bytes (b2k_stage_unit of the row
+// size) with a row stride of S units, S odd and >= units per row, so
 // that the one-row-per-lane vector stores are bank-conflict free.  The warp then copies the tile
 // to global memory unit by unit: consecutive lanes -> consecutive units -> full-width coalesced
 // stores.  When S equals the units per row the stage is the exact image of the output block.
 template <typename real, int ROW_ELEMS>
 struct TileStage {
     static constexpr int ROW_BYTES = ROW_ELEMS * (int)sizeof(real);
-    static constexpr int UB = (ROW_BYTES % 16 == 0) ? 16 : (ROW_BYTES % 8 == 0 ? 8 : 4);
+    static constexpr int UB = b2k_stage_unit(ROW_BYTES);
     static constexpr int RU = ROW_BYTES / UB;          // units per row
     // bank-conflict degree of one-row-per-lane vector stores at row stride RU units
     static constexpr int cgcd(int a, int b) { return b ? cgcd(b, a % b) : a; }

@@ -567,12 +567,16 @@ k_rne_wrench(const __grid_constant__ RneP<real, N> P, const real *__restrict__ q
 // Here one lane does all the calls of its row with the link rotations (sincos) computed once;
 // the loops over unit vectors are runtime loops (code size of ONE recursion), the small n x n
 // accumulators live in local memory.
+// MODE of k_rne_fan: the operation's offset from B2K_GEN_INERTIA
 enum { FAN_INERTIA = 0, FAN_GRAVLOAD = 1, FAN_ITORQUE = 2, FAN_CORIOLIS = 3, FAN_ACCEL = 4 };
+static_assert(B2K_GEN_INERTIA + FAN_GRAVLOAD == B2K_GEN_GRAVLOAD && B2K_GEN_INERTIA + FAN_ITORQUE == B2K_GEN_ITORQUE &&
+                  B2K_GEN_INERTIA + FAN_CORIOLIS == B2K_GEN_CORIOLIS && B2K_GEN_INERTIA + FAN_ACCEL == B2K_GEN_ACCEL,
+              "FAN_* = B2K_GEN_* - B2K_GEN_INERTIA");
 
 template <int MODE, int N>
 struct FanShape {
-    static constexpr int NIN = (MODE == FAN_INERTIA || MODE == FAN_GRAVLOAD) ? 1 : (MODE == FAN_ACCEL ? 3 : 2);
-    static constexpr int OUT = (MODE == FAN_INERTIA || MODE == FAN_CORIOLIS) ? N * N : N;
+    static constexpr int NIN = B2K_RNE_OPS[B2K_GEN_INERTIA + MODE].nin;
+    static constexpr int OUT = B2K_RNE_OPS[B2K_GEN_INERTIA + MODE].out_row(0, N);
 };
 
 // Solves A X = B by Gaussian elimination with partial pivoting (numpy.linalg.solve = LAPACK gesv), A = M (N x N,
@@ -778,126 +782,6 @@ void rne_fill_params(const b2k_rne_s *r, const double *grav, const double *fext,
     b2k_fill_trig<real>(P.trig);
 }
 
-template <typename real, int N, bool MDH, bool ALLREV, bool WRENCH>
-constexpr auto rne_kernel()
-{
-    if constexpr (WRENCH) return k_rne_wrench<real, N, MDH, ALLREV>;
-    else return k_rne<real, N, MDH, ALLREV>;
-}
-
-template <typename real, int N, bool WRENCH>
-int rne_launch_n(const b2k_rne_s *r, const real *q, const real *qd, const real *qdd, long long nrows,
-                 const double *grav, const double *fext, real *tau, real *wbase, cudaStream_t st)
-{
-    RneP<real, N> P;
-    rne_fill_params<real, N>(r, grav, fext, P);
-    const size_t inb = fkj_q_bytes<real>(N);
-    const size_t wsm = (3 * inb + (size_t)TileStage<real, N>::BYTES + (WRENCH ? (size_t)TileStage<real, 6>::BYTES : 0) + 15) & ~(size_t)15;
-    const size_t smem = wsm * B2K_WARPS_PER_BLOCK;
-    const int qmode = (fkj_qmode<real>(q, N) && fkj_qmode<real>(qd, N) && fkj_qmode<real>(qdd, N)) ? 1 : 0;
-    if (((uintptr_t)tau) % TileStage<real, N>::UB) { b2k_set_error("rne: tau must be %d-byte aligned", TileStage<real, N>::UB); return B2K_ERR_INVALID; }
-    if (WRENCH && ((uintptr_t)wbase) % TileStage<real, 6>::UB) { b2k_set_error("rne: wbase must be %d-byte aligned", TileStage<real, 6>::UB); return B2K_ERR_INVALID; }
-    const long long ntiles = (nrows + 31) / 32;
-    const long long nblk_needed = (ntiles + B2K_WARPS_PER_BLOCK - 1) / B2K_WARPS_PER_BLOCK;
-    auto launch = [&](auto kern) -> int {
-        int per_sm = b2k_blocks_per_sm((const void *)kern, B2K_THREADS, smem);
-        if (per_sm < 1) return per_sm < 0 ? per_sm : (b2k_set_error("rne kernel does not fit on an SM"), B2K_ERR_INVALID);
-        long long grid = nblk_needed; // one tile per warp, one-shot grid (see b2k_fkj.cuh launcher)
-        if (grid < 1) grid = 1;
-        if constexpr (WRENCH) kern<<<(unsigned)grid, B2K_THREADS, smem, st>>>(P, q, qd, qdd, nrows, tau, wbase, (int)wsm, (int)inb, qmode);
-        else kern<<<(unsigned)grid, B2K_THREADS, smem, st>>>(P, q, qd, qdd, nrows, tau, (int)wsm, (int)inb, qmode);
-        b2k_count_launch();
-        B2K_CUDA(cudaGetLastError());
-        return B2K_OK;
-    };
-    bool allrev = true;
-    for (int j = 0; j < N; j++) allrev = allrev && !P.prismatic[j];
-    if (r->mdh) return allrev ? launch(rne_kernel<real, N, true, true, WRENCH>()) : launch(rne_kernel<real, N, true, false, WRENCH>());
-    return allrev ? launch(rne_kernel<real, N, false, true, WRENCH>()) : launch(rne_kernel<real, N, false, false, WRENCH>());
-}
-
-// WRENCH: k_rne_wrench (tau and the base wrench wbase (nrows, 6)); otherwise k_rne and wbase is unused
-template <typename real, bool WRENCH>
-int rne_launch(const b2k_rne_s *r, const void *q, const void *qd, const void *qdd, long long nrows, const double *grav,
-               const double *fext, void *tau, void *wbase, cudaStream_t st)
-{
-#define B2K_CASE(NN) \
-    case NN: return rne_launch_n<real, NN, WRENCH>(r, (const real *)q, (const real *)qd, (const real *)qdd, nrows, grav, fext, (real *)tau, (real *)wbase, st);
-    switch (r->n) {
-        B2K_CASE(1) B2K_CASE(2) B2K_CASE(3) B2K_CASE(4) B2K_CASE(5)
-        B2K_CASE(6) B2K_CASE(7) B2K_CASE(8) B2K_CASE(9) B2K_CASE(10)
-    default:
-        b2k_set_error("rne: unsupported joint count %d", r->n);
-        return B2K_ERR_INVALID;
-    }
-#undef B2K_CASE
-}
-
-// ------------------------------------------------------------------ fan-out launcher
-template <typename real, int N, int MODE>
-int rne_fan_launch_mode(const b2k_rne_s *r, const real *in0, const real *in1, const real *in2, long long nrows,
-                        const double *grav, real *out, cudaStream_t st)
-{
-    typedef FanShape<MODE, N> SH;
-    RneP<real, N> P;
-    rne_fill_params<real, N>(r, (MODE == FAN_GRAVLOAD || MODE == FAN_ACCEL) ? grav : nullptr, nullptr, P);
-    if (MODE == FAN_CORIOLIS) { // the reference works on robot.nofriction(True, True) (Dynamics.py:818)
-        for (int j = 0; j < N; j++) { P.c_b[j] = 0; P.c_tcp[j] = 0; P.c_tcm[j] = 0; }
-    }
-    const size_t inb = fkj_q_bytes<real>(N);
-    const size_t wsm = (SH::NIN * inb + (size_t)TileStage<real, SH::OUT>::BYTES + 15) & ~(size_t)15;
-    const size_t smem = wsm * B2K_WARPS_PER_BLOCK;
-    int qmode = fkj_qmode<real>(in0, N);
-    if (SH::NIN >= 2) qmode = qmode && fkj_qmode<real>(in1, N);
-    if (SH::NIN >= 3) qmode = qmode && fkj_qmode<real>(in2, N);
-    if (((uintptr_t)out) % TileStage<real, SH::OUT>::UB) { b2k_set_error("rne fan-out: output must be %d-byte aligned", TileStage<real, SH::OUT>::UB); return B2K_ERR_INVALID; }
-    const long long ntiles = (nrows + 31) / 32;
-    const long long grid = (ntiles + B2K_WARPS_PER_BLOCK - 1) / B2K_WARPS_PER_BLOCK;
-    bool allrev = true;
-    for (int j = 0; j < N; j++) allrev = allrev && !P.prismatic[j];
-    auto launch = [&](auto kern) -> int {
-        int per_sm = b2k_blocks_per_sm((const void *)kern, B2K_THREADS, smem);
-        if (per_sm < 1) return per_sm < 0 ? per_sm : (b2k_set_error("rne fan-out kernel does not fit on an SM"), B2K_ERR_INVALID);
-        kern<<<(unsigned)grid, B2K_THREADS, smem, st>>>(P, in0, in1, in2, nrows, out, (int)wsm, (int)inb, qmode);
-        b2k_count_launch();
-        B2K_CUDA(cudaGetLastError());
-        return B2K_OK;
-    };
-    if (r->mdh) return allrev ? launch(k_rne_fan<real, N, true, true, MODE>) : launch(k_rne_fan<real, N, true, false, MODE>);
-    return allrev ? launch(k_rne_fan<real, N, false, true, MODE>) : launch(k_rne_fan<real, N, false, false, MODE>);
-}
-
-template <typename real, int N>
-int rne_fan_launch_n(const b2k_rne_s *r, int mode, const real *in0, const real *in1, const real *in2, long long nrows,
-                     const double *grav, real *out, cudaStream_t st)
-{
-    switch (mode) {
-    case FAN_INERTIA: return rne_fan_launch_mode<real, N, FAN_INERTIA>(r, in0, in1, in2, nrows, grav, out, st);
-    case FAN_GRAVLOAD: return rne_fan_launch_mode<real, N, FAN_GRAVLOAD>(r, in0, in1, in2, nrows, grav, out, st);
-    case FAN_ITORQUE: return rne_fan_launch_mode<real, N, FAN_ITORQUE>(r, in0, in1, in2, nrows, grav, out, st);
-    case FAN_CORIOLIS: return rne_fan_launch_mode<real, N, FAN_CORIOLIS>(r, in0, in1, in2, nrows, grav, out, st);
-    case FAN_ACCEL: return rne_fan_launch_mode<real, N, FAN_ACCEL>(r, in0, in1, in2, nrows, grav, out, st);
-    }
-    b2k_set_error("rne fan-out: bad mode %d", mode);
-    return B2K_ERR_INVALID;
-}
-
-template <typename real>
-int rne_fan_launch(const b2k_rne_s *r, int mode, const void *in0, const void *in1, const void *in2, long long nrows,
-                   const double *grav, void *out, cudaStream_t st)
-{
-#define B2K_CASE(NN) \
-    case NN: return rne_fan_launch_n<real, NN>(r, mode, (const real *)in0, (const real *)in1, (const real *)in2, nrows, grav, (real *)out, st);
-    switch (r->n) {
-        B2K_CASE(1) B2K_CASE(2) B2K_CASE(3) B2K_CASE(4) B2K_CASE(5)
-        B2K_CASE(6) B2K_CASE(7) B2K_CASE(8) B2K_CASE(9) B2K_CASE(10)
-    default:
-        b2k_set_error("rne fan-out: unsupported joint count %d", r->n);
-        return B2K_ERR_INVALID;
-    }
-#undef B2K_CASE
-}
-
 // ------------------------------------------------------------------ analytical derivatives of the recursion (DESIGN f-13)
 // DERIV_INVERSE: in = (q, qd, qdd); out0 = dtau/dq, out1 = dtau/dqd (N, n, n), [i, k] = dtau_i / dx_k, tau exactly what
 //                k_rne computes with the same gravity and tip wrench.
@@ -1030,54 +914,71 @@ k_rne_deriv(const __grid_constant__ RneP<real, N> P, const real *__restrict__ in
     }
 }
 
-template <typename real, int N, int MODE>
-int rne_deriv_launch_mode(const b2k_rne_s *r, const real *in0, const real *in1, const real *in2, long long nrows,
-                          const double *grav, const double *fext, real *out0, real *out1, real *out2, cudaStream_t st)
+// ------------------------------------------------------------------ the generic launch path of every operation
+// The generic kernel of operation OP (B2K_GEN_*) for one link-table shape
+template <typename real, int N, bool MDH, bool ALLREV, int OP>
+constexpr auto rne_generic_kernel()
 {
-    typedef TileStage<real, N * N> OS;
+    if constexpr (OP == B2K_GEN_RNE) return k_rne<real, N, MDH, ALLREV>;
+    else if constexpr (OP == B2K_GEN_RNE_WRENCH) return k_rne_wrench<real, N, MDH, ALLREV>;
+    else if constexpr (OP == B2K_GEN_RNE_DERIV) return k_rne_deriv<real, N, MDH, ALLREV, DERIV_INVERSE>;
+    else if constexpr (OP == B2K_GEN_ACCEL_DERIV) return k_rne_deriv<real, N, MDH, ALLREV, DERIV_FORWARD>;
+    else return k_rne_fan<real, N, MDH, ALLREV, OP - B2K_GEN_INERTIA>;
+}
+
+// One launch of operation OP's generic kernel over a.nrows rows: a one-shot grid, one 32-row tile per warp.  The caller
+// (b2k_api.cu) has checked every array against B2K_RNE_OPS[OP], the outputs against their stage unit.
+template <typename real, int N, int OP>
+int rne_generic_launch_op(const b2k_rne_s *r, const b2k_rne_args &a, cudaStream_t st)
+{
+    constexpr b2k_rne_op_s op = B2K_RNE_OPS[OP];
     RneP<real, N> P;
-    rne_fill_params<real, N>(r, grav, MODE == DERIV_INVERSE ? fext : nullptr, P);
+    rne_fill_params<real, N>(r, op.grav ? a.grav : nullptr, op.fext ? a.fext : nullptr, P);
+    if (OP == B2K_GEN_CORIOLIS) { // the reference works on robot.nofriction(True, True) (Dynamics.py:818)
+        for (int j = 0; j < N; j++) { P.c_b[j] = 0; P.c_tcp[j] = 0; P.c_tcm[j] = 0; }
+    }
+    // per warp: the input tiles, then the output stage (the base wrench has its own behind tau's; the derivative
+    // outputs take turns in one)
     const size_t inb = fkj_q_bytes<real>(N);
-    const size_t wsm = (3 * inb + (size_t)OS::BYTES + 15) & ~(size_t)15;
+    const size_t stage = (size_t)TileStage<real, op.out_row(0, N)>::BYTES + (op.wrench ? (size_t)TileStage<real, 6>::BYTES : 0);
+    const size_t wsm = (op.nin * inb + stage + 15) & ~(size_t)15;
     const size_t smem = wsm * B2K_WARPS_PER_BLOCK;
-    const int qmode = (fkj_qmode<real>(in0, N) && fkj_qmode<real>(in1, N) && fkj_qmode<real>(in2, N)) ? 1 : 0;
-    for (real *o : {out0, out1, out2})
-        if (o && ((uintptr_t)o) % OS::UB) { b2k_set_error("rne derivatives: outputs must be %d-byte aligned", OS::UB); return B2K_ERR_INVALID; }
-    const long long ntiles = (nrows + 31) / 32;
-    const long long grid = (ntiles + B2K_WARPS_PER_BLOCK - 1) / B2K_WARPS_PER_BLOCK;
-    bool allrev = true;
-    for (int j = 0; j < N; j++) allrev = allrev && !P.prismatic[j];
+    const real *in[3] = {(const real *)a.in[0], (const real *)a.in[1], (const real *)a.in[2]};
+    real *out[3] = {(real *)a.out[0], (real *)a.out[1], (real *)a.out[2]};
+    int qmode = 1;
+    for (int i = 0; i < op.nin; i++) qmode = qmode && fkj_qmode<real>(in[i], N);
+    const long long ntiles = (a.nrows + 31) / 32;
+    const unsigned grid = (unsigned)((ntiles + B2K_WARPS_PER_BLOCK - 1) / B2K_WARPS_PER_BLOCK);
+    const char *what = OP == B2K_GEN_RNE || OP == B2K_GEN_RNE_WRENCH ? "rne" : (OP >= B2K_GEN_RNE_DERIV ? "rne derivative" : "rne fan-out");
     auto launch = [&](auto kern) -> int {
-        int per_sm = b2k_blocks_per_sm((const void *)kern, B2K_THREADS, smem);
-        if (per_sm < 1) return per_sm < 0 ? per_sm : (b2k_set_error("rne derivative kernel does not fit on an SM"), B2K_ERR_INVALID);
-        kern<<<(unsigned)grid, B2K_THREADS, smem, st>>>(P, in0, in1, in2, nrows, out0, out1, out2, (int)wsm, (int)inb, qmode);
+        const int per_sm = b2k_blocks_per_sm((const void *)kern, B2K_THREADS, smem);
+        if (per_sm < 1) return per_sm < 0 ? per_sm : (b2k_set_error("%s kernel does not fit on an SM", what), B2K_ERR_INVALID);
+        if constexpr (B2K_RNE_OPS[OP].nout == 1) kern<<<grid, B2K_THREADS, smem, st>>>(P, in[0], in[1], in[2], a.nrows, out[0], (int)wsm, (int)inb, qmode);
+        else if constexpr (B2K_RNE_OPS[OP].wrench) kern<<<grid, B2K_THREADS, smem, st>>>(P, in[0], in[1], in[2], a.nrows, out[0], out[1], (int)wsm, (int)inb, qmode);
+        else kern<<<grid, B2K_THREADS, smem, st>>>(P, in[0], in[1], in[2], a.nrows, out[0], out[1], out[2], (int)wsm, (int)inb, qmode);
         b2k_count_launch();
         B2K_CUDA(cudaGetLastError());
         return B2K_OK;
     };
-    if (r->mdh) return allrev ? launch(k_rne_deriv<real, N, true, true, MODE>) : launch(k_rne_deriv<real, N, true, false, MODE>);
-    return allrev ? launch(k_rne_deriv<real, N, false, true, MODE>) : launch(k_rne_deriv<real, N, false, false, MODE>);
+    bool allrev = true;
+    for (int j = 0; j < N; j++) allrev = allrev && !P.prismatic[j];
+    if (r->mdh) return allrev ? launch(rne_generic_kernel<real, N, true, true, OP>()) : launch(rne_generic_kernel<real, N, true, false, OP>());
+    return allrev ? launch(rne_generic_kernel<real, N, false, true, OP>()) : launch(rne_generic_kernel<real, N, false, false, OP>());
 }
 
-// mode DERIV_INVERSE or DERIV_FORWARD (fext and out2 unused by the inverse / forward mode respectively)
-template <typename real>
-int rne_deriv_launch(const b2k_rne_s *r, int mode, const void *in0, const void *in1, const void *in2, long long nrows,
-                     const double *grav, const double *fext, void *out0, void *out1, void *out2, cudaStream_t st)
+// The generic kernels of the operations OPS for one dtype, the entry point of the translation unit that instantiates
+// them; op is one of OPS (b2k_api.cu picks the unit).
+template <typename real, int... OPS>
+int rne_generic_launch(const b2k_rne_s *r, int op, const b2k_rne_args &a, cudaStream_t st)
 {
-#define B2K_CASE(NN)                                                                                                        \
-    case NN:                                                                                                                \
-        return mode == DERIV_FORWARD                                                                                        \
-                   ? rne_deriv_launch_mode<real, NN, DERIV_FORWARD>(r, (const real *)in0, (const real *)in1,               \
-                                                                    (const real *)in2, nrows, grav, fext, (real *)out0,     \
-                                                                    (real *)out1, (real *)out2, st)                        \
-                   : rne_deriv_launch_mode<real, NN, DERIV_INVERSE>(r, (const real *)in0, (const real *)in1,               \
-                                                                    (const real *)in2, nrows, grav, fext, (real *)out0,     \
-                                                                    (real *)out1, nullptr, st);
+    int rc = B2K_ERR_INVALID;
+#define B2K_CASE(NN) \
+    case NN: ((op == OPS && (rc = rne_generic_launch_op<real, NN, OPS>(r, a, st), true)) || ...); return rc;
     switch (r->n) {
         B2K_CASE(1) B2K_CASE(2) B2K_CASE(3) B2K_CASE(4) B2K_CASE(5)
         B2K_CASE(6) B2K_CASE(7) B2K_CASE(8) B2K_CASE(9) B2K_CASE(10)
     default:
-        b2k_set_error("rne derivatives: unsupported joint count %d", r->n);
+        b2k_set_error("rne: unsupported joint count %d", r->n);
         return B2K_ERR_INVALID;
     }
 #undef B2K_CASE

@@ -1,7 +1,6 @@
 // fp64 instantiations of the analytical derivatives of the recursion (rne_derivatives, accel_derivatives)
 #include "b2k_rne.cuh"
-int b2k_rne_deriv_launch_f64(const b2k_rne_s *r, int mode, const void *in0, const void *in1, const void *in2, long long nrows,
-                             const double *grav, const double *fext, void *out0, void *out1, void *out2, cudaStream_t st)
+int b2k_rne_generic_deriv_f64(const b2k_rne_s *r, int op, int dtype, const b2k_rne_args &a, cudaStream_t st)
 {
-    return rne_deriv_launch<double>(r, mode, in0, in1, in2, nrows, grav, fext, out0, out1, out2, st);
+    return rne_generic_launch<double, B2K_GEN_RNE_DERIV, B2K_GEN_ACCEL_DERIV>(r, op, a, st);
 }

@@ -1,7 +1,6 @@
 // fp32 instantiations of the dynamics fan-out kernels (inertia, gravload, itorque, coriolis, accel)
 #include "b2k_rne.cuh"
-int b2k_rne_fan_launch_f32(const b2k_rne_s *r, int mode, const void *in0, const void *in1, const void *in2, long long nrows,
-                           const double *grav, void *out, cudaStream_t st)
+int b2k_rne_generic_fan_f32(const b2k_rne_s *r, int op, int dtype, const b2k_rne_args &a, cudaStream_t st)
 {
-    return rne_fan_launch<float>(r, mode, in0, in1, in2, nrows, grav, out, st);
+    return rne_generic_launch<float, B2K_GEN_INERTIA, B2K_GEN_GRAVLOAD, B2K_GEN_ITORQUE, B2K_GEN_CORIOLIS, B2K_GEN_ACCEL>(r, op, a, st);
 }

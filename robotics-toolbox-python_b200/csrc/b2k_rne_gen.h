@@ -6,11 +6,8 @@
 
 #include "b2k_common.cuh"
 
-enum { B2K_GEN_RNE = 0, B2K_GEN_INERTIA = 1, B2K_GEN_GRAVLOAD = 2, B2K_GEN_ITORQUE = 3, B2K_GEN_CORIOLIS = 4, B2K_GEN_ACCEL = 5,
-       B2K_GEN_RNE_WRENCH = 6 };
-
 struct b2k_gen_opts {
-    int mode = B2K_GEN_RNE;
+    int mode = B2K_GEN_RNE; // B2K_GEN_RNE..B2K_GEN_RNE_WRENCH (b2k_common.cuh)
     int grav_mask = 7;  // bit k: base acceleration component k may be non-zero
     int has_fext = 0;   // a tip wrench is given
 };

@@ -582,9 +582,10 @@ std::string build_source(const GenFn &gen, int n, int mode, int dtype, Program &
     p.consts = g.consts;
     p.nc = (int)g.consts.size();
     p.n_mul = g.n_mul; p.n_fma = g.n_fma; p.n_add = g.n_add;
-    p.nin = (mode == B2K_GEN_RNE || mode == B2K_GEN_ACCEL || mode == B2K_GEN_RNE_WRENCH) ? 3 : ((mode == B2K_GEN_ITORQUE || mode == B2K_GEN_CORIOLIS) ? 2 : 1);
-    p.nout = (mode == B2K_GEN_INERTIA || mode == B2K_GEN_CORIOLIS) ? n * n : n;
-    p.nout2 = mode == B2K_GEN_RNE_WRENCH ? 6 : 0; // tau (N, n) and the base wrench (N, 6)
+    const b2k_rne_op_s &op = B2K_RNE_OPS[mode];
+    p.nin = op.nin;
+    p.nout = op.out_row(0, n);
+    p.nout2 = op.nout > 1 ? op.out_row(1, n) : 0; // tau (N, n) and the base wrench (N, 6)
     p.nres = mode == B2K_GEN_ACCEL ? n * n + n : p.nout + p.nout2;
     const int es = dtype == B2K_F64 ? 8 : 4;
     // one-row-per-lane reads of an exact-image tile: conflict degree gcd(row words, banks served per wavefront)
@@ -809,7 +810,7 @@ long long b2k_rne_spec_launch(const b2k_rne_s *r, int mode, int dtype, const voi
     int has_fext = 0;
     if (rne && fext)
         for (int k = 0; k < 6; k++) has_fext |= (fext[k] != 0.0);
-    const bool uses_grav = rne || mode == B2K_GEN_GRAVLOAD || mode == B2K_GEN_ACCEL;
+    const bool uses_grav = B2K_RNE_OPS[mode].grav;
     const Key key(mode, dtype, uses_grav ? grav_mask_of(grav) : 0, has_fext);
     Program *p = get_program(static_cast<SpecCache *>(r->spec), dh_gen(r, key), r->n, key);
     if (!p || !p->ok) return refuse(p ? p->why : "no cache");
@@ -858,7 +859,7 @@ extern "C" int b2k_rne_spec_info(b2k_rne_t r, int mode, int dtype, const double 
         {
             // mode 200 + m: the forward-dynamics integrator built around operation m (only m = accel exists)
             const int gm = mode % 100;
-            const bool ug = gm == B2K_GEN_RNE || gm == B2K_GEN_GRAVLOAD || gm == B2K_GEN_ACCEL || gm == B2K_GEN_RNE_WRENCH;
+            const bool ug = gm >= 0 && gm < B2K_GEN_NOPS && B2K_RNE_OPS[gm].grav;
             const Key key(mode, dtype, ug ? grav_mask_of(grav) : 0, has_fext);
             const Key gkey(gm, dtype, ug ? grav_mask_of(grav) : 0, has_fext);
             Program *p = get_program(static_cast<SpecCache *>(r->spec), dh_gen(r, gkey), r->n, key);
@@ -925,8 +926,6 @@ static Program *tree_program(b2k_tree_t t, int mode, int dtype, int gmask)
     }, t->n, key);
 }
 
-static bool mode_uses_gravity(int mode) { return mode == B2K_GEN_RNE || mode == B2K_GEN_GRAVLOAD || mode == B2K_GEN_ACCEL; }
-
 // Robot.rne (mode 0) and the operations DynamicsMixin builds on it (modes 1-5: inertia, gravload, itorque, coriolis, accel)
 // for a rigid-body tree: the generated kernel on the full tiles, one padded tile for the ragged tail.
 static int tree_run(const char *fn, b2k_tree_t t, int mode, int dtype, const void *in0, const void *in1, const void *in2, int64_t N,
@@ -935,9 +934,9 @@ static int tree_run(const char *fn, b2k_tree_t t, int mode, int dtype, const voi
     if (!t) { b2k_set_error("%s: tree handle is NULL", fn); return B2K_ERR_INVALID; }
     if (mode < B2K_GEN_RNE || mode > B2K_GEN_ACCEL) { b2k_set_error("%s: operation %d is not one of B2K_DYN_*", fn, mode); return B2K_ERR_INVALID; }
     if (dtype != B2K_F32 && dtype != B2K_F64) { b2k_set_error("%s: dtype must be B2K_F32 or B2K_F64", fn); return B2K_ERR_INVALID; }
-    const int nin = (mode == B2K_GEN_RNE || mode == B2K_GEN_ACCEL) ? 3 : ((mode == B2K_GEN_ITORQUE || mode == B2K_GEN_CORIOLIS) ? 2 : 1);
+    const int nin = B2K_RNE_OPS[mode].nin;
     if (N < 0 || (N > 0 && (!in0 || (nin >= 2 && !in1) || (nin >= 3 && !in2) || !out))) { b2k_set_error("%s: bad arguments", fn); return B2K_ERR_INVALID; }
-    const bool ug = mode_uses_gravity(mode);
+    const bool ug = B2K_RNE_OPS[mode].grav;
     if (ug && !grav) { b2k_set_error("%s: grav is NULL (pass MINUS the robot's gravity: a_grav of Robot.rne)", fn); return B2K_ERR_INVALID; }
     const uintptr_t al = (uintptr_t)in0 | (uintptr_t)(nin >= 2 ? in1 : in0) | (uintptr_t)(nin >= 3 ? in2 : in0) | (uintptr_t)out;
     if (al & 15) { b2k_set_error("%s: arrays must be 16-byte aligned", fn); return B2K_ERR_INVALID; }
@@ -1016,7 +1015,7 @@ extern "C" int b2k_tree_info(b2k_tree_t t, int op, int dtype, const double *grav
 {
     if (!t || !buf || cap < 1) { b2k_set_error("b2k_tree_info: bad arguments"); return B2K_ERR_INVALID; }
     if (op < B2K_GEN_RNE || op > B2K_GEN_ACCEL) { b2k_set_error("b2k_tree_info: operation %d is not one of B2K_DYN_*", op); return B2K_ERR_INVALID; }
-    Program *p = tree_program(t, op, dtype, mode_uses_gravity(op) ? grav_mask_of(grav) : 0);
+    Program *p = tree_program(t, op, dtype, B2K_RNE_OPS[op].grav ? grav_mask_of(grav) : 0);
     if (!p || !p->ok) snprintf(buf, (size_t)cap, "unavailable (%s)", p ? p->why.c_str() : "no cache");
     else if (op == B2K_GEN_RNE)
         snprintf(buf, (size_t)cap, "k_rne_spec<%s,tree n=%d>: %d mul + %d fma + %d add per row, %d constants, %d regs, %zu B smem/block",
