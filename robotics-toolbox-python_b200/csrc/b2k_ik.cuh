@@ -457,20 +457,25 @@ __device__ __forceinline__ bool ik_qp_step(const IkP<real, N> &K, const IkQp<rea
 // (Jw^T Jw + d^2 I)^-1 Jw^T ew for n < 6 (n x n), Jw = diag(ws) J, ew = diag(ws) e -- the same operator
 // as the reference's SVD wherever the factorisation exists; where it does not (a singular
 // configuration with d = 0) the search is abandoned, where the reference takes a wild step.
+// A mask that leaves fewer weighted rows than joints makes Jw^T Jw singular for every q, so such a step of n < 6
+// joints takes the 6x6 row form too: with the masked rows decoupled it is the minimum-norm step whenever the
+// weighted rows of J are independent.
 template <typename real, int N>
 __device__ __forceinline__ bool ik_pinv_step(const IkP<real, N> &K, real (*J)[6], const real *e, real *g)
 {
     real ew[6];
     const real d2 = K.lambda * K.lambda;
+    int wrows = 0; // rows the weights keep
 #pragma unroll
     for (int a = 0; a < 6; a++) {
         ew[a] = K.ws[a] * e[a];
+        wrows += K.ws[a] != (real)0 ? 1 : 0;
         if (!K.unit_w) {
 #pragma unroll
             for (int j = 0; j < N; j++) J[j][a] *= K.ws[a];
         }
     }
-    if (N >= 6) {
+    if (N >= 6 || wrows < N) {
         real A[21];
 #pragma unroll
         for (int a = 0; a < 6; a++)
@@ -519,7 +524,8 @@ __device__ __forceinline__ bool ik_eval(const ChainP<real, N> &P, const IkP<real
 {
     Pose<real> Te;
     real zj[N][3], pj[N][3], e[6];
-    // jindex is dense 0..n-1 here (checked on the host, like the reference's C++ loop assumes)
+    // q holds the n joints in chain order whatever the chain's jindex (a sub-chain's jindices need not be 0..n-1): joint j
+    // reads q[j], as q0, q_out and the joint limits are laid out (b2k_ik_lm)
     chain_forward<real, N, true, PROF, 1>(P, [&](int j, int) { return q[j]; }, Te, zj, pj);
     ik_angle_axis<real>(Te, Tp, e);
     real E = 0;
