@@ -1,10 +1,14 @@
 """Forward-dynamics front end shared by DHRobot.fdyn and Robot.fdyn (reference DynamicsMixin.fdyn, Dynamics.py:185-422,
 which every robot class inherits through BaseRobot): argument handling, the scipy route for a Python torque callable,
 and the call into the device-resident Dormand-Prince ensemble integrator (b2k_rne_fdyn / b2k_tree_fdyn)."""
+import warnings
+
 import numpy as np
 
 from . import _buffers as B
 from . import _lib
+
+_EPS = np.finfo(float).eps
 
 
 def fdyn(robot, entry, handle, kernel_gravity, T, q0, Q=None, Q_args=None, qd0=None, solver="RK45", solver_args=None, dt=None,
@@ -51,6 +55,19 @@ def fdyn(robot, entry, handle, kernel_gravity, T, q0, Q=None, Q_args=None, qd0=N
     unknown = set(solver_args) - {"rtol", "atol", "max_step", "first_step"}
     if unknown:
         raise ValueError(f"unsupported solver_args for the device integrator: {sorted(unknown)}")
+    rtol, atol = solver_args.get("rtol", 1e-3), solver_args.get("atol", 1e-6)
+    if np.ndim(rtol) or np.ndim(atol):
+        raise ValueError("the device integrator takes scalar rtol and atol (one tolerance for every state component)")
+    rtol, atol = float(rtol), float(atol)
+    if rtol < 100 * _EPS:  # scipy's validate_tol
+        warnings.warn(f"At least one element of `rtol` is too small. Setting `rtol = np.maximum(rtol, {100 * _EPS})`.", stacklevel=3)
+        rtol = 100 * _EPS
+    first_step = solver_args.get("first_step")
+    if first_step is not None:  # scipy's validate_first_step; None selects the first step automatically
+        if first_step <= 0:
+            raise ValueError("`first_step` must be positive.")
+        if first_step > abs(T):
+            raise ValueError("`first_step` exceeds bounds.")
     dt_ = B.pick_dtype(q0, dtype)
     host = not B.is_tensor(q0)
     q0d = B.to_device(q0, dt_)
@@ -89,14 +106,16 @@ def fdyn(robot, entry, handle, kernel_gravity, T, q0, Q=None, Q_args=None, qd0=N
             x.fill_(float("nan"))
     _lib.check(entry(
         handle, B.code(dt_), B.ptr(q0d), B.ptr(qd0d), nb, float(T), _lib.dptr(g), mode, _lib.dptr(tau), B.ptr(tau_rows),
-        _lib.dptr(kp), _lib.dptr(kd), _lib.dptr(qs), float(solver_args.get("rtol", 1e-3)), float(solver_args.get("atol", 1e-6)),
-        float(solver_args.get("max_step", np.inf)), float(solver_args.get("first_step") or 0.0), float(dt or 0.0), int(grid), M,
+        _lib.dptr(kp), _lib.dptr(kd), _lib.dptr(qs), rtol, atol,
+        float(solver_args.get("max_step", np.inf)), float(first_step or 0.0), float(dt or 0.0), int(grid), M,
         B.ptr(t_out), B.ptr(q_out), B.ptr(qd_out), B.ptr(cnt), B.ptr(stat), B.stream_ptr(q0d)))
     st = B.to_host(stat)
     if (st & 1).any():
         raise RuntimeError("integration completed with failed status ")  # the reference's message for a failed step
     if (st & 2).any():
         raise RuntimeError(f"more than max_steps = {M} accepted steps; pass dt for a uniform grid or raise max_steps")
+    if grid and (B.to_host(cnt) != M).any():  # every grid sample must have been written
+        raise RuntimeError(f"the integrator filled {B.to_host(cnt).min()} of the {M} samples of the output grid")
     if single:
         k = int(cnt[0])
         t, q, qd = (B.to_host(x[0, :k]) for x in (t_out, q_out, qd_out))

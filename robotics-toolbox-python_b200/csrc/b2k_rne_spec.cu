@@ -461,6 +461,10 @@ k_fdyn(const __grid_constant__ SpecP P, const __grid_constant__ FdynP F, const r
         t = tn;
         for (int i = 0; i < NS; i++) { y[i] = yn[i]; K[0][i] = K[6][i]; }
     }
+    // np.arange(0, T, dt) can end on T itself (T = 2.1, dt = 0.3), and k dt in `real` may round above T (fp32): the
+    // samples not yet written are the state at T
+    if (F.grid && status == 0)
+        for (; next_grid < F.M; next_grid++) emit((real)next_grid * F.dt, y);
     out_count[tr] = count;
     out_status[tr] = status | (count > F.M ? 2 : 0); // 2: more accepted steps than the capacity M
 }

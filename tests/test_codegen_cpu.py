@@ -182,6 +182,22 @@ def test_generated_kernels_compile_for_sm_90a_through_the_library():
         lib.b2k_rne_destroy(h)
 
 
+@pytest.mark.skipif(not any(os.path.exists(p) for p in ("/usr/local/cuda/lib64/libnvrtc.so.12", "/usr/local/cuda/lib64/libnvrtc.so")),
+                    reason="NVRTC not installed")
+@pytest.mark.parametrize("n", range(1, 11))
+def test_fdyn_integrator_compiles_at_every_joint_count(n):
+    """k_fdyn carries K[7][2n] and the n*n + n LDL^T scratch per lane: it builds for sm_90a at every joint count the
+    device sweep runs (tests/test_gpu_fdyn.py), DH at odd n and MDH at even n, in both dtypes."""
+    lib = rtb._lib.lib()
+    mdh = n % 2 == 0
+    h = handle(n, mdh, ch.pack_rne(random_links(np.random.default_rng(900 + n), n, mdh), mdh=mdh))
+    for dt in (rtb._lib.F64, rtb._lib.F32):
+        buf = C.create_string_buffer(4096)
+        rtb._lib.check(lib.b2k_rne_spec_info(h, 205, dt, rtb._lib.dptr(np.array([0.5, -1.0, 3.0])), 0, buf, 4096))
+        assert buf.value.startswith(b"k_fdyn<"), buf.value[:600]
+    lib.b2k_rne_destroy(h)
+
+
 # ------------------------------------------------------------------ rigid-body trees (Robot.rne)
 TREE_HARNESS = r"""
 #include <cmath>
