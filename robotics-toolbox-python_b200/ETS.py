@@ -684,24 +684,19 @@ class ETS:
         E = B.empty((N,), dt, like=Td)
         if seed is None:
             seed = int(np.random.default_rng().integers(0, 2**63 - 1))
+        lead = (self._chain, B.code(dt), B.ptr(Td), N, B.ptr(q0d), int(ilimit), int(slimit), float(tol),
+                int(bool(joint_limits)), _lib.dptr(we))
+        tail = (B.ptr(q), B.ptr(succ), B.ptr(its), B.ptr(srch), B.ptr(E), B.stream_ptr(Td))
+        seed, rng_per_row = int(seed) & (2**64 - 1), int(bool(rng_per_row))
         if qp is not None:  # the Python loop with the quadratic-programming step (semantics is SEM_PYTHON)
             kj, ks, kq, km, ps, pi = qp
-            _lib.check(_lib.lib().b2k_ikine_qp(
-                self._chain, B.code(dt), B.ptr(Td), N, B.ptr(q0d), int(ilimit), int(slimit), float(tol),
-                int(bool(joint_limits)), _lib.dptr(we), int(seed) & (2**64 - 1), int(bool(rng_per_row)), kj, ks, kq, km,
-                ps, _lib.dptr(pi), B.ptr(q), B.ptr(succ), B.ptr(its), B.ptr(srch), B.ptr(E), B.stream_ptr(Td)))
+            _lib.check(_lib.lib().b2k_ikine_qp(*lead, seed, rng_per_row, kj, ks, kq, km, ps, _lib.dptr(pi), *tail))
         elif null is None:
-            _lib.check(_lib.lib().b2k_ik_lm(
-                self._chain, B.code(dt), B.ptr(Td), N, B.ptr(q0d), int(ilimit), int(slimit), float(tol),
-                int(bool(joint_limits)), _lib.dptr(we), float(k), meth, int(seed) & (2**64 - 1), semantics,
-                int(bool(rng_per_row)), B.ptr(q), B.ptr(succ), B.ptr(its), B.ptr(srch), B.ptr(E), B.stream_ptr(Td)))
+            _lib.check(_lib.lib().b2k_ik_lm(*lead, float(k), meth, seed, semantics, rng_per_row, *tail))
         else:  # the Python loop with the null-space terms (semantics is SEM_PYTHON)
             kq, km, ps, pi = null
-            _lib.check(_lib.lib().b2k_ikine_null(
-                self._chain, B.code(dt), B.ptr(Td), N, B.ptr(q0d), int(ilimit), int(slimit), float(tol),
-                int(bool(joint_limits)), _lib.dptr(we), float(k), meth, int(seed) & (2**64 - 1),
-                int(bool(rng_per_row)), float(kq), float(km), float(ps), _lib.dptr(pi), B.ptr(q), B.ptr(succ),
-                B.ptr(its), B.ptr(srch), B.ptr(E), B.stream_ptr(Td)))
+            _lib.check(_lib.lib().b2k_ikine_null(*lead, float(k), meth, seed, rng_per_row, float(kq), float(km),
+                                                 float(ps), _lib.dptr(pi), *tail))
         if host:
             q, succ, its, srch, E = (B.to_host(x) for x in (q, succ, its, srch, E))
         return q, succ, its, srch, E, single
@@ -712,11 +707,8 @@ class ETS:
         (ETS.ik_LM, ETS.py:2014-2170 -> fknm.IK_LM_c).  One target (4,4) returns the reference's tuple
         ``(q, success, iterations, searches, residual)``; an (N,4,4) batch returns the same tuple of
         arrays, row i being the reference called on target i."""
-        q, s, it, sr, E, single = self._ik(Tep, q0, ilimit, slimit, tol, mask, joint_limits, k, method, seed,
-                                           _lib.SEM_CPP, True, dtype)
-        if single:
-            return q[0], int(s[0]), int(it[0]), int(sr[0]), float(E[0])
-        return q, s, it, sr, E
+        return self._ik_tuple(self._ik(Tep, q0, ilimit, slimit, tol, mask, joint_limits, k, method, seed,
+                                       _lib.SEM_CPP, True, dtype))
 
     def _ik_tuple(self, r):
         q, s, it, sr, E, single = r
@@ -743,6 +735,16 @@ class ETS:
         return self._ik_tuple(self._ik(Tep, q0, ilimit, slimit, tol, mask, joint_limits, 0.0, _lib.IK_GN,
                                        seed, _lib.SEM_CPP, True, dtype))
 
+    def _pi_vector(self, pi):
+        """pi of the null-space terms and the QP damper as a contiguous fp64 n-vector; a scalar holds for every joint"""
+        n = self.n
+        pa = np.asarray(pi, dtype=np.float64)
+        if pa.ndim == 0:
+            pa = np.full(n, float(pa))
+        elif pa.shape != (n,):
+            raise ValueError(f"pi must be a scalar or have {n} elements, got shape {pa.shape}")
+        return np.ascontiguousarray(pa)
+
     def _null_args(self, kq, km, ps, pi):
         """(kq, km, ps, pi as an n-vector) for b2k_ikine_null, or None when neither null-space term is on.
         The terms of the reference's _calc_qnull run only for a gain > 0; on a chain of n <= 6 joints a full-rank J
@@ -750,19 +752,13 @@ class ETS:
         kq, km = float(kq), float(km)
         if not (kq > 0 or km > 0):
             return None
-        n = self.n
-        pa = np.asarray(pi, dtype=np.float64)
-        if pa.ndim == 0:
-            pa = np.full(n, float(pa))
-        elif pa.shape != (n,):
-            raise ValueError(f"pi must be a scalar or have {n} elements, got shape {pa.shape}")
-        pa = np.ascontiguousarray(pa)
+        pa = self._pi_vector(pi)
         ps = float(ps)
         if not (np.isfinite(kq) and np.isfinite(km) and np.isfinite(ps) and np.isfinite(pa).all()):
             raise ValueError("kq, km, ps and pi must be finite")
         if kq > 0 and (pa == ps).any():
             raise ValueError(f"ps == pi at joint {int(np.argmax(pa == ps))}: the joint-limit term divides by ps - pi")
-        if n < 7:
+        if self.n < 7:
             return None
         return kq, km, ps, pa
 
@@ -813,21 +809,15 @@ class ETS:
     def _qp_args(self, kj, ks, kq, km, ps, pi):
         """(kj, ks, kq, km, ps, pi as an n-vector) for b2k_ikine_qp, after the checks DESIGN (f-11) lists"""
         kj, ks, kq, km, ps = (float(x) for x in (kj, ks, kq, km, ps))
-        n = self.n
-        pa = np.asarray(pi, dtype=np.float64)
-        if pa.ndim == 0:
-            pa = np.full(n, float(pa))
-        elif pa.shape != (n,):
-            raise ValueError(f"pi must be a scalar or have {n} elements, got shape {pa.shape}")
-        pa = np.ascontiguousarray(pa)
+        pa = self._pi_vector(pi)
         if not all(np.isfinite(x) for x in (kj, ks, kq, km, ps)) or not np.isfinite(pa).all():
             raise ValueError("kj, ks, kq, km, ps and pi must be finite")
         if not (kj > 0 and ks > 0):
             raise ValueError("kj and ks must be > 0: the step's quadratic form is not positive definite otherwise")
         if kq > 0 and (pa == ps).any():
             raise ValueError(f"ps == pi at joint {int(np.argmax(pa == ps))}: the velocity damper divides by pi - ps")
-        if km > 0 and n < 6:
-            raise ValueError(f"km > 0 needs at least 6 joints (n = {n}): J J^T is singular for fewer")
+        if km > 0 and self.n < 6:
+            raise ValueError(f"km > 0 needs at least 6 joints (n = {self.n}): J J^T is singular for fewer")
         return kj, ks, kq, km, ps, pa
 
     def ikine_QP(self, Tep, q0=None, ilimit: int = 30, slimit: int = 100, tol: float = 1e-6, mask=None,

@@ -487,25 +487,20 @@ extern "C" int b2k_rne_wrench_host(b2k_rne_t r, int dtype, const void *q, const 
 }
 
 // ------------------------------------------------------------------ inverse kinematics
-int b2k_ik_launch_f32(const b2k_chain_s *, const void *, long long, const void *, int, int, double, int, const double *,
-                      double, int, unsigned long long, int, int, void *, int *, int *, int *, void *, cudaStream_t);
-int b2k_ik_launch_f64(const b2k_chain_s *, const void *, long long, const void *, int, int, double, int, const double *,
-                      double, int, unsigned long long, int, int, void *, int *, int *, int *, void *, cudaStream_t);
+// the launchers (b2k_ik.cuh), one translation unit per family of kernels and dtype
+typedef int IkLaunchFn(const b2k_chain_s *, const IkArgs &, cudaStream_t);
+IkLaunchFn b2k_ik_launch_f32, b2k_ik_launch_f64, b2k_ik_nr_launch_f32, b2k_ik_nr_launch_f64, b2k_ik_ns_launch_f32,
+    b2k_ik_ns_launch_f64, b2k_ik_qp_launch_f32, b2k_ik_qp_launch_f64;
 
-int b2k_ik_nr_launch_f32(const b2k_chain_s *, const void *, long long, const void *, int, int, double, int, const double *,
-                         double, int, unsigned long long, int, int, void *, int *, int *, int *, void *, cudaStream_t);
-int b2k_ik_nr_launch_f64(const b2k_chain_s *, const void *, long long, const void *, int, int, double, int, const double *,
-                         double, int, unsigned long long, int, int, void *, int *, int *, int *, void *, cudaStream_t);
+enum { IK_LM, IK_NULL, IK_QP }; // b2k_ik_lm, b2k_ikine_null, b2k_ikine_qp
 
-extern "C" int b2k_ik_lm(b2k_chain_t c, int dtype, const void *Tep, int64_t N, const void *q0, int ilimit, int slimit,
-                         double tol, int reject_jl, const double *we, double lambda, int method, uint64_t seed,
-                         int semantics, int rng_per_row, void *q_out, int32_t *success, int32_t *iterations,
-                         int32_t *searches, void *residual, void *stream)
+// Every argument of the three IK entry points is checked before any CUDA call; then the variant and the method pick the
+// translation unit.
+static int ik_dispatch(const char *fn, int variant, b2k_chain_t c, int dtype, IkArgs a, void *stream)
 {
-    const char *fn = "b2k_ik_lm";
     if (!c) { b2k_set_error("%s: chain handle is NULL", fn); return B2K_ERR_INVALID; }
     if (dtype != B2K_F32 && dtype != B2K_F64) { b2k_set_error("%s: dtype must be B2K_F32 or B2K_F64", fn); return B2K_ERR_INVALID; }
-    if (N < 0) { b2k_set_error("%s: N is negative", fn); return B2K_ERR_INVALID; }
+    if (a.N < 0) { b2k_set_error("%s: N is negative", fn); return B2K_ERR_INVALID; }
     // The solver works on the chain's own joint vector (q0 and q_out hold the n joints in chain order, i.e.
     // q[ets.jindices] -- what IKSolver.solve hands back, IK.py:216-240,346); a sub-chain of a larger robot
     // (jindices 3..6, say) is therefore served as it is.  Two joints driven by one coordinate are not.
@@ -513,36 +508,81 @@ extern "C" int b2k_ik_lm(b2k_chain_t c, int dtype, const void *Tep, int64_t N, c
         b2k_set_error("%s: two joints of the chain share a jindex (coupled joints are outside the solver's model)", fn);
         return B2K_ERR_INVALID;
     }
-    if (ilimit < 1 || slimit < 1) { b2k_set_error("%s: ilimit and slimit must be >= 1", fn); return B2K_ERR_INVALID; }
-    if (method < B2K_LM_CHAN || method > B2K_IK_GN) { b2k_set_error("%s: bad method %d", fn, method); return B2K_ERR_INVALID; }
-    if (semantics != B2K_IK_SEM_CPP && semantics != B2K_IK_SEM_PYTHON) { b2k_set_error("%s: bad semantics %d", fn, semantics); return B2K_ERR_INVALID; }
-    int rc;
-    if ((rc = check_out(fn, "Tep", Tep, N)) || (rc = check_out(fn, "q_out", q_out, N)) ||
-        (rc = check_out(fn, "success", success, N)) || (rc = check_out(fn, "iterations", iterations, N)) ||
-        (rc = check_out(fn, "searches", searches, N)) || (rc = check_out(fn, "residual", residual, N)))
-        return rc;
-    if ((method == B2K_IK_NR || method == B2K_IK_GN) && lambda < 0) { b2k_set_error("%s: pinv_damping is negative", fn); return B2K_ERR_INVALID; }
-    if (N == 0) return B2K_OK;
-    B2K_ON_DEVICE_OF(Tep);
-    cudaStream_t st = (cudaStream_t)stream;
-    if (method == B2K_IK_NR || method == B2K_IK_GN) {
-        auto nr = dtype == B2K_F64 ? b2k_ik_nr_launch_f64 : b2k_ik_nr_launch_f32;
-        return nr(c, Tep, N, q0, ilimit, slimit, tol, reject_jl, we, method == B2K_IK_GN ? 0.0 : lambda, method, seed,
-                  semantics, rng_per_row, q_out, success, iterations, searches, residual, st);
+    if (variant == IK_NULL && (c->n < 7 || c->n > B2K_MAX_JOINTS)) {
+        b2k_set_error("%s: the null-space terms need a redundant chain of 7..%d joints (n = %d)", fn, B2K_MAX_JOINTS, c->n);
+        return B2K_ERR_INVALID;
     }
-    if (dtype == B2K_F64)
-        return b2k_ik_launch_f64(c, Tep, N, q0, ilimit, slimit, tol, reject_jl, we, lambda, method, seed, semantics,
-                                 rng_per_row, q_out, success, iterations, searches, residual, st);
-    return b2k_ik_launch_f32(c, Tep, N, q0, ilimit, slimit, tol, reject_jl, we, lambda, method, seed, semantics,
-                             rng_per_row, q_out, success, iterations, searches, residual, st);
+    if (variant == IK_QP && (c->n < 1 || c->n > B2K_MAX_JOINTS)) { b2k_set_error("%s: unsupported joint count %d", fn, c->n); return B2K_ERR_INVALID; }
+    if (a.ilimit < 1 || a.slimit < 1) { b2k_set_error("%s: ilimit and slimit must be >= 1", fn); return B2K_ERR_INVALID; }
+    if (variant != IK_QP && (a.method < B2K_LM_CHAN || a.method > B2K_IK_GN)) { b2k_set_error("%s: bad method %d", fn, a.method); return B2K_ERR_INVALID; }
+    if (variant == IK_LM && a.semantics != B2K_IK_SEM_CPP && a.semantics != B2K_IK_SEM_PYTHON) {
+        b2k_set_error("%s: bad semantics %d", fn, a.semantics);
+        return B2K_ERR_INVALID;
+    }
+    const auto &g = a.gains;
+    if (variant == IK_NULL) {
+        if (!isfinite(g.kq) || !isfinite(g.km)) { b2k_set_error("%s: kq and km must be finite", fn); return B2K_ERR_INVALID; }
+        if (!(g.kq > 0) && !(g.km > 0)) { b2k_set_error("%s: at least one of kq and km must be > 0", fn); return B2K_ERR_INVALID; }
+        if (!isfinite(g.ps)) { b2k_set_error("%s: ps must be finite", fn); return B2K_ERR_INVALID; }
+    }
+    if (variant == IK_QP) {
+        if (!isfinite(g.kj) || !isfinite(g.ks) || !isfinite(g.kq) || !isfinite(g.km) || !isfinite(g.ps)) {
+            b2k_set_error("%s: kj, ks, kq, km and ps must be finite", fn);
+            return B2K_ERR_INVALID;
+        }
+        if (!(g.kj > 0) || !(g.ks > 0)) {
+            b2k_set_error("%s: kj and ks must be > 0 (the step's quadratic form is not positive definite otherwise)", fn);
+            return B2K_ERR_INVALID;
+        }
+    }
+    // pi: read by the null-space terms always, by the QP step only for its velocity damper (kq > 0)
+    if (variant == IK_NULL || (variant == IK_QP && g.kq > 0)) {
+        if (!g.pi) { b2k_set_error("%s: pi is NULL", fn); return B2K_ERR_INVALID; }
+        for (int i = 0; i < c->n; i++) {
+            if (!isfinite(g.pi[i])) { b2k_set_error("%s: pi[%d] is not finite", fn, i); return B2K_ERR_INVALID; }
+            if (g.kq > 0 && g.ps == g.pi[i]) {
+                b2k_set_error("%s: ps == pi[%d] divides by zero in the %s", fn, i,
+                              variant == IK_NULL ? "joint-limit term" : "velocity damper");
+                return B2K_ERR_INVALID;
+            }
+        }
+    }
+    if (variant == IK_QP && g.km > 0 && c->n < 6) {
+        b2k_set_error("%s: km > 0 needs at least 6 joints (n = %d): J J^T is singular for fewer", fn, c->n);
+        return B2K_ERR_INVALID;
+    }
+    int rc;
+    if ((rc = check_out(fn, "Tep", a.Tep, a.N)) || (rc = check_out(fn, "q_out", a.q_out, a.N)) ||
+        (rc = check_out(fn, "success", a.success, a.N)) || (rc = check_out(fn, "iterations", a.iterations, a.N)) ||
+        (rc = check_out(fn, "searches", a.searches, a.N)) || (rc = check_out(fn, "residual", a.residual, a.N)))
+        return rc;
+    const bool pinv = variant != IK_QP && (a.method == B2K_IK_NR || a.method == B2K_IK_GN);
+    if (pinv && a.lambda < 0) { b2k_set_error("%s: pinv_damping is negative", fn); return B2K_ERR_INVALID; }
+    if (a.N == 0) return B2K_OK;
+    B2K_ON_DEVICE_OF(a.Tep);
+    // What the kernels read of lambda, method and semantics: GN takes the undamped pseudo-inverse step, the QP step is
+    // neither damped nor weighted, and the null-space terms and the QP step run in the Python solver loop only.
+    if (variant == IK_QP) a.lambda = 0.0, a.method = 0;
+    else if (a.method == B2K_IK_GN) a.lambda = 0.0;
+    if (variant != IK_LM) a.semantics = B2K_IK_SEM_PYTHON;
+    const bool f64 = dtype == B2K_F64;
+    IkLaunchFn *launch = variant == IK_QP     ? (f64 ? b2k_ik_qp_launch_f64 : b2k_ik_qp_launch_f32)
+                         : variant == IK_NULL ? (f64 ? b2k_ik_ns_launch_f64 : b2k_ik_ns_launch_f32)
+                         : pinv               ? (f64 ? b2k_ik_nr_launch_f64 : b2k_ik_nr_launch_f32)
+                                              : (f64 ? b2k_ik_launch_f64 : b2k_ik_launch_f32);
+    return launch(c, a, (cudaStream_t)stream);
 }
 
-int b2k_ik_ns_launch_f32(const b2k_chain_s *, const void *, long long, const void *, int, int, double, int, const double *,
-                         double, int, unsigned long long, int, void *, int *, int *, int *, void *, const IkNullArgs &,
-                         cudaStream_t);
-int b2k_ik_ns_launch_f64(const b2k_chain_s *, const void *, long long, const void *, int, int, double, int, const double *,
-                         double, int, unsigned long long, int, void *, int *, int *, int *, void *, const IkNullArgs &,
-                         cudaStream_t);
+extern "C" int b2k_ik_lm(b2k_chain_t c, int dtype, const void *Tep, int64_t N, const void *q0, int ilimit, int slimit,
+                         double tol, int reject_jl, const double *we, double lambda, int method, uint64_t seed,
+                         int semantics, int rng_per_row, void *q_out, int32_t *success, int32_t *iterations,
+                         int32_t *searches, void *residual, void *stream)
+{
+    return ik_dispatch("b2k_ik_lm", IK_LM, c, dtype,
+                       {Tep, q0, q_out, success, iterations, searches, residual, N, ilimit, slimit, tol, reject_jl, we,
+                        lambda, method, seed, semantics, rng_per_row, {}},
+                       stream);
+}
 
 extern "C" int b2k_ikine_null(b2k_chain_t c, int dtype, const void *Tep, int64_t N, const void *q0, int ilimit,
                               int slimit, double tol, int reject_jl, const double *we, double lambda, int method,
@@ -550,92 +590,21 @@ extern "C" int b2k_ikine_null(b2k_chain_t c, int dtype, const void *Tep, int64_t
                               void *q_out, int32_t *success, int32_t *iterations, int32_t *searches, void *residual,
                               void *stream)
 {
-    const char *fn = "b2k_ikine_null";
-    if (!c) { b2k_set_error("%s: chain handle is NULL", fn); return B2K_ERR_INVALID; }
-    if (dtype != B2K_F32 && dtype != B2K_F64) { b2k_set_error("%s: dtype must be B2K_F32 or B2K_F64", fn); return B2K_ERR_INVALID; }
-    if (N < 0) { b2k_set_error("%s: N is negative", fn); return B2K_ERR_INVALID; }
-    if (!c->distinct_jindex) {
-        b2k_set_error("%s: two joints of the chain share a jindex (coupled joints are outside the solver's model)", fn);
-        return B2K_ERR_INVALID;
-    }
-    if (c->n < 7 || c->n > B2K_MAX_JOINTS) {
-        b2k_set_error("%s: the null-space terms need a redundant chain of 7..%d joints (n = %d)", fn, B2K_MAX_JOINTS, c->n);
-        return B2K_ERR_INVALID;
-    }
-    if (ilimit < 1 || slimit < 1) { b2k_set_error("%s: ilimit and slimit must be >= 1", fn); return B2K_ERR_INVALID; }
-    if (method < B2K_LM_CHAN || method > B2K_IK_GN) { b2k_set_error("%s: bad method %d", fn, method); return B2K_ERR_INVALID; }
-    if (!isfinite(kq) || !isfinite(km)) { b2k_set_error("%s: kq and km must be finite", fn); return B2K_ERR_INVALID; }
-    if (!(kq > 0) && !(km > 0)) { b2k_set_error("%s: at least one of kq and km must be > 0", fn); return B2K_ERR_INVALID; }
-    if (!isfinite(ps)) { b2k_set_error("%s: ps must be finite", fn); return B2K_ERR_INVALID; }
-    if (!pi) { b2k_set_error("%s: pi is NULL", fn); return B2K_ERR_INVALID; }
-    for (int i = 0; i < c->n; i++) {
-        if (!isfinite(pi[i])) { b2k_set_error("%s: pi[%d] is not finite", fn, i); return B2K_ERR_INVALID; }
-        if (kq > 0 && ps == pi[i]) { b2k_set_error("%s: ps == pi[%d] divides by zero in the joint-limit term", fn, i); return B2K_ERR_INVALID; }
-    }
-    int rc;
-    if ((rc = check_out(fn, "Tep", Tep, N)) || (rc = check_out(fn, "q_out", q_out, N)) ||
-        (rc = check_out(fn, "success", success, N)) || (rc = check_out(fn, "iterations", iterations, N)) ||
-        (rc = check_out(fn, "searches", searches, N)) || (rc = check_out(fn, "residual", residual, N)))
-        return rc;
-    if ((method == B2K_IK_NR || method == B2K_IK_GN) && lambda < 0) { b2k_set_error("%s: pinv_damping is negative", fn); return B2K_ERR_INVALID; }
-    if (N == 0) return B2K_OK;
-    B2K_ON_DEVICE_OF(Tep);
-    const IkNullArgs ns{kq, km, ps, pi};
-    auto launch = dtype == B2K_F64 ? b2k_ik_ns_launch_f64 : b2k_ik_ns_launch_f32;
-    return launch(c, Tep, N, q0, ilimit, slimit, tol, reject_jl, we, method == B2K_IK_GN ? 0.0 : lambda, method, seed,
-                  rng_per_row, q_out, success, iterations, searches, residual, ns, (cudaStream_t)stream);
+    return ik_dispatch("b2k_ikine_null", IK_NULL, c, dtype,
+                       {Tep, q0, q_out, success, iterations, searches, residual, N, ilimit, slimit, tol, reject_jl, we,
+                        lambda, method, seed, 0, rng_per_row, {0.0, 0.0, kq, km, ps, pi}},
+                       stream);
 }
-
-int b2k_ik_qp_launch_f32(const b2k_chain_s *, const void *, long long, const void *, int, int, double, int, const double *,
-                         unsigned long long, int, void *, int *, int *, int *, void *, const IkQpArgs &, cudaStream_t);
-int b2k_ik_qp_launch_f64(const b2k_chain_s *, const void *, long long, const void *, int, int, double, int, const double *,
-                         unsigned long long, int, void *, int *, int *, int *, void *, const IkQpArgs &, cudaStream_t);
 
 extern "C" int b2k_ikine_qp(b2k_chain_t c, int dtype, const void *Tep, int64_t N, const void *q0, int ilimit,
                             int slimit, double tol, int reject_jl, const double *we, uint64_t seed, int rng_per_row,
                             double kj, double ks, double kq, double km, double ps, const double *pi, void *q_out,
                             int32_t *success, int32_t *iterations, int32_t *searches, void *residual, void *stream)
 {
-    const char *fn = "b2k_ikine_qp";
-    if (!c) { b2k_set_error("%s: chain handle is NULL", fn); return B2K_ERR_INVALID; }
-    if (dtype != B2K_F32 && dtype != B2K_F64) { b2k_set_error("%s: dtype must be B2K_F32 or B2K_F64", fn); return B2K_ERR_INVALID; }
-    if (N < 0) { b2k_set_error("%s: N is negative", fn); return B2K_ERR_INVALID; }
-    if (!c->distinct_jindex) {
-        b2k_set_error("%s: two joints of the chain share a jindex (coupled joints are outside the solver's model)", fn);
-        return B2K_ERR_INVALID;
-    }
-    if (c->n < 1 || c->n > B2K_MAX_JOINTS) { b2k_set_error("%s: unsupported joint count %d", fn, c->n); return B2K_ERR_INVALID; }
-    if (ilimit < 1 || slimit < 1) { b2k_set_error("%s: ilimit and slimit must be >= 1", fn); return B2K_ERR_INVALID; }
-    if (!isfinite(kj) || !isfinite(ks) || !isfinite(kq) || !isfinite(km) || !isfinite(ps)) {
-        b2k_set_error("%s: kj, ks, kq, km and ps must be finite", fn);
-        return B2K_ERR_INVALID;
-    }
-    if (!(kj > 0) || !(ks > 0)) {
-        b2k_set_error("%s: kj and ks must be > 0 (the step's quadratic form is not positive definite otherwise)", fn);
-        return B2K_ERR_INVALID;
-    }
-    if (kq > 0) {
-        if (!pi) { b2k_set_error("%s: pi is NULL", fn); return B2K_ERR_INVALID; }
-        for (int i = 0; i < c->n; i++) {
-            if (!isfinite(pi[i])) { b2k_set_error("%s: pi[%d] is not finite", fn, i); return B2K_ERR_INVALID; }
-            if (ps == pi[i]) { b2k_set_error("%s: ps == pi[%d] divides by zero in the velocity damper", fn, i); return B2K_ERR_INVALID; }
-        }
-    }
-    if (km > 0 && c->n < 6) {
-        b2k_set_error("%s: km > 0 needs at least 6 joints (n = %d): J J^T is singular for fewer", fn, c->n);
-        return B2K_ERR_INVALID;
-    }
-    int rc;
-    if ((rc = check_out(fn, "Tep", Tep, N)) || (rc = check_out(fn, "q_out", q_out, N)) ||
-        (rc = check_out(fn, "success", success, N)) || (rc = check_out(fn, "iterations", iterations, N)) ||
-        (rc = check_out(fn, "searches", searches, N)) || (rc = check_out(fn, "residual", residual, N)))
-        return rc;
-    if (N == 0) return B2K_OK;
-    B2K_ON_DEVICE_OF(Tep);
-    const IkQpArgs qp{kj, ks, kq, km, ps, pi};
-    auto launch = dtype == B2K_F64 ? b2k_ik_qp_launch_f64 : b2k_ik_qp_launch_f32;
-    return launch(c, Tep, N, q0, ilimit, slimit, tol, reject_jl, we, seed, rng_per_row, q_out, success, iterations,
-                  searches, residual, qp, (cudaStream_t)stream);
+    return ik_dispatch("b2k_ikine_qp", IK_QP, c, dtype,
+                       {Tep, q0, q_out, success, iterations, searches, residual, N, ilimit, slimit, tol, reject_jl, we,
+                        0.0, 0, seed, 0, rng_per_row, {kj, ks, kq, km, ps, pi}},
+                       stream);
 }
 
 // ------------------------------------------------------------------ dynamics fan-outs

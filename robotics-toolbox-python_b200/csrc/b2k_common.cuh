@@ -97,16 +97,27 @@ struct b2k_chain_s {
     int distinct_jindex; // no two joints read the same column of q
 };
 
-// null-space gains and influence band of b2k_ikine_null, as the host passes them (validated there; b2k_ik.cuh)
-struct IkNullArgs {
-    double kq, km, ps;
-    const double *pi; // host, n
-};
-
-// gains and damper band of b2k_ikine_qp, as the host passes them (validated there; b2k_ik.cuh)
-struct IkQpArgs {
-    double kj, ks, kq, km, ps;
-    const double *pi; // host, n; read only when kq > 0
+// One call of b2k_ik_lm, b2k_ikine_null or b2k_ikine_qp as the host passes it to the launchers (b2k_ik.cuh), after
+// ik_dispatch (b2k_api.cu) has validated it.  Tep .. residual are device arrays of N rows; we and gains.pi are host.
+struct IkArgs {
+    const void *Tep, *q0;
+    void *q_out;
+    int *success, *iterations, *searches;
+    void *residual;
+    long long N;
+    int ilimit, slimit;
+    double tol;
+    int reject_jl;
+    const double *we;
+    double lambda;
+    int method;
+    unsigned long long seed;
+    int semantics, rng_per_row;
+    // the gains and band of the null-space terms (kq, km, ps, pi) and of the QP step (all six); pi holds n values
+    struct {
+        double kj, ks, kq, km, ps;
+        const double *pi;
+    } gains;
 };
 
 // the unit a per-warp output stage of rows of `row_bytes` is copied in (TileStage<real, n>::UB in b2k_fkj.cuh): 16 bytes

@@ -629,13 +629,9 @@ __device__ __forceinline__ bool ik_wrap_and_check(const IkP<real, N> &K, real *q
 // two_phase != 0 a lane does only the FIRST search of a problem; a problem whose first search
 // fails is appended to the hard list (with its iteration contribution) for k_ik_restarts.
 // Resident blocks per SM asked of ptxas: with the normal equations and the Jacobian in registers the fp32 kernels
-// fit 128 registers (4 blocks) without spilling; the fp64 ones would take ~250 (2 blocks) and run 1-4 % faster held to 168 (3 blocks, ~150 B of spills).  -DB2K_IK_MINB=n overrides both
+// fit 128 registers (4 blocks) without spilling; the fp64 ones would take ~250 (2 blocks) and run 1-4 % faster held to 168 (3 blocks, ~150 B of spills)
 // (DESIGN 3.5 has the sweep: 4 / 5 / 6 blocks measure the same, 8 spills and is 10 % slower).
-#ifdef B2K_IK_MINB
-template <typename real> constexpr int ik_min_blocks() { return B2K_IK_MINB; }
-#else
 template <typename real> constexpr int ik_min_blocks() { return sizeof(real) == 4 ? 4 : 3; }
-#endif
 // The kernels with the null-space term (k_ik_lm_ns, k_ik_restarts_ns) hold J, the Gram factor and the N Hessian sums
 // at once.  Chosen from -Xptxas -v: fp32 fits 168 registers (3 blocks) without spilling up to N = 9 and 255 (2 blocks)
 // at N = 10; fp64 at 255 (2 blocks) spills less than the plain fp64 k_ik_lm does at 168 (DESIGN (f-7) has the table).
@@ -1004,47 +1000,50 @@ constexpr auto ik_kernel_b()
     else return &k_ik_restarts<real, N, PROF, G, STEP>;
 }
 
-template <typename real, int N, int STEP, bool NS = false>
-int ik_launch_n(const b2k_chain_s *c, const real *Tep, long long nprob, const real *q0, int ilimit, int slimit,
-                double tol, int reject_jl, const double *we, double lambda, int method, unsigned long long seed,
-                int semantics, int rng_per_row, real *q_out, int *success, int *iterations, int *searches,
-                real *residual, cudaStream_t st, const IkNullArgs *ns = nullptr, const IkQpArgs *qp = nullptr)
+template <typename real, int N, int STEP, bool NS>
+int ik_launch_n(const b2k_chain_s *c, const IkArgs &a, cudaStream_t st)
 {
+    const real *Tep = (const real *)a.Tep, *q0 = (const real *)a.q0;
+    real *q_out = (real *)a.q_out, *residual = (real *)a.residual;
+    int *success = a.success, *iterations = a.iterations, *searches = a.searches;
+    const long long nprob = a.N;
+    const int ilimit = a.ilimit, slimit = a.slimit;
     ChainP<real, N> P;
     b2k_fill_chain<real, N>(c, nullptr, nullptr, true, P);
     IkP<real, N> K;
     for (int i = 0; i < N; i++) { K.qlim_l[i] = (real)c->qlim_l[i]; K.qlim_h[i] = (real)c->qlim_h[i]; }
     K.unit_w = 1;
     for (int k = 0; k < 6; k++) {
-        K.we[k] = we ? (real)we[k] : (real)1;
+        K.we[k] = a.we ? (real)a.we[k] : (real)1;
         if (K.we[k] != (real)1) K.unit_w = 0;
         // NR weighs only the cost E, never the step (ik.cpp:141-146); GN weighs both (ik.cpp:102-103)
-        K.ws[k] = (method == B2K_IK_GN && we) ? (real)sqrt(we[k] > 0 ? we[k] : 0.0) : (real)1;
+        K.ws[k] = (a.method == B2K_IK_GN && a.we) ? (real)sqrt(a.we[k] > 0 ? a.we[k] : 0.0) : (real)1;
     }
-    K.lambda = (real)lambda; K.tol = (real)tol;
-    K.ilimit = ilimit; K.slimit = slimit; K.method = method; K.reject_jl = reject_jl ? 1 : 0;
-    K.semantics = semantics; K.rng_per_row = rng_per_row ? 1 : 0; K.has_q0 = q0 ? 1 : 0; K.seed = seed;
+    K.lambda = (real)a.lambda; K.tol = (real)a.tol;
+    K.ilimit = ilimit; K.slimit = slimit; K.method = a.method; K.reject_jl = a.reject_jl ? 1 : 0;
+    K.semantics = a.semantics; K.rng_per_row = a.rng_per_row ? 1 : 0; K.has_q0 = q0 ? 1 : 0; K.seed = a.seed;
+    const auto &gn = a.gains;
     std::conditional_t<STEP == 2, IkQp<real, N>, IkNs<real, N>> S{};
     if constexpr (STEP == 2) {
-        S.use_q = qp->kq > 0 ? 1 : 0;
-        S.use_m = qp->km > 0 ? 1 : 0;
-        S.kj_ks = (real)(qp->kj / qp->ks);
-        S.inv_kmks = S.use_m ? (real)(1.0 / (qp->km * qp->ks)) : (real)0;
-        S.inv_kq = S.use_q ? (real)(1.0 / qp->kq) : (real)0;
-        S.ps = (real)qp->ps;
-        for (int i = 0; i < N; i++) S.pi[i] = S.use_q ? (real)qp->pi[i] : (real)0;
+        S.use_q = gn.kq > 0 ? 1 : 0;
+        S.use_m = gn.km > 0 ? 1 : 0;
+        S.kj_ks = (real)(gn.kj / gn.ks);
+        S.inv_kmks = S.use_m ? (real)(1.0 / (gn.km * gn.ks)) : (real)0;
+        S.inv_kq = S.use_q ? (real)(1.0 / gn.kq) : (real)0;
+        S.ps = (real)gn.ps;
+        for (int i = 0; i < N; i++) S.pi[i] = S.use_q ? (real)gn.pi[i] : (real)0;
     } else if constexpr (NS) {
-        S.use_q = ns->kq > 0 ? 1 : 0;
-        S.use_m = ns->km > 0 ? 1 : 0;
-        S.inv_kq = S.use_q ? (real)(1.0 / ns->kq) : (real)0; // the reference scales by 1.0 / λ (IK.py _calc_qnull)
-        S.inv_km = S.use_m ? (real)(1.0 / ns->km) : (real)0;
-        S.ps = (real)ns->ps;
-        for (int i = 0; i < N; i++) S.pi[i] = (real)ns->pi[i];
+        S.use_q = gn.kq > 0 ? 1 : 0;
+        S.use_m = gn.km > 0 ? 1 : 0;
+        S.inv_kq = S.use_q ? (real)(1.0 / gn.kq) : (real)0; // the reference scales by 1.0 / λ (IK.py _calc_qnull)
+        S.inv_km = S.use_m ? (real)(1.0 / gn.km) : (real)0;
+        S.ps = (real)gn.ps;
+        for (int i = 0; i < N; i++) S.pi[i] = (real)gn.pi[i];
     }
     // one launch of kern (NS, STEP = 2: with S appended as its last argument)
-    auto go = [&](auto kern, long long grid, auto... a) {
-        if constexpr (NS || STEP == 2) kern<<<(unsigned)grid, B2K_THREADS, 0, st>>>(a..., S);
-        else kern<<<(unsigned)grid, B2K_THREADS, 0, st>>>(a...);
+    auto go = [&](auto kern, long long grid, auto... args) {
+        if constexpr (NS || STEP == 2) kern<<<(unsigned)grid, B2K_THREADS, 0, st>>>(args..., S);
+        else kern<<<(unsigned)grid, B2K_THREADS, 0, st>>>(args...);
     };
     // Two phases when restarts are allowed and the batch is large enough to matter: phase A runs the
     // first search of every problem (one lane each); phase B runs the restarts of the problems that
@@ -1101,30 +1100,27 @@ int ik_launch_n(const b2k_chain_s *c, const real *Tep, long long nprob, const re
         B2K_CUDA(cudaGetLastError());
         return B2K_OK;
     };
-    int rc = c->dh_like ? launch_a(ik_kernel_a<real, N, 1, STEP, NS>()) : launch_a(ik_kernel_a<real, N, 0, STEP, NS>());
-    if (rc == B2K_OK && two_phase) {
+    // phase A, then (two phases) the restart rounds, on the kernels of the chain profile PROF
+    auto launch_all = [&](auto prof) -> int {
+        constexpr int PROF = decltype(prof)::value;
+        const int rc = launch_a(ik_kernel_a<real, N, PROF, STEP, NS>());
+        if (rc != B2K_OK || !two_phase) return rc;
         // Restart rounds: 4 lanes (searches 1-4), ONE batch of 8 lanes (searches 5-12), then whole warps (32 searches
         // per batch) for the handful of problems still unsolved -- a protocol whose hardest problem needs 50 (or all
         // 100) searches otherwise runs 6 (12) serial batches of 30 evaluations for a few dozen problems.  A search
         // limit too small for the earlier rounds starts with 8-lane groups, or keeps them to the end.
         constexpr int G1 = 4, G3 = 32;
-        if (slimit > 1 + G1) {
-            rc = c->dh_like ? launch_b(ik_kernel_b<real, N, 1, G1, STEP, NS>(), G1, hard_idx, hard_count, 1, 1, cont_idx, cont_count)
-                            : launch_b(ik_kernel_b<real, N, 0, G1, STEP, NS>(), G1, hard_idx, hard_count, 1, 1, cont_idx, cont_count);
-            if (rc == B2K_OK && slimit > 1 + G1 + G) {
-                rc = c->dh_like ? launch_b(ik_kernel_b<real, N, 1, G, STEP, NS>(), G, cont_idx, cont_count, 1 + G1, 1, hard_idx, third_count)
-                                : launch_b(ik_kernel_b<real, N, 0, G, STEP, NS>(), G, cont_idx, cont_count, 1 + G1, 1, hard_idx, third_count);
-                if (rc == B2K_OK)
-                    rc = c->dh_like ? launch_b(ik_kernel_b<real, N, 1, G3, STEP, NS>(), G3, hard_idx, third_count, 1 + G1 + G, 0x7fffffff, nullptr, nullptr)
-                                    : launch_b(ik_kernel_b<real, N, 0, G3, STEP, NS>(), G3, hard_idx, third_count, 1 + G1 + G, 0x7fffffff, nullptr, nullptr);
-            } else if (rc == B2K_OK)
-                rc = c->dh_like ? launch_b(ik_kernel_b<real, N, 1, G, STEP, NS>(), G, cont_idx, cont_count, 1 + G1, 0x7fffffff, nullptr, nullptr)
-                                : launch_b(ik_kernel_b<real, N, 0, G, STEP, NS>(), G, cont_idx, cont_count, 1 + G1, 0x7fffffff, nullptr, nullptr);
-        } else {
-            rc = c->dh_like ? launch_b(ik_kernel_b<real, N, 1, G, STEP, NS>(), G, hard_idx, hard_count, 1, 0x7fffffff, nullptr, nullptr)
-                            : launch_b(ik_kernel_b<real, N, 0, G, STEP, NS>(), G, hard_idx, hard_count, 1, 0x7fffffff, nullptr, nullptr);
-        }
-    }
+        if (slimit <= 1 + G1)
+            return launch_b(ik_kernel_b<real, N, PROF, G, STEP, NS>(), G, hard_idx, hard_count, 1, 0x7fffffff, nullptr, nullptr);
+        const int rc1 = launch_b(ik_kernel_b<real, N, PROF, G1, STEP, NS>(), G1, hard_idx, hard_count, 1, 1, cont_idx, cont_count);
+        if (rc1 != B2K_OK) return rc1;
+        if (slimit <= 1 + G1 + G)
+            return launch_b(ik_kernel_b<real, N, PROF, G, STEP, NS>(), G, cont_idx, cont_count, 1 + G1, 0x7fffffff, nullptr, nullptr);
+        const int rc2 = launch_b(ik_kernel_b<real, N, PROF, G, STEP, NS>(), G, cont_idx, cont_count, 1 + G1, 1, hard_idx, third_count);
+        if (rc2 != B2K_OK) return rc2;
+        return launch_b(ik_kernel_b<real, N, PROF, G3, STEP, NS>(), G3, hard_idx, third_count, 1 + G1 + G, 0x7fffffff, nullptr, nullptr);
+    };
+    int rc = c->dh_like ? launch_all(std::integral_constant<int, 1>()) : launch_all(std::integral_constant<int, 0>());
     if (scratch) {
         cudaError_t e = cudaFreeAsync(scratch, st);
         if (e != cudaSuccess && rc == B2K_OK) rc = b2k_cuda_fail(e, "cudaFreeAsync");
@@ -1132,73 +1128,22 @@ int ik_launch_n(const b2k_chain_s *c, const real *Tep, long long nprob, const re
     return rc;
 }
 
-template <typename real, int STEP = 0>
-int ik_launch(const b2k_chain_s *c, const void *Tep, long long nprob, const void *q0, int ilimit, int slimit, double tol,
-              int reject_jl, const double *we, double lambda, int method, unsigned long long seed, int semantics,
-              int rng_per_row, void *q_out, int *success, int *iterations, int *searches, void *residual,
-              cudaStream_t st)
+// The launcher of one translation unit (b2k_ik_*.cu): the kernels STEP and NS pick (ik_kernel_a / ik_kernel_b) at the
+// chain's joint count.  The null-space kernels exist for 7..10 joints only: a full-rank J of a chain with n <= 6 has an
+// empty null space, and b2k_ikine_null rejects such chains.
+template <typename real, int STEP, bool NS = false>
+int ik_launch(const b2k_chain_s *c, const IkArgs &a, cudaStream_t st)
 {
+    constexpr int NMIN = NS ? 7 : 1;
 #define B2K_CASE(NN)                                                                                                   \
     case NN:                                                                                                           \
-        return ik_launch_n<real, NN, STEP>(c, (const real *)Tep, nprob, (const real *)q0, ilimit, slimit, tol, reject_jl, we, \
-                                     lambda, method, seed, semantics, rng_per_row, (real *)q_out, success, iterations, \
-                                     searches, (real *)residual, st);
+        if constexpr (NN >= NMIN) return ik_launch_n<real, NN, STEP, NS>(c, a, st);                                    \
+        break;
     switch (c->n) {
         B2K_CASE(1) B2K_CASE(2) B2K_CASE(3) B2K_CASE(4) B2K_CASE(5)
         B2K_CASE(6) B2K_CASE(7) B2K_CASE(8) B2K_CASE(9) B2K_CASE(10)
-    default:
-        b2k_set_error("ik_lm: unsupported joint count %d", c->n);
-        return B2K_ERR_INVALID;
     }
 #undef B2K_CASE
-}
-
-// b2k_ikine_null: the Python solver loop with the null-space term, for 7..10 joints (a full-rank J of a chain with n <= 6
-// has an empty null space; the host sends those chains to ik_launch).  STEP as the method asks.
-template <typename real>
-int ik_ns_launch(const b2k_chain_s *c, const void *Tep, long long nprob, const void *q0, int ilimit, int slimit, double tol,
-                 int reject_jl, const double *we, double lambda, int method, unsigned long long seed, int rng_per_row,
-                 void *q_out, int *success, int *iterations, int *searches, void *residual, const IkNullArgs &ns,
-                 cudaStream_t st)
-{
-#define B2K_CASE(NN)                                                                                                   \
-    case NN:                                                                                                           \
-        return pinv ? ik_launch_n<real, NN, 1, true>(c, (const real *)Tep, nprob, (const real *)q0, ilimit, slimit, tol,  \
-                                                     reject_jl, we, lambda, method, seed, B2K_IK_SEM_PYTHON,           \
-                                                     rng_per_row, (real *)q_out, success, iterations, searches,        \
-                                                     (real *)residual, st, &ns)                                        \
-                    : ik_launch_n<real, NN, 0, true>(c, (const real *)Tep, nprob, (const real *)q0, ilimit, slimit, tol,  \
-                                                     reject_jl, we, lambda, method, seed, B2K_IK_SEM_PYTHON,           \
-                                                     rng_per_row, (real *)q_out, success, iterations, searches,        \
-                                                     (real *)residual, st, &ns);
-    const bool pinv = method == B2K_IK_NR || method == B2K_IK_GN;
-    switch (c->n) {
-        B2K_CASE(7) B2K_CASE(8) B2K_CASE(9) B2K_CASE(10)
-    default:
-        b2k_set_error("ikine_null: unsupported joint count %d (7..10)", c->n);
-        return B2K_ERR_INVALID;
-    }
-#undef B2K_CASE
-}
-
-// b2k_ikine_qp: the Python solver loop with the quadratic-programming step, for 1..10 joints
-template <typename real>
-int ik_qp_launch(const b2k_chain_s *c, const void *Tep, long long nprob, const void *q0, int ilimit, int slimit, double tol,
-                 int reject_jl, const double *we, unsigned long long seed, int rng_per_row, void *q_out, int *success,
-                 int *iterations, int *searches, void *residual, const IkQpArgs &qp, cudaStream_t st)
-{
-#define B2K_CASE(NN)                                                                                                   \
-    case NN:                                                                                                           \
-        return ik_launch_n<real, NN, 2, false>(c, (const real *)Tep, nprob, (const real *)q0, ilimit, slimit, tol,     \
-                                               reject_jl, we, 0.0, 0, seed, B2K_IK_SEM_PYTHON, rng_per_row,          \
-                                               (real *)q_out, success, iterations, searches, (real *)residual, st,    \
-                                               nullptr, &qp);
-    switch (c->n) {
-        B2K_CASE(1) B2K_CASE(2) B2K_CASE(3) B2K_CASE(4) B2K_CASE(5)
-        B2K_CASE(6) B2K_CASE(7) B2K_CASE(8) B2K_CASE(9) B2K_CASE(10)
-    default:
-        b2k_set_error("ikine_qp: unsupported joint count %d", c->n);
-        return B2K_ERR_INVALID;
-    }
-#undef B2K_CASE
+    b2k_set_error("ik: unsupported joint count %d", c->n);
+    return B2K_ERR_INVALID;
 }

@@ -1,10 +1,3 @@
 // f64 instantiations of the IK kernels with the pseudo-inverse step (Newton-Raphson / Gauss-Newton)
 #include "b2k_ik.cuh"
-int b2k_ik_nr_launch_f64(const b2k_chain_s *c, const void *Tep, long long nprob, const void *q0, int ilimit, int slimit,
-                         double tol, int reject_jl, const double *we, double lambda, int method, unsigned long long seed,
-                         int semantics, int rng_per_row, void *q_out, int *success, int *iterations, int *searches,
-                         void *residual, cudaStream_t st)
-{
-    return ik_launch<double, 1>(c, Tep, nprob, q0, ilimit, slimit, tol, reject_jl, we, lambda, method, seed, semantics,
-                            rng_per_row, q_out, success, iterations, searches, residual, st);
-}
+int b2k_ik_nr_launch_f64(const b2k_chain_s *c, const IkArgs &a, cudaStream_t st) { return ik_launch<double, 1>(c, a, st); }

@@ -149,6 +149,53 @@ def test_widened_entry_points_validate_before_launching():
     assert lib.b2k_chain_destroy(h) == 0
 
 
+IK_PANDA = rtb.models.Panda().ets()  # kept alive: the table below passes its chain handle
+IK_SHARED = rtb.ET.Rz(jindex=0) * rtb.ET.tx(0.3) * rtb.ET.Ry(jindex=0)  # two joints read q[0]
+
+
+def _ik_lm_call(chain=None, dtype=1, N=4, ilimit=30, slimit=100, method=0, semantics=0, lam=1.0, Tep=8, q_out=8,
+                succ=8, its=8, srch=8, res=8):
+    lib = rtb._lib.lib()
+    chain = IK_PANDA._chain if chain is None else chain
+    rc = lib.b2k_ik_lm(chain, dtype, Tep, N, None, ilimit, slimit, 1e-6, 1, None, lam, method, 0, semantics, 1, q_out,
+                       succ, its, srch, res, None)
+    return rc, lib.b2k_last_error().decode()
+
+
+@pytest.mark.parametrize("kw,msg", [
+    (dict(chain=0), "chain handle is NULL"),
+    (dict(dtype=2), "dtype must be"),
+    (dict(N=-1), "N is negative"),
+    (dict(chain=IK_SHARED._chain), "share a jindex"),
+    (dict(ilimit=0), "ilimit and slimit"),
+    (dict(slimit=0), "ilimit and slimit"),
+    (dict(method=-1), "bad method -1"),
+    (dict(method=5), "bad method 5"),
+    (dict(semantics=2), "bad semantics 2"),
+    (dict(Tep=None), "Tep is NULL"),
+    (dict(q_out=None), "q_out is NULL"),
+    (dict(succ=None), "success is NULL"),
+    (dict(its=None), "iterations is NULL"),
+    (dict(srch=None), "searches is NULL"),
+    (dict(res=None), "residual is NULL"),
+    (dict(method=rtb._lib.IK_NR, lam=-0.5), "pinv_damping is negative"),
+    (dict(method=rtb._lib.IK_GN, lam=-0.5), "pinv_damping is negative"),
+    (dict(N=-1, dtype=2), "dtype must be"),  # the checks run in the order above
+    (dict(method=5, res=None), "bad method"),
+    (dict(res=None, method=rtb._lib.IK_NR, lam=-0.5), "residual is NULL"),
+    (dict(N=0), None),
+    (dict(N=0, Tep=None, q_out=None, succ=None, its=None, srch=None, res=None), None),
+    (dict(N=0, method=2, semantics=1, lam=-1.0), None),  # the LM damping rules take any lambda
+])
+def test_ik_lm_rejects_bad_arguments_before_launching(kw, msg):
+    rc, err = _ik_lm_call(**kw)
+    if msg is None:
+        assert rc == 0, err
+        return
+    assert rc == -1
+    assert msg in err, err
+
+
 # ------------------------------------------------------------------ host-side mirror of the reference interface
 def test_models_match_the_reference_tables():
     """Product model tables == the independent restatement used to generate the goldens."""
