@@ -391,7 +391,10 @@ int b2k_tree_fdyn(b2k_tree_t tree, int dtype, const void *q0, const void *qd0, i
  *   Mx_in (N,6,6) a given Mx (Cx then needs no M)    xd (N,6) task-space velocity    w (N,6) wrench
  * inverse B2K_OPS_INV: Ji = inv(Ja), n must be 6, partial pivoting as LAPACK getrf; a row with an exactly zero pivot gets
  * NaN in every output that depends on Ji (numpy raises LinAlgError for it).  B2K_OPS_PINV: Ji = pinv(Ja) by one-sided
- * Jacobi SVD, singular values <= 1e-15 s_max dropped as numpy.linalg.pinv does.  One launch writes any non-NULL output:
+ * Jacobi SVD, singular values <= 1e-15 s_max dropped as numpy.linalg.pinv does.  The cut is the same in fp32, where it
+ * keeps a singular value that is zero in exact arithmetic but ~1e-8 s_max after rounding, so the fp32 pseudo-inverse of
+ * a numerically rank-deficient Ja is not meaningful; only exact structure is dropped reliably (an all-zero column of Ja
+ * for n <= 6, an all-zero row for n >= 7).  One launch writes any non-NULL output:
  *   Ji  (N,n,6)                                                         needs Ja or Ji_in
  *   Mx  (N,6,6) = Ji^T M Ji                      (inertia_x)            needs M
  *   Cx  (N,6,6) = Ji^T C Ji - Mx Jd Ji           (coriolis_x)           needs C, Jd and M or Mx_in
