@@ -428,9 +428,11 @@ int b2k_ikine_6s(int dtype, const double *dh, const double *base, const double *
                  const int32_t *conf, void *q, int32_t *ok, void *stream);
 
 /* ---------------------------------------------------------------- pure functions of the Jacobian
+ * The six functions below take a batch of Jacobians J (N,6,n), n = 1..B2K_MAX_JOINTS.  J, qd and the output must be
+ * aligned to their element size.  Every argument is checked before any CUDA call; N = 0 needs no arrays (NULL is
+ * accepted) and touches no device.
  * b2k_hessian replaces fknm.ETS_hessian0 / ETS_hessiane (fknm.cpp:583-783 -> _ETS_hessian
  * methods.cpp:16-32): H (N,n,6,n) from J (N,6,n); pass jacob0 for hessian0, jacobe for hessiane.
- * These and the other functions of J below take n = 1..B2K_MAX_JOINTS; any other n is rejected before any CUDA call.
  * b2k_manipulability is the Yoshikawa measure of ETS.manipulability (ETS.py:1780-1787):
  * m = sqrt|det(Ja Ja^T)| over the Cartesian rows selected by axes_mask (bit k = row k of J;
  * 63 = all, 7 = translational, 56 = rotational); |det Ja| when Ja is square. */
@@ -439,7 +441,7 @@ int b2k_hessian(int dtype, int n, const void *J, int64_t N, void *H, void *strea
  * "Manipulator Differential Kinematics Part II"), D (N, n^(order-1), 6, n) from jacob0 J (N,6,n), order = 3..5:
  * D[a_1, ..., a_{order-1}, :, j] = d^(order-1) J[:, j] / dq_{a_1} ... dq_{a_{order-1}}, symmetric in the a's.  Order 1
  * is J itself and order 2 the Hessian of b2k_hessian.  J's columns are taken in chain order, as b2k_hessian takes
- * them.  J and D are aligned to their element size; every argument is checked before any CUDA call. */
+ * them. */
 int b2k_partial_fkine(int dtype, int n, int order, const void *J, int64_t N, void *D, void *stream);
 int b2k_manipulability(int dtype, int n, const void *J, int64_t N, uint32_t axes_mask, void *m, void *stream);
 /* The singular-value measures of ETS.manipulability (ETS.py:1789-1796) over the Cartesian rows in axes_mask:

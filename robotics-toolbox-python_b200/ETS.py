@@ -458,15 +458,8 @@ class ETS:
             raise ValueError("one of q or the Jacobian must be supplied")
         if J is None:
             J = jac(q, tool=tool, dtype=dtype)
-        host = not B.is_tensor(J)
-        dt = B.pick_dtype(J, dtype)
-        Jd = B.to_device(J, dt)
-        single = Jd.dim() == 2
-        Jd = (Jd.reshape(1, 6, -1) if single else Jd).contiguous()
-        n = self.n
-        if tuple(Jd.shape[1:]) != (6, n):
-            raise ValueError(f"the Jacobian must be (6,{n}) or (N,6,{n})")
-        N = Jd.shape[0]
+        Jd, dt, host, single = self._jprep(J, dtype)
+        N, n = Jd.shape[0], self.n
         H = B.empty((N, n, 6, n), dt, like=Jd)
         _lib.check(_lib.lib().b2k_hessian(B.code(dt), n, B.ptr(Jd), N, B.ptr(H), B.stream_ptr(Jd)))
         if host:

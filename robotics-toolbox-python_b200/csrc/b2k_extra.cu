@@ -2,6 +2,8 @@
 // manipulability, Jacobian time derivative and manipulability Jacobian.  Replaces fknm.ETS_hessian0 /
 // ETS_hessiane (reference fknm.cpp:583-783 -> _ETS_hessian methods.cpp:16-32), the yoshikawa branch of
 // ETS.manipulability (ETS.py:1780-1787), Robot.jacob0_dot (Robot.py:964-1099) and ETS.jacobm (ETS.py:1628-1685).
+#include <algorithm>
+
 #include "b2k_common.cuh"
 #include "b2k_ik.cuh" // ik_angle_axis
 
@@ -539,106 +541,133 @@ __global__ void __launch_bounds__(128) k_singular(const real *__restrict__ J, lo
     m[row] = kind == 0 ? smin : (smax > 0 ? smin / smax : (real)0);
 }
 
+// ------------------------------------------------------------------ the C ABI of the functions of J
+enum JacFunOp { HESSIAN, YOSHIKAWA, SINGULAR, JACOB_DOT, JACOBM, PARTIAL_FKINE };
+
+// One call as its entry point passes it: J (N,6,n), qd (N,n) and the output are device arrays.
+struct JacFunArgs {
+    const void *J, *qd;
+    void *out;
+    long long N;
+    unsigned axes_mask;
+    int k; // the SVD kind (0 minsingular, 1 invcondition) or the derivative order (3..5)
+};
+
 template <typename real>
-static int extra_launch(int what, int n, const void *J, long long N, unsigned axes_mask, void *out, cudaStream_t st,
-                        const void *aux = nullptr)
+int b2k_pfk_launch(int n, int order, const void *J, long long nrows, void *D, cudaStream_t st); // b2k_pfk.cu
+
+template <typename real, int N>
+static void jacfun_launch_n(JacFunOp op, const JacFunArgs &a, cudaStream_t st)
 {
-#define B2K_CASE(NN)                                                                                                  \
-    case NN:                                                                                                          \
-        if (what == 0 || what == 2) {                                                                                 \
-            long long blocks = (N + 7) / 8;                                                                           \
-            /* k_hessian: 4 resident blocks per SM (64 registers x 256 threads); one wave, so that the per-thread  */ \
-            /* index table is set up once per ~200 rows                                                             */ \
-            const long long cap = (long long)b2k_num_sms() * (what == 0 ? 4 : 16);                                    \
-            if (blocks > cap) blocks = cap;                                                                           \
-            if (what == 0 && NN >= 3 && ((uintptr_t)out & 15) == 0 &&                                                \
-                b2k_blocks_per_sm((const void *)k_hessian_tile<real, NN>, 128, HessTile<real, NN>::SMEM) >= 1)         \
-                k_hessian_tile<real, NN><<<(unsigned)((N + 31) / 32), 128, HessTile<real, NN>::SMEM, st>>>((const real *)J, N, (real *)out); \
-            else if (what == 0) k_hessian<real, NN><<<(unsigned)blocks, 256, 0, st>>>((const real *)J, N, (real *)out, (int)(((uintptr_t)out & (2 * sizeof(real) - 1)) == 0)); \
-            else k_jacob_dot_lane<real, NN><<<(unsigned)((N + B2K_XT - 1) / B2K_XT), B2K_XT, 0, st>>>((const real *)J, (const real *)aux, N, (real *)out); \
-        } else if (what == 3) {                                                                                       \
-            if (axes_mask == 63u && NN >= 6) k_jacobm_all<real, NN><<<(unsigned)((N + 127) / 128), 128, 0, st>>>((const real *)J, N, (real *)out); \
-            else k_jacobm<real, NN><<<(unsigned)((N + 127) / 128), 128, 0, st>>>((const real *)J, N, axes_mask, (real *)out); \
-        } else if (what == 4 || what == 5) {                                                                          \
-            if (axes_mask == 63u) k_singular_all<real, NN><<<(unsigned)((N + 127) / 128), 128, 0, st>>>((const real *)J, N, what - 4, (real *)out); \
-            else k_singular<real, NN><<<(unsigned)((N + 127) / 128), 128, 0, st>>>((const real *)J, N, axes_mask, what - 4, (real *)out); \
-        } else if (axes_mask == 63u && NN > 6) {                                                                      \
-            k_yoshikawa_all<real, NN><<<(unsigned)((N + B2K_XT - 1) / B2K_XT), B2K_XT, 0, st>>>((const real *)J, N, (real *)out); \
-        } else {                                                                                                      \
-            k_yoshikawa<real, NN><<<(unsigned)((N + 127) / 128), 128, 0, st>>>((const real *)J, N, axes_mask, (real *)out); \
-        }                                                                                                             \
-        break;
-    switch (n) {
-        B2K_CASE(1) B2K_CASE(2) B2K_CASE(3) B2K_CASE(4) B2K_CASE(5)
-        B2K_CASE(6) B2K_CASE(7) B2K_CASE(8) B2K_CASE(9) B2K_CASE(10)
-    default:
-        b2k_set_error("unsupported joint count %d", n);
-        return B2K_ERR_INVALID;
+    const real *J = (const real *)a.J;
+    real *out = (real *)a.out;
+    const long long rows = a.N;
+    const unsigned mask = a.axes_mask & 63u, lanes = (unsigned)((rows + 127) / 128), staged = (unsigned)((rows + B2K_XT - 1) / B2K_XT);
+    switch (op) {
+    case HESSIAN:
+        if constexpr (N >= 3)
+            if (((uintptr_t)out & 15) == 0 && b2k_blocks_per_sm((const void *)k_hessian_tile<real, N>, 128, HessTile<real, N>::SMEM) >= 1) {
+                k_hessian_tile<real, N><<<(unsigned)((rows + 31) / 32), 128, HessTile<real, N>::SMEM, st>>>(J, rows, out);
+                return;
+            }
+        // k_hessian: 4 resident blocks per SM (64 registers x 256 threads); one wave, so that the per-thread index table
+        // is set up once per ~200 rows
+        k_hessian<real, N><<<(unsigned)std::min((rows + 7) / 8, 4LL * b2k_num_sms()), 256, 0, st>>>(
+            J, rows, out, (int)(((uintptr_t)out & (2 * sizeof(real) - 1)) == 0));
+        return;
+    case YOSHIKAWA:
+        if constexpr (N > 6)
+            if (mask == 63u) { k_yoshikawa_all<real, N><<<staged, B2K_XT, 0, st>>>(J, rows, out); return; }
+        k_yoshikawa<real, N><<<lanes, 128, 0, st>>>(J, rows, mask, out);
+        return;
+    case SINGULAR:
+        if (mask == 63u) k_singular_all<real, N><<<lanes, 128, 0, st>>>(J, rows, a.k, out);
+        else k_singular<real, N><<<lanes, 128, 0, st>>>(J, rows, mask, a.k, out);
+        return;
+    case JACOB_DOT:
+        k_jacob_dot_lane<real, N><<<staged, B2K_XT, 0, st>>>(J, (const real *)a.qd, rows, out);
+        return;
+    case JACOBM:
+        if constexpr (N >= 6)
+            if (mask == 63u) { k_jacobm_all<real, N><<<lanes, 128, 0, st>>>(J, rows, out); return; }
+        k_jacobm<real, N><<<lanes, 128, 0, st>>>(J, rows, mask, out);
+        return;
+    case PARTIAL_FKINE: return; // b2k_pfk_launch
     }
-#undef B2K_CASE
+}
+
+template <typename real>
+static int jacfun_launch(JacFunOp op, int n, const JacFunArgs &a, cudaStream_t st)
+{
+    if (op == PARTIAL_FKINE) return b2k_pfk_launch<real>(n, a.k, a.J, a.N, a.out, st);
+    switch (n) {
+    case 1: jacfun_launch_n<real, 1>(op, a, st); break;
+    case 2: jacfun_launch_n<real, 2>(op, a, st); break;
+    case 3: jacfun_launch_n<real, 3>(op, a, st); break;
+    case 4: jacfun_launch_n<real, 4>(op, a, st); break;
+    case 5: jacfun_launch_n<real, 5>(op, a, st); break;
+    case 6: jacfun_launch_n<real, 6>(op, a, st); break;
+    case 7: jacfun_launch_n<real, 7>(op, a, st); break;
+    case 8: jacfun_launch_n<real, 8>(op, a, st); break;
+    case 9: jacfun_launch_n<real, 9>(op, a, st); break;
+    case 10: jacfun_launch_n<real, 10>(op, a, st); break;
+    default: b2k_set_error("unsupported joint count %d", n); return B2K_ERR_INVALID;
+    }
     b2k_count_launch();
     B2K_CUDA(cudaGetLastError());
     return B2K_OK;
 }
 
+// Every argument of the six entry points is checked before any CUDA call, in one order.  N = 0 needs no arrays (NULL is
+// accepted) and touches no device.
+static int jacfun_dispatch(const char *fn, JacFunOp op, int dtype, int n, const JacFunArgs &a, void *stream)
+{
+    if (dtype != B2K_F32 && dtype != B2K_F64) { b2k_set_error("%s: dtype must be B2K_F32 or B2K_F64", fn); return B2K_ERR_INVALID; }
+    if (n < 1 || n > B2K_MAX_JOINTS) { b2k_set_error("%s: unsupported joint count %d (1..%d)", fn, n, B2K_MAX_JOINTS); return B2K_ERR_INVALID; }
+    if (a.N < 0) { b2k_set_error("%s: N is negative", fn); return B2K_ERR_INVALID; }
+    if (op == SINGULAR && a.k != 0 && a.k != 1) { b2k_set_error("%s: kind must be 0 (minsingular) or 1 (invcondition), not %d", fn, a.k); return B2K_ERR_INVALID; }
+    if (op == PARTIAL_FKINE && (a.k < 3 || a.k > 5)) { b2k_set_error("%s: unsupported order %d (3..5)", fn, a.k); return B2K_ERR_INVALID; }
+    if ((op == YOSHIKAWA || op == SINGULAR || op == JACOBM) && (a.axes_mask & 63u) == 0) { b2k_set_error("%s: no Cartesian axis selected", fn); return B2K_ERR_INVALID; }
+    static const char *const out_name[] = {"H", "m", "m", "Jd", "Jm", "D"};
+    const struct { const void *p; const char *name; bool read; } arrays[] = {{a.J, "J", true}, {a.qd, "qd", op == JACOB_DOT}, {a.out, out_name[op], true}};
+    for (const auto &x : arrays)
+        if (x.read && a.N > 0 && !x.p) { b2k_set_error("%s: %s is NULL", fn, x.name); return B2K_ERR_INVALID; }
+    const unsigned es = dtype == B2K_F64 ? 8u : 4u;
+    for (const auto &x : arrays)
+        if (x.read && ((uintptr_t)x.p & (es - 1))) { b2k_set_error("%s: %s is not aligned to its element size (%u bytes)", fn, x.name, es); return B2K_ERR_INVALID; }
+    if (a.N == 0) return B2K_OK;
+    B2K_ON_DEVICE_OF(a.J);
+    return dtype == B2K_F64 ? jacfun_launch<double>(op, n, a, (cudaStream_t)stream) : jacfun_launch<float>(op, n, a, (cudaStream_t)stream);
+}
+
 extern "C" int b2k_hessian(int dtype, int n, const void *J, int64_t N, void *H, void *stream)
 {
-    if (N < 0 || (N > 0 && (!J || !H))) { b2k_set_error("b2k_hessian: bad arguments"); return B2K_ERR_INVALID; }
-    if (dtype != B2K_F32 && dtype != B2K_F64) { b2k_set_error("b2k_hessian: bad dtype"); return B2K_ERR_INVALID; }
-    if (n < 1 || n > B2K_MAX_JOINTS) { b2k_set_error("b2k_hessian: unsupported joint count %d", n); return B2K_ERR_INVALID; }
-    if (N == 0) return B2K_OK;
-    B2K_ON_DEVICE_OF(J);
-    return dtype == B2K_F64 ? extra_launch<double>(0, n, J, N, 0, H, (cudaStream_t)stream)
-                            : extra_launch<float>(0, n, J, N, 0, H, (cudaStream_t)stream);
+    return jacfun_dispatch("b2k_hessian", HESSIAN, dtype, n, {J, nullptr, H, N, 0u, 0}, stream);
+}
+
+extern "C" int b2k_partial_fkine(int dtype, int n, int order, const void *J, int64_t N, void *D, void *stream)
+{
+    return jacfun_dispatch("b2k_partial_fkine", PARTIAL_FKINE, dtype, n, {J, nullptr, D, N, 0u, order}, stream);
 }
 
 extern "C" int b2k_manipulability(int dtype, int n, const void *J, int64_t N, uint32_t axes_mask, void *m, void *stream)
 {
-    if (N < 0 || (N > 0 && (!J || !m))) { b2k_set_error("b2k_manipulability: bad arguments"); return B2K_ERR_INVALID; }
-    if (dtype != B2K_F32 && dtype != B2K_F64) { b2k_set_error("b2k_manipulability: bad dtype"); return B2K_ERR_INVALID; }
-    if (n < 1 || n > B2K_MAX_JOINTS) { b2k_set_error("b2k_manipulability: unsupported joint count %d", n); return B2K_ERR_INVALID; }
-    if ((axes_mask & 63u) == 0) { b2k_set_error("b2k_manipulability: no Cartesian axis selected"); return B2K_ERR_INVALID; }
-    if (N == 0) return B2K_OK;
-    B2K_ON_DEVICE_OF(J);
-    return dtype == B2K_F64 ? extra_launch<double>(1, n, J, N, axes_mask & 63u, m, (cudaStream_t)stream)
-                            : extra_launch<float>(1, n, J, N, axes_mask & 63u, m, (cudaStream_t)stream);
+    return jacfun_dispatch("b2k_manipulability", YOSHIKAWA, dtype, n, {J, nullptr, m, N, axes_mask, 0}, stream);
 }
-
 
 extern "C" int b2k_manipulability_svd(int dtype, int n, const void *J, int64_t N, uint32_t axes_mask, int kind, void *m, void *stream)
 {
-    if (N < 0 || (N > 0 && (!J || !m))) { b2k_set_error("b2k_manipulability_svd: bad arguments"); return B2K_ERR_INVALID; }
-    if (dtype != B2K_F32 && dtype != B2K_F64) { b2k_set_error("b2k_manipulability_svd: bad dtype"); return B2K_ERR_INVALID; }
-    if (n < 1 || n > B2K_MAX_JOINTS) { b2k_set_error("b2k_manipulability_svd: unsupported joint count %d", n); return B2K_ERR_INVALID; }
-    if ((axes_mask & 63u) == 0) { b2k_set_error("b2k_manipulability_svd: no Cartesian axis selected"); return B2K_ERR_INVALID; }
-    if (kind != 0 && kind != 1) { b2k_set_error("b2k_manipulability_svd: kind must be 0 (minsingular) or 1 (invcondition)"); return B2K_ERR_INVALID; }
-    if (N == 0) return B2K_OK;
-    B2K_ON_DEVICE_OF(J);
-    return dtype == B2K_F64 ? extra_launch<double>(4 + kind, n, J, N, axes_mask & 63u, m, (cudaStream_t)stream)
-                            : extra_launch<float>(4 + kind, n, J, N, axes_mask & 63u, m, (cudaStream_t)stream);
+    return jacfun_dispatch("b2k_manipulability_svd", SINGULAR, dtype, n, {J, nullptr, m, N, axes_mask, kind}, stream);
 }
 
 extern "C" int b2k_jacob_dot(int dtype, int n, const void *J, const void *qd, int64_t N, void *Jd, void *stream)
 {
-    if (N < 0 || (N > 0 && (!J || !qd || !Jd))) { b2k_set_error("b2k_jacob_dot: bad arguments"); return B2K_ERR_INVALID; }
-    if (dtype != B2K_F32 && dtype != B2K_F64) { b2k_set_error("b2k_jacob_dot: bad dtype"); return B2K_ERR_INVALID; }
-    if (n < 1 || n > B2K_MAX_JOINTS) { b2k_set_error("b2k_jacob_dot: unsupported joint count %d", n); return B2K_ERR_INVALID; }
-    if (N == 0) return B2K_OK;
-    B2K_ON_DEVICE_OF(J);
-    return dtype == B2K_F64 ? extra_launch<double>(2, n, J, N, 0, Jd, (cudaStream_t)stream, qd)
-                            : extra_launch<float>(2, n, J, N, 0, Jd, (cudaStream_t)stream, qd);
+    return jacfun_dispatch("b2k_jacob_dot", JACOB_DOT, dtype, n, {J, qd, Jd, N, 0u, 0}, stream);
 }
 
 extern "C" int b2k_jacobm(int dtype, int n, const void *J, int64_t N, uint32_t axes_mask, void *Jm, void *stream)
 {
-    if (N < 0 || (N > 0 && (!J || !Jm))) { b2k_set_error("b2k_jacobm: bad arguments"); return B2K_ERR_INVALID; }
-    if (dtype != B2K_F32 && dtype != B2K_F64) { b2k_set_error("b2k_jacobm: bad dtype"); return B2K_ERR_INVALID; }
-    if (n < 1 || n > B2K_MAX_JOINTS) { b2k_set_error("b2k_jacobm: unsupported joint count %d", n); return B2K_ERR_INVALID; }
-    if ((axes_mask & 63u) == 0) { b2k_set_error("b2k_jacobm: no Cartesian axis selected"); return B2K_ERR_INVALID; }
-    if (N == 0) return B2K_OK;
-    B2K_ON_DEVICE_OF(J);
-    return dtype == B2K_F64 ? extra_launch<double>(3, n, J, N, axes_mask & 63u, Jm, (cudaStream_t)stream)
-                            : extra_launch<float>(3, n, J, N, axes_mask & 63u, Jm, (cudaStream_t)stream);
+    return jacfun_dispatch("b2k_jacobm", JACOBM, dtype, n, {J, nullptr, Jm, N, axes_mask, 0}, stream);
 }
 
 

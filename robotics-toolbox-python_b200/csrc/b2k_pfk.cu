@@ -215,8 +215,11 @@ int pfk_order(int order, const void *J, long long nrows, void *D, cudaStream_t s
     }
 }
 
+} // namespace
+
+// The launcher of b2k_partial_fkine; jacfun_dispatch (b2k_extra.cu) has checked its arguments
 template <typename real>
-int pfk_dispatch(int n, int order, const void *J, long long nrows, void *D, cudaStream_t st)
+int b2k_pfk_launch(int n, int order, const void *J, long long nrows, void *D, cudaStream_t st)
 {
     switch (n) {
     case 1: return pfk_order<real, 1>(order, J, nrows, D, st);
@@ -228,25 +231,10 @@ int pfk_dispatch(int n, int order, const void *J, long long nrows, void *D, cuda
     case 7: return pfk_order<real, 7>(order, J, nrows, D, st);
     case 8: return pfk_order<real, 8>(order, J, nrows, D, st);
     case 9: return pfk_order<real, 9>(order, J, nrows, D, st);
-    default: return pfk_order<real, 10>(order, J, nrows, D, st);
+    case 10: return pfk_order<real, 10>(order, J, nrows, D, st);
     }
+    b2k_set_error("b2k_partial_fkine: unsupported joint count %d", n);
+    return B2K_ERR_INVALID;
 }
-
-bool misaligned(const void *p, unsigned bytes) { return ((uintptr_t)p & (bytes - 1)) != 0; }
-
-} // namespace
-
-extern "C" int b2k_partial_fkine(int dtype, int n, int order, const void *J, int64_t N, void *D, void *stream)
-{
-    const char *fn = "b2k_partial_fkine";
-    if (dtype != B2K_F32 && dtype != B2K_F64) { b2k_set_error("%s: bad dtype", fn); return B2K_ERR_INVALID; }
-    if (n < 1 || n > B2K_MAX_JOINTS) { b2k_set_error("%s: unsupported joint count %d", fn, n); return B2K_ERR_INVALID; }
-    if (order < 3 || order > 5) { b2k_set_error("%s: unsupported order %d (3..5)", fn, order); return B2K_ERR_INVALID; }
-    if (N < 0 || (N > 0 && (!J || !D))) { b2k_set_error("%s: bad arguments", fn); return B2K_ERR_INVALID; }
-    const unsigned es = dtype == B2K_F64 ? 8u : 4u;
-    if (misaligned(J, es) || misaligned(D, es)) { b2k_set_error("%s: J or D is not aligned to its element size", fn); return B2K_ERR_INVALID; }
-    if (N == 0) return B2K_OK;
-    B2K_ON_DEVICE_OF(J);
-    return dtype == B2K_F64 ? pfk_dispatch<double>(n, order, J, N, D, (cudaStream_t)stream)
-                            : pfk_dispatch<float>(n, order, J, N, D, (cudaStream_t)stream);
-}
+template int b2k_pfk_launch<float>(int, int, const void *, long long, void *, cudaStream_t);
+template int b2k_pfk_launch<double>(int, int, const void *, long long, void *, cudaStream_t);

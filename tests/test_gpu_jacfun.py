@@ -1,5 +1,5 @@
 """The kernels of b2k_extra.cu that consume a Jacobian -- Yoshikawa manipulability, the singular-value measures,
-jacobm and jacob0_dot -- at every joint count, axis selection and dtype, so that every kernel extra_launch selects is
+jacobm and jacob0_dot -- at every joint count, axis selection and dtype, so that every kernel jacfun_launch selects is
 reached (the Hessian has its own exhaustive test in test_gpu_widened_r2.py).
 
 Most checks call the C ABI directly and compare with the batched float64 restatement in jacfun_ref.py; fp32 runs
