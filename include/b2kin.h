@@ -456,7 +456,10 @@ int b2k_manipulability_svd(int dtype, int n, const void *J, int64_t N, uint32_t 
 int b2k_jacob_dot(int dtype, int n, const void *J, const void *qd, int64_t N, void *Jd, void *stream);
 int b2k_jacobm(int dtype, int n, const void *J, int64_t N, uint32_t axes_mask, void *Jm, void *stream);
 
-/* ---------------------------------------------------------------- pose error, position-based servo
+/* ---------------------------------------------------------------- pose error, position-based servo, trajectories
+ * The eight functions below check every argument before any CUDA call.  Their device arrays must be aligned to their
+ * element size (arrived: 4 bytes).  N = 0 needs no device arrays (NULL is accepted) and touches no device; an array
+ * documented as optional may be NULL at any N.  Host tables that are not optional must not be NULL, whatever N is.
  * b2k_angle_axis replaces fknm.Angle_Axis (fknm.cpp:112-162 -> _angle_axis ik.cpp:241-286), batched:
  * e (N,6) = [translation error; angle-axis rotation error] between Te (N,4,4) and Tep.
  * tep_stride = 16: one target per row, Tep (N,4,4); tep_stride = 0: a single (4,4) target for every row.
@@ -477,8 +480,7 @@ int b2k_p_servo_rpy(int dtype, const void *Te, const void *Tep, int64_t N, int64
 int b2k_jacob0_analytical(int dtype, int n, const void *T, const void *J, int64_t N, int representation, void *Ja,
                           void *stream);
 
-/* ---------------------------------------------------------------- trajectory producer
- * b2k_jtraj replaces tools.trajectory.jtraj (tools/trajectory.py:686-780): quintic joint-space blend
+/* b2k_jtraj replaces tools.trajectory.jtraj (tools/trajectory.py:686-780): quintic joint-space blend
  * from q0 to qf (host n-vectors; qd0 / qd1 boundary velocities or NULL = 0) sampled at N points,
  * written straight into device buffers q, qd, qdd (N,n) (qd / qdd may be NULL) so the batch can feed
  * b2k_fkine / b2k_rne without touching the host.

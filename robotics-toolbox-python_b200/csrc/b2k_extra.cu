@@ -1,11 +1,12 @@
-// b2k_extra.cu -- pure functions of the Jacobian (SURVEY 8f-2): manipulator Hessian, Yoshikawa
-// manipulability, Jacobian time derivative and manipulability Jacobian.  Replaces fknm.ETS_hessian0 /
-// ETS_hessiane (reference fknm.cpp:583-783 -> _ETS_hessian methods.cpp:16-32), the yoshikawa branch of
-// ETS.manipulability (ETS.py:1780-1787), Robot.jacob0_dot (Robot.py:964-1099) and ETS.jacobm (ETS.py:1628-1685).
+// b2k_extra.cu -- pure functions of the Jacobian (SURVEY 8f-2): manipulator Hessian, Yoshikawa and singular-value
+// manipulability, Jacobian time derivative and manipulability Jacobian, and the C ABI of these six functions with
+// partial_fkine (whose kernels are in b2k_pfk.cu).  Replaces fknm.ETS_hessian0 / ETS_hessiane (reference
+// fknm.cpp:583-783 -> _ETS_hessian methods.cpp:16-32), ETS.manipulability (ETS.py:1780-1796), Robot.jacob0_dot
+// (Robot.py:964-1099) and ETS.jacobm (ETS.py:1628-1685).
 #include <algorithm>
 
 #include "b2k_common.cuh"
-#include "b2k_ik.cuh" // ik_angle_axis
+#include "b2k_ik.cuh" // ik_chol_factor / ik_chol_subst, b2k_gram_chol6, b2k_hess_term
 
 // H[a, 0:3, b] = Jw_a x Jv_b, H[a, 3:6, b] = Jw_a x Jw_b for b >= a; mirrored translational block and a zero
 // rotational block for b < a (methods.cpp:18-31).  A store stream: 6 n^2 outputs per row against 6 n inputs.
@@ -668,264 +669,4 @@ extern "C" int b2k_jacob_dot(int dtype, int n, const void *J, const void *qd, in
 extern "C" int b2k_jacobm(int dtype, int n, const void *J, int64_t N, uint32_t axes_mask, void *Jm, void *stream)
 {
     return jacfun_dispatch("b2k_jacobm", JACOBM, dtype, n, {J, nullptr, Jm, N, axes_mask, 0}, stream);
-}
-
-
-// ------------------------------------------------------------------ joint-space trajectory producer (SURVEY 8f-3)
-// jtraj (reference tools/trajectory.py:686-780): quintic blend q0 -> qf with boundary velocities qd0, qd1:
-//   q(s) = A s^5 + B s^4 + C s^3 + E s + F,  qd = (5A s^4 + 4B s^3 + 3C s^2 + E) / tscal,
-//   qdd = (20A s^3 + 12B s^2 + 6C s) / tscal^2,  s = t / tscal in [0, 1].
-// Rows are time samples; one thread per (row, joint) element so the three (N,n) outputs are written coalesced and a
-// q batch is produced where the FK / RNE kernels consume it, without a host round trip.
-struct JtrajP {
-    double A[B2K_MAX_JOINTS], B[B2K_MAX_JOINTS], C[B2K_MAX_JOINTS], E[B2K_MAX_JOINTS], F[B2K_MAX_JOINTS];
-    double inv_tscal, inv_nm1;
-    int n;
-};
-
-template <typename real>
-__global__ void __launch_bounds__(256) k_jtraj(const __grid_constant__ JtrajP P, const real *__restrict__ ts, long long nrows,
-                                               real *__restrict__ q, real *__restrict__ qd, real *__restrict__ qdd)
-{
-    const long long total = nrows * P.n;
-    for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.x * blockDim.x) {
-        long long row; int j;
-        split_elem(e, P.n, total, row, j);
-        // normalised time: the caller's samples, or np.linspace(0, 1, N)[row] (last sample exactly 1)
-        const real s = ts ? ts[row] * (real)P.inv_tscal
-                          : (row == nrows - 1 ? (real)1 : (real)((double)row * P.inv_nm1));
-        const real A = (real)P.A[j], B = (real)P.B[j], C = (real)P.C[j], E = (real)P.E[j], F = (real)P.F[j];
-        const real it = (real)P.inv_tscal;
-        q[e] = fma(fma(fma(fma(A, s, B), s, C) * s, s, E), s, F);
-        if (qd) qd[e] = fma(fma(fma((real)5 * A, s, (real)4 * B), s, (real)3 * C) * s, s, E) * it;
-        if (qdd) qdd[e] = fma(fma((real)20 * A, s, (real)12 * B), s, (real)6 * C) * s * it * it;
-    }
-}
-
-extern "C" int b2k_jtraj(int dtype, int n, const double *q0, const double *qf, const double *qd0, const double *qd1,
-                         int64_t N, const void *t, double tscal, void *q, void *qd, void *qdd, void *stream)
-{
-    const char *fn = "b2k_jtraj";
-    if (n < 1 || n > B2K_MAX_JOINTS) { b2k_set_error("%s: n must be 1..%d", fn, B2K_MAX_JOINTS); return B2K_ERR_INVALID; }
-    if (dtype != B2K_F32 && dtype != B2K_F64) { b2k_set_error("%s: bad dtype", fn); return B2K_ERR_INVALID; }
-    if (!q0 || !qf) { b2k_set_error("%s: q0 / qf is NULL", fn); return B2K_ERR_INVALID; }
-    if (N < 0 || (N > 0 && !q)) { b2k_set_error("%s: bad N / q", fn); return B2K_ERR_INVALID; }
-    if (!(tscal > 0)) { b2k_set_error("%s: tscal must be positive", fn); return B2K_ERR_INVALID; }
-    if (N == 0) return B2K_OK;
-    B2K_ON_DEVICE_OF(q);
-    JtrajP P;
-    P.n = n;
-    P.inv_tscal = 1.0 / tscal;
-    P.inv_nm1 = N > 1 ? 1.0 / (double)(N - 1) : 0.0;
-    for (int j = 0; j < n; j++) { // trajectory.py:753-757
-        const double d = qf[j] - q0[j], v0 = qd0 ? qd0[j] : 0.0, v1 = qd1 ? qd1[j] : 0.0;
-        P.A[j] = 6 * d - 3 * (v1 + v0) * tscal;
-        P.B[j] = -15 * d + (8 * v0 + 7 * v1) * tscal;
-        P.C[j] = 10 * d - (6 * v0 + 4 * v1) * tscal;
-        P.E[j] = v0 * tscal;
-        P.F[j] = q0[j];
-    }
-    const long long total = N * n;
-    long long blocks = (total + 255) / 256;
-    const long long cap = (long long)b2k_num_sms() * 16;
-    if (blocks > cap) blocks = cap;
-    cudaStream_t st = (cudaStream_t)stream;
-    if (dtype == B2K_F64)
-        k_jtraj<double><<<(unsigned)blocks, 256, 0, st>>>(P, (const double *)t, N, (double *)q, (double *)qd, (double *)qdd);
-    else
-        k_jtraj<float><<<(unsigned)blocks, 256, 0, st>>>(P, (const float *)t, N, (float *)q, (float *)qd, (float *)qdd);
-    b2k_count_launch();
-    B2K_CUDA(cudaGetLastError());
-    return B2K_OK;
-}
-
-
-// ------------------------------------------------------------------ pose error / position-based servo
-// Batched fknm.Angle_Axis (fknm.cpp:112-162 -> _angle_axis ik.cpp:241-286) and tools/p_servo.py:46-106 with
-// method="angle-axis": e = angle_axis(Te, Tep), v = gain .* e, arrived = sum|e| < threshold.
-// Lane per row; tep_stride = 0 broadcasts one target to every row.
-template <typename real, bool VEC>
-__global__ void __launch_bounds__(256) k_pose_error(const real *__restrict__ Te, const real *__restrict__ Tep,
-                                                    long long tep_stride, long long nrows, real g0, real g1, real g2,
-                                                    real g3, real g4, real g5, real threshold, real *__restrict__ out,
-                                                    int *__restrict__ arrived)
-{
-    const long long row = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (row >= nrows) return;
-    // the three used rows of each 4x4 matrix as 16-byte vector loads where both arrays are 16-byte aligned (the launcher
-    // looks; any torch allocation is): a third of the load instructions of the scalar form
-    real ar[12], Tp[12], e[6];
-    if (VEC) {
-        load12<real>(Te + row * 16, ar);
-        load12<real>(Tep + row * tep_stride, Tp);
-    } else {
-#pragma unroll
-        for (int k = 0; k < 12; k++) { ar[k] = Te[row * 16 + k]; Tp[k] = Tep[row * tep_stride + k]; }
-    }
-    Pose<real> T;
-    pose_from_const<real>(T, ar);
-    ik_angle_axis<real>(T, Tp, e);
-    const real g[6] = {g0, g1, g2, g3, g4, g5};
-    real sum = 0;
-#pragma unroll
-    for (int k = 0; k < 6; k++) {
-        sum += fabs(e[k]);
-        out[row * 6 + k] = g[k] * e[k];
-    }
-    if (arrived) arrived[row] = sum < threshold ? 1 : 0;
-}
-
-static int pose_error_launch(const char *fn, int dtype, const void *Te, const void *Tep, int64_t N, int64_t tep_stride,
-                             const double *gain, double threshold, void *out, int32_t *arrived, void *stream)
-{
-    if (dtype != B2K_F32 && dtype != B2K_F64) { b2k_set_error("%s: bad dtype", fn); return B2K_ERR_INVALID; }
-    if (N < 0 || (N > 0 && (!Te || !Tep || !out))) { b2k_set_error("%s: bad arguments", fn); return B2K_ERR_INVALID; }
-    if (tep_stride != 0 && tep_stride != 16) { b2k_set_error("%s: tep_stride must be 0 (one target) or 16", fn); return B2K_ERR_INVALID; }
-    if (N == 0) return B2K_OK;
-    B2K_ON_DEVICE_OF(Te);
-    double g[6];
-    for (int k = 0; k < 6; k++) g[k] = gain ? gain[k] : 1.0;
-    cudaStream_t st = (cudaStream_t)stream;
-    const unsigned blocks = (unsigned)((N + 255) / 256);
-    const bool vec = (((uintptr_t)Te | (uintptr_t)Tep) & 15) == 0;
-#define B2K_PE(REAL, V)                                                                                                        \
-    k_pose_error<REAL, V><<<blocks, 256, 0, st>>>((const REAL *)Te, (const REAL *)Tep, tep_stride, N, (REAL)g[0], (REAL)g[1], \
-                                                  (REAL)g[2], (REAL)g[3], (REAL)g[4], (REAL)g[5], (REAL)threshold, (REAL *)out, arrived)
-    if (dtype == B2K_F64) { if (vec) B2K_PE(double, true); else B2K_PE(double, false); }
-    else { if (vec) B2K_PE(float, true); else B2K_PE(float, false); }
-#undef B2K_PE
-    b2k_count_launch();
-    B2K_CUDA(cudaGetLastError());
-    return B2K_OK;
-}
-
-extern "C" int b2k_angle_axis(int dtype, const void *Te, const void *Tep, int64_t N, int64_t tep_stride, void *e, void *stream)
-{
-    return pose_error_launch("b2k_angle_axis", dtype, Te, Tep, N, tep_stride, nullptr, 0.0, e, nullptr, stream);
-}
-
-extern "C" int b2k_p_servo(int dtype, const void *Te, const void *Tep, int64_t N, int64_t tep_stride, const double *gain,
-                           double threshold, void *v, int32_t *arrived, void *stream)
-{
-    if (N > 0 && !arrived) { b2k_set_error("b2k_p_servo: arrived is NULL"); return B2K_ERR_INVALID; }
-    return pose_error_launch("b2k_p_servo", dtype, Te, Tep, N, tep_stride, gain, threshold, v, arrived, stream);
-}
-
-// ------------------------------------------------------------------ scalar / multi-axis trajectory profiles (SURVEY 8f-3)
-// quintic (tools/trajectory.py:271-416), trapezoidal (429-615) and their multi-axis form mtraj (617-684): every axis
-// follows the same kind of profile between its own end points.  The per-axis parameters are worked out on the host in
-// fp64 (quintic: the 6x6 boundary-condition system of quintic_func; trapezoidal: V, blend time tb and acceleration a of
-// trapezoidal_func); one thread per (sample, axis) element evaluates position, velocity and acceleration.
-struct MtrajP {
-    double c[B2K_MAX_JOINTS][6]; // quintic: polynomial coefficients, highest power first; trapezoidal: q0, qf, V, tb, a, T
-    int n, kind;
-};
-
-template <typename real>
-__global__ void __launch_bounds__(256) k_mtraj(const __grid_constant__ MtrajP P, const real *__restrict__ t, long long nrows,
-                                               real *__restrict__ s, real *__restrict__ sd, real *__restrict__ sdd)
-{
-    const long long total = nrows * P.n;
-    for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.x * blockDim.x) {
-        long long row; int j;
-        split_elem(e, P.n, total, row, j);
-        const real tk = t ? t[row] : (real)row; // `t: int` means t = arange(0, t) (trajectory.py:330, 489)
-        real p, pd, pdd;
-        if (P.kind == 0) { // np.polyval of coeffs, coeffs_d, coeffs_dd (trajectory.py:405-415)
-            const real c5 = (real)P.c[j][0], c4 = (real)P.c[j][1], c3 = (real)P.c[j][2], c2 = (real)P.c[j][3],
-                       c1 = (real)P.c[j][4], c0 = (real)P.c[j][5];
-            p = fma(fma(fma(fma(fma(c5, tk, c4), tk, c3), tk, c2), tk, c1), tk, c0);
-            pd = fma(fma(fma(fma((real)5 * c5, tk, (real)4 * c4), tk, (real)3 * c3), tk, (real)2 * c2), tk, c1);
-            pdd = fma(fma(fma((real)20 * c5, tk, (real)12 * c4), tk, (real)6 * c3), tk, (real)2 * c2);
-        } else { // trapezoidalfunc (trajectory.py:566-600)
-            const real q0 = (real)P.c[j][0], qf = (real)P.c[j][1], V = (real)P.c[j][2], tb = (real)P.c[j][3],
-                       a = (real)P.c[j][4], T = (real)P.c[j][5];
-            if (tk < 0) { p = q0; pd = 0; pdd = 0; }
-            else if (tk <= tb) { p = q0 + a / 2 * tk * tk; pd = a * tk; pdd = a; }
-            else if (tk <= T - tb) { p = (qf + q0 - V * T) / 2 + V * tk; pd = V; pdd = 0; }
-            else if (tk <= T) { p = qf - a / 2 * T * T + a * T * tk - a / 2 * tk * tk; pd = a * T - a * tk; pdd = -a; }
-            else { p = qf; pd = 0; pdd = 0; }
-        }
-        s[e] = p;
-        if (sd) sd[e] = pd;
-        if (sdd) sdd[e] = pdd;
-    }
-}
-
-// solve the 6x6 system of quintic_func (Gaussian elimination with partial pivoting, fp64)
-static bool quintic_coeffs(double q0, double qf, double T, double v0, double vf, double *c)
-{
-    const double T2 = T * T, T3 = T2 * T, T4 = T3 * T, T5 = T4 * T;
-    double X[6][7] = {{0, 0, 0, 0, 0, 1, q0},          {T5, T4, T3, T2, T, 1, qf},         {0, 0, 0, 0, 1, 0, v0},
-                      {5 * T4, 4 * T3, 3 * T2, 2 * T, 1, 0, vf}, {0, 0, 0, 2, 0, 0, 0}, {20 * T3, 12 * T2, 6 * T, 2, 0, 0, 0}};
-    for (int k = 0; k < 6; k++) {
-        int p = k;
-        for (int i = k + 1; i < 6; i++)
-            if (fabs(X[i][k]) > fabs(X[p][k])) p = i;
-        if (X[p][k] == 0.0) return false;
-        if (p != k)
-            for (int j = 0; j < 7; j++) { double tmp = X[k][j]; X[k][j] = X[p][j]; X[p][j] = tmp; }
-        for (int i = k + 1; i < 6; i++) {
-            const double f = X[i][k] / X[k][k];
-            for (int j = k; j < 7; j++) X[i][j] -= f * X[k][j];
-        }
-    }
-    for (int i = 5; i >= 0; i--) {
-        double acc = X[i][6];
-        for (int j = i + 1; j < 6; j++) acc -= X[i][j] * c[j];
-        c[i] = acc / X[i][i];
-    }
-    return true;
-}
-
-extern "C" int b2k_mtraj(int dtype, int kind, int n, const double *q0, const double *qf, const double *qd0, const double *qdf,
-                         const double *V, int64_t N, const void *t, double tf, void *s, void *sd, void *sdd, double *tblend,
-                         void *stream)
-{
-    const char *fn = "b2k_mtraj";
-    if (n < 1 || n > B2K_MAX_JOINTS) { b2k_set_error("%s: n must be 1..%d", fn, B2K_MAX_JOINTS); return B2K_ERR_INVALID; }
-    if (dtype != B2K_F32 && dtype != B2K_F64) { b2k_set_error("%s: bad dtype", fn); return B2K_ERR_INVALID; }
-    if (kind != 0 && kind != 1) { b2k_set_error("%s: kind must be 0 (quintic) or 1 (trapezoidal)", fn); return B2K_ERR_INVALID; }
-    if (!q0 || !qf) { b2k_set_error("%s: q0 / qf is NULL", fn); return B2K_ERR_INVALID; }
-    if (N < 0 || (N > 0 && !s)) { b2k_set_error("%s: bad N / output", fn); return B2K_ERR_INVALID; }
-    if (!(tf > 0)) { b2k_set_error("%s: the final time must be positive (at least two samples)", fn); return B2K_ERR_INVALID; }
-    MtrajP P;
-    P.n = n;
-    P.kind = kind;
-    for (int j = 0; j < n; j++) {
-        if (kind == 0) {
-            if (!quintic_coeffs(q0[j], qf[j], tf, qd0 ? qd0[j] : 0.0, qdf ? qdf[j] : 0.0, P.c[j])) {
-                b2k_set_error("%s: singular boundary-condition system", fn);
-                return B2K_ERR_INVALID;
-            }
-        } else { // trapezoidal_func, trajectory.py:552-565
-            double v;
-            if (!V || V[j] != V[j]) v = (qf[j] - q0[j]) / tf * 1.5; // NaN = not given
-            else {
-                const double d = qf[j] - q0[j];
-                v = fabs(V[j]) * (d > 0 ? 1.0 : (d < 0 ? -1.0 : 0.0));
-                if (fabs(v) < fabs(d) / tf) { b2k_set_error("V too small"); return B2K_ERR_INVALID; }
-                if (fabs(v) > 2 * fabs(d) / tf) { b2k_set_error("V too big"); return B2K_ERR_INVALID; }
-            }
-            double tb, a;
-            if (v == 0) { tb = INFINITY; a = 0; }
-            else { tb = (q0[j] - qf[j] + v * tf) / v; a = v / tb; }
-            P.c[j][0] = q0[j]; P.c[j][1] = qf[j]; P.c[j][2] = v; P.c[j][3] = tb; P.c[j][4] = a; P.c[j][5] = tf;
-            if (tblend) tblend[j] = tb;
-        }
-    }
-    if (N == 0) return B2K_OK;
-    B2K_ON_DEVICE_OF(s);
-    const long long total = N * n;
-    long long blocks = (total + 255) / 256;
-    const long long cap = (long long)b2k_num_sms() * 16;
-    if (blocks > cap) blocks = cap;
-    cudaStream_t st = (cudaStream_t)stream;
-    if (dtype == B2K_F64)
-        k_mtraj<double><<<(unsigned)blocks, 256, 0, st>>>(P, (const double *)t, N, (double *)s, (double *)sd, (double *)sdd);
-    else
-        k_mtraj<float><<<(unsigned)blocks, 256, 0, st>>>(P, (const float *)t, N, (float *)s, (float *)sd, (float *)sdd);
-    b2k_count_launch();
-    B2K_CUDA(cudaGetLastError());
-    return B2K_OK;
 }

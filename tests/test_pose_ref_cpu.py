@@ -2,6 +2,7 @@
 the kernels of b2k_pose.cu and the angle-axis error against -- agrees with the oracle's float64 restatements at generic
 rows and satisfies the defining identities in mpmath; and the C entry points of those kernels reject bad arguments with
 B2K_ERR_INVALID before any CUDA call."""
+import ctypes as C
 import os
 import sys
 
@@ -174,3 +175,134 @@ def test_ctraj_rejects_bad_rows_or_pointers(args):
     T = np.eye(4)
     dp = rtb._lib.dptr
     _launches_nothing(lambda lib: lib.b2k_ctraj(1, dp(T), dp(T), s, N, out, None), b"bad arguments")
+
+
+# ---- the eight pose-error and trajectory entry points on one table of bad arguments.  Each call has valid arguments
+# except the ones a case names; a host buffer stands in for the (never dereferenced) device arrays.  Without a device, a
+# call that reached the CUDA runtime would report a CUDA error instead.
+POSE_SIG = {"b2k_angle_axis": "dtype Te Tep N tep_stride e",
+            "b2k_p_servo": "dtype Te Tep N tep_stride gain threshold v arrived",
+            "b2k_p_servo_rpy": "dtype Te Tep N tep_stride gain threshold v arrived",
+            "b2k_jacob0_analytical": "dtype n T J N representation Ja",
+            "b2k_jtraj": "dtype n q0 qf qd0 qd1 N t tscal q qd qdd",
+            "b2k_mtraj": "dtype kind n q0 qf qd0 qdf V N t tf s sd sdd tblend",
+            "b2k_ctraj": "dtype T0 T1 s N T",
+            "b2k_mstraj": "dtype n npieces row0 rows kind tscal t0 dt coef N q"}
+# the device arrays in the order they are checked, and the required ones; the host tables that must not be NULL; the
+# entry point's own scalars as (name, bad value, good value); nmax: the joint-count range, None: no joint count
+POSE_DEV = {"b2k_angle_axis": "Te Tep e", "b2k_p_servo": "Te Tep v arrived", "b2k_p_servo_rpy": "Te Tep v arrived",
+            "b2k_jacob0_analytical": "T J Ja", "b2k_jtraj": "t q qd qdd", "b2k_mtraj": "t s sd sdd", "b2k_ctraj": "s T",
+            "b2k_mstraj": "q"}
+POSE_OPTIONAL = ("t", "qd", "qdd", "sd", "sdd")
+POSE_HOST = {"b2k_jtraj": "q0 qf", "b2k_mtraj": "q0 qf", "b2k_ctraj": "T0 T1", "b2k_mstraj": "row0 rows kind tscal t0 dt coef"}
+POSE_SCALARS = {"b2k_angle_axis": [("tep_stride", 1, 16)], "b2k_p_servo": [("tep_stride", 32, 16)],
+                "b2k_p_servo_rpy": [("tep_stride", -16, 16)], "b2k_jacob0_analytical": [("representation", 4, 0)],
+                "b2k_jtraj": [("tscal", 0.0, 1.0)], "b2k_mtraj": [("kind", 2, 0), ("tf", 0.0, 3.0)]}
+POSE_NMAX = {"b2k_jacob0_analytical": 10, "b2k_jtraj": 10, "b2k_mtraj": 10, "b2k_mstraj": 16}
+_HOST = np.zeros(64)  # q0, qf, T0, T1 and the mstraj tables of fp64
+_HD = _HOST.ctypes.data_as(rtb._lib.dp)
+
+
+def _pose_call(fn, **kw):
+    """fn's status and message; row0 / rows / kind of b2k_mstraj are numpy arrays (one piece of N rows by default)"""
+    lib = rtb._lib.lib()
+    a = dict(dtype=1, n=4, N=4, tep_stride=16, gain=None, threshold=0.1, representation=0, qd0=None, qd1=None, qdf=None,
+             V=None, tblend=None, tscal=1.0, kind=0, tf=3.0, npieces=1, q0=_HD, qf=_HD, T0=_HD, T1=_HD, t0=_HD, dt=_HD,
+             coef=_HD)
+    a.update({d: p for d in "Te Tep e v arrived T J Ja t q qd qdd s sd sdd".split()})
+    if fn == "b2k_mstraj":
+        a.update(tscal=_HD, row0=np.zeros(1, np.int64), rows=np.array([max(kw.get("N", 4), 0)], np.int64),
+                 kind=np.zeros(1, np.int32))
+    a.update(kw)
+    if fn == "b2k_mstraj":
+        for k, ct in (("row0", C.c_int64), ("rows", C.c_int64), ("kind", C.c_int32)):
+            if isinstance(a[k], np.ndarray):
+                a[k] = a[k].ctypes.data_as(C.POINTER(ct))
+    n0 = lib.b2k_launch_count()
+    rc = getattr(lib, fn)(*[a[k] for k in POSE_SIG[fn].split()], None)
+    assert lib.b2k_launch_count() == n0, fn
+    return rc, lib.b2k_last_error().decode()
+
+
+def _pose_cases():
+    """(fn, case, arguments, what the message says; None: the call is accepted)"""
+    for fn in POSE_SIG:
+        dev = POSE_DEV[fn].split()
+        yield fn, "dtype 2", dict(dtype=2), "dtype"
+        if fn in POSE_NMAX:
+            for n in (-1, 0, POSE_NMAX[fn] + 1):
+                yield fn, f"n {n}", dict(n=n), "n must be"
+        yield fn, "N -1", dict(N=-1), "N is negative"
+        for name, bad, _ in POSE_SCALARS.get(fn, []):
+            yield fn, f"{name} {bad}", {name: bad}, name
+        for name in POSE_HOST.get(fn, "").split():
+            yield fn, f"{name} NULL", {name: None}, f"{name} is NULL"
+            yield fn, f"N 0, {name} NULL", {name: None, "N": 0}, f"{name} is NULL"
+        for name in dev:
+            if name not in POSE_OPTIONAL:
+                yield fn, f"{name} NULL", {name: None}, f"{name} is NULL"
+            for dt, half in ((0, 2), (1, 4)):
+                yield fn, f"{name} fp{32 * (dt + 1)} +{half}", {"dtype": dt, name: p + (2 if name == "arrived" else half)}, \
+                    f"{name} is not aligned"
+        yield fn, "N 0, misaligned", {"N": 0, dev[0]: p + 4}, f"{dev[0]} is not aligned"
+        yield fn, "N 0, every device array NULL", {"N": 0, **{d: None for d in dev}}, None
+        yield fn, "N 0, fp32", dict(N=0, dtype=0), None
+    for name, bad in (("npieces", dict(npieces=0)), ("piece 0", dict(row0=np.ones(1, np.int64))),
+                      ("piece 0", dict(kind=np.full(1, 2, np.int32))), ("piece 0", dict(rows=np.full(1, -1, np.int64))),
+                      ("cover", dict(rows=np.full(1, 3, np.int64)))):
+        yield "b2k_mstraj", f"{name}: {bad}", bad, name
+    # b2k_mtraj's trapezoidal profiles that do not exist, after the argument check; axis 2 is the one out of range
+    qf, V = np.ones(4), np.array([np.nan, 0.5, 0.1, np.nan])
+    yield "b2k_mtraj", "V too small", dict(N=0, kind=1, qf=qf.ctypes.data_as(rtb._lib.dp), V=V.ctypes.data_as(rtb._lib.dp)), \
+        "b2k_mtraj: axis 2: V too small"
+    V2 = np.array([np.nan, 0.5, 0.9, np.nan])
+    yield "b2k_mtraj", "V too big", dict(N=4, kind=1, qf=qf.ctypes.data_as(rtb._lib.dp), V=V2.ctypes.data_as(rtb._lib.dp)), \
+        "b2k_mtraj: axis 2: V too big"
+
+
+POSE_CASES = list(_pose_cases())
+
+
+@pytest.mark.parametrize("fn, case, kw, want", POSE_CASES, ids=[f"{c[0]}-{c[1]}" for c in POSE_CASES])
+def test_pose_entry_points_reject_bad_arguments_before_any_cuda_call(fn, case, kw, want):
+    rc, msg = _pose_call(fn, **kw)
+    if want is None:
+        assert rc == 0, msg
+    else:
+        assert rc == -1 and msg.startswith(fn + ":") and want in msg, msg
+
+
+@pytest.mark.parametrize("fn", POSE_SIG)
+def test_pose_entry_points_check_in_one_order(fn):
+    """dtype, n, N, the entry point's scalars, host tables, required device arrays, alignment: with every defect present
+    the first one is reported, and repairing it reports the next."""
+    dev = POSE_DEV[fn].split()
+    args = dict(dtype=2, n=0, N=-1, **{k: bad for k, bad, _ in POSE_SCALARS.get(fn, [])},
+                **{k: None for k in POSE_HOST.get(fn, "").split()},
+                **{d: (p + 2 if d in POSE_OPTIONAL else None) for d in dev})
+    steps = [({}, "dtype"), (dict(dtype=1), "n must be" if fn in POSE_NMAX else "N is negative")]
+    if fn in POSE_NMAX:
+        steps.append((dict(n=4), "N is negative"))
+    fix = dict(N=4)
+    for name, _, good in POSE_SCALARS.get(fn, []):
+        steps.append((fix, name))
+        fix = {name: good}
+    tables = dict(row0=np.zeros(1, np.int64), rows=np.full(1, 4, np.int64), kind=np.zeros(1, np.int32))
+    for name in POSE_HOST.get(fn, "").split():
+        steps.append((fix, f"{name} is NULL"))
+        fix = {name: tables[name] if fn == "b2k_mstraj" and name in tables else _HD}
+    if fn == "b2k_mstraj":
+        steps += [(dict(fix, npieces=0), "npieces"), (dict(npieces=1, row0=np.ones(1, np.int64)), "piece 0"),
+                  (dict(row0=np.zeros(1, np.int64), rows=np.full(1, 3, np.int64)), "cover")]
+        fix = dict(rows=np.full(1, 4, np.int64))
+    for name in dev:
+        if name not in POSE_OPTIONAL:
+            steps.append((fix, f"{name} is NULL"))
+            fix = {name: p + 2}
+    for name in dev:
+        steps.append((fix, f"{name} is not aligned"))
+        fix = {name: p}
+    for fix, want in steps:
+        args.update(fix)
+        rc, msg = _pose_call(fn, **args)
+        assert rc == -1 and msg.startswith(fn + ":") and want in msg, (want, msg)
