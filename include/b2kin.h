@@ -99,6 +99,22 @@ int b2k_chain_destroy(b2k_chain_t chain);
 /* n = joints, m = elementary transforms, q_width = max jindex + 1 */
 int b2k_chain_info(b2k_chain_t chain, int *n, int *m, int *q_width);
 
+/* ---------------------------------------------------------------- entry points that walk a chain
+ * b2k_fkine, b2k_fkine_frames, b2k_jacob0, b2k_jacobe, b2k_fkine_jacob0, b2k_fkine_jacobe, b2k_fkine_planar,
+ * b2k_gravjac, b2k_pay, b2k_paycap and the host front ends b2k_fkine_host and b2k_fkine_jacob0_host take a chain handle
+ * and q (N, ldq), q_width <= ldq <= B2K_MAX_QWIDTH.  Every argument is checked before any CUDA call, in this order: the
+ * chain handle, dtype, N >= 0, q, ldq; then the entry point's own scalars and host tables; then its device arrays in
+ * argument order.  A device array may be NULL only when N = 0 (T or J of b2k_fkine_planar: when not wanted), and must
+ * be aligned as follows (NULL counts as aligned):
+ *   q                                  its element size
+ *   T of the fkj calls, out of frames  32 bytes
+ *   J of the fkj calls                 the piece a row of 6n elements is copied in: 16 bytes when the row is a
+ *                                      multiple of 16 bytes, else 8 when a multiple of 8, else 4 (fp64: 16; fp32:
+ *                                      16 for even n, else 8)
+ *   T, J of b2k_fkine_planar           the same rule on rows of 9 and 3n elements
+ *   static-force arrays                their element size (joint: 4 bytes)
+ * The host front ends take host arrays and need no alignment.  N = 0 returns B2K_OK without touching a device. */
+
 /* ---------------------------------------------------------------- forward kinematics
  * Replaces fknm.ETS_fkine (fknm.cpp:923-1064 -> _ETS_fkine methods.cpp:318-352):
  *   T[i] = base * prod_k ET_k(q[i, jindex_k]) * tool
@@ -112,7 +128,7 @@ int b2k_fkine(b2k_chain_t chain, int dtype, const void *q, int64_t N, int64_t ld
  * Frame k is  base * A_0 J_0(q) ... J_after[k](q) * tails[k]  -- the pose right after joint after[k] (0-based position
  * of the joint along the chain) times a constant 4x4 (row-major, host) -- or, for after[k] = -1, the constant tails[k]
  * itself (the base frame, links that depend on no joint; the caller multiplies the base in).  after[] ascending.
- * out is (N, nslots, 4, 4) row-major, 32-byte aligned; frame k goes to slot[k] of every row; slots not named are left
+ * out is (N, nslots, 4, 4) row-major; frame k goes to slot[k] of every row; slots not named are left
  * untouched (a branched robot takes one call per branch into the same array).  The chain's tool constant and the
  * transforms behind its last joint do not enter. */
 int b2k_fkine_frames(b2k_chain_t chain, int dtype, const void *q, int64_t N, int64_t ldq, const double *base,
@@ -147,8 +163,7 @@ int b2k_fkine_jacobe(b2k_chain_t chain, int dtype, const void *q, int64_t N, int
  *   T (N,3,3) row-major = base * prod_k ET2_k(q[i, jindex_k]) * tool
  *   J (N,3,n), rows (vx, vy, w), columns in chain order: frame 0 = jacob0, in the chain's start frame;
  *     frame 1 = jacobe = blkdiag(R^T, 1) jacob0, R the rotation of the pose (tool in, base out).
- * T or J may be NULL, not both; both from one pass when both are given.  n = 1..B2K_MAX_JOINTS, fp32 / fp64; q rows
- * as b2k_fkine.  Every argument is checked before any CUDA call; N = 0 touches no device. */
+ * T or J may be NULL, not both; both from one pass when both are given.  n = 1..B2K_MAX_JOINTS, fp32 / fp64. */
 int b2k_fkine_planar(b2k_chain_t chain, int dtype, const void *q, int64_t N, int64_t ldq, const double *base,
                      const double *tool, int frame, void *T, void *J, void *stream);
 
@@ -343,8 +358,9 @@ int b2k_rne_accel_derivatives(b2k_rne_t rne, int dtype, const void *q, const voi
  * ROBOT STORES IT (host 3-vector, not negated).  `mass` is a host table of n x 4 doubles (m_j, c_j): c_j is link j's
  * centre of mass in the frame right after joint j's elementary transform.  Flipped joints follow the chain, as in
  * b2k_jacob0 (b2k_rne ignores flip).  Wrenches W = [fx fy fz mx my mz] are device arrays: w_stride 0 = one wrench for
- * every row, 6 = (N, 6).  frame 0: W in the world frame; 1: in the end-effector frame.  Arguments are validated before
- * any CUDA call (NULL pointers, n range, frame, natural alignment); N = 0 returns without touching the device.
+ * every row, 6 = (N, 6).  frame 0: W in the world frame; 1: in the end-effector frame.  b2k_pay_jacobian and
+ * b2k_friction check their arguments as the chain entry points do (n range instead of a chain; device arrays aligned to
+ * their element size).
  *   b2k_gravjac      taug (N,n) = -sum_i J_ci^T m_i g and J0 (N,6,n) = jacob0       DynamicsMixin.gravjac
  *   b2k_pay          tau (N,n) = -J^T W, J = jacob0 (frame 0) or jacobe (frame 1)  DynamicsMixin.pay (given q)
  *   b2k_pay_jacobian tau (N,n) = -J^T W from a given J (N,6,n)                      DynamicsMixin.pay (given J)

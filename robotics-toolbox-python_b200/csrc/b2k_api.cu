@@ -13,13 +13,10 @@
 
 #include "b2k_common.cuh"
 
-// per-dtype launchers (b2k_fkj_f32.cu / b2k_fkj_f64.cu / b2k_ik_*.cu)
-int b2k_fkj_launch_f32(const b2k_chain_s *, int, const void *, long long, long long, const double *, const double *,
-                       void *, void *, cudaStream_t);
-int b2k_fkj_launch_f64(const b2k_chain_s *, int, const void *, long long, long long, const double *, const double *,
-                       void *, void *, cudaStream_t);
-
-enum { FKJ_T = 1, FKJ_J0 = 2, FKJ_JE = 4 };
+// the fkj launchers (b2k_fkj.cuh), one translation unit per dtype
+typedef int FkjLaunchFn(const b2k_chain_s *c, int mode, const void *q, long long nrows, long long ldq, const double *base,
+                        const double *tool, void *T, void *J, cudaStream_t st);
+FkjLaunchFn b2k_fkj_launch_f32, b2k_fkj_launch_f64;
 
 // ------------------------------------------------------------------ error / accounting plumbing
 static thread_local char g_err[512] = "";
@@ -31,6 +28,36 @@ void b2k_set_error(const char *fmt, ...)
     va_start(ap, fmt);
     vsnprintf(g_err, sizeof(g_err), fmt, ap);
     va_end(ap);
+}
+
+int b2k_check_chain(const char *fn, const b2k_chain_s *c, int dtype, const void *q, int64_t N, int64_t ldq, bool q_on_device)
+{
+    if (!c) { b2k_set_error("%s: chain handle is NULL", fn); return B2K_ERR_INVALID; }
+    if (dtype != B2K_F32 && dtype != B2K_F64) { b2k_set_error("%s: dtype must be B2K_F32 or B2K_F64", fn); return B2K_ERR_INVALID; }
+    if (c->n < 1 || c->n > B2K_MAX_JOINTS) { b2k_set_error("%s: unsupported joint count %d", fn, c->n); return B2K_ERR_INVALID; }
+    if (N < 0) { b2k_set_error("%s: N = %lld is negative", fn, (long long)N); return B2K_ERR_INVALID; }
+    if (N > 0 && !q) { b2k_set_error("%s: q is NULL", fn); return B2K_ERR_INVALID; }
+    if (ldq < c->q_width || ldq > B2K_MAX_QWIDTH) {
+        b2k_set_error("%s: q row width %lld outside [%d, %d] (chain reads columns up to %d)", fn, (long long)ldq,
+                      c->q_width, B2K_MAX_QWIDTH, c->q_width - 1);
+        return B2K_ERR_INVALID;
+    }
+    return q_on_device ? b2k_check_array(fn, "q", q, N, dtype == B2K_F64 ? 8u : 4u) : B2K_OK;
+}
+
+int b2k_check_array(const char *fn, const char *name, const void *p, int64_t N, unsigned align)
+{
+    if (N > 0 && !p) { b2k_set_error("%s: %s is NULL", fn, name); return B2K_ERR_INVALID; }
+    if (((uintptr_t)p) & (align - 1)) { b2k_set_error("%s: %s must be %u-byte aligned", fn, name, align); return B2K_ERR_INVALID; }
+    return B2K_OK;
+}
+
+int b2k_check_affine(const char *fn, const char *name, const double *M, int index)
+{
+    if (!M || (M[12] == 0.0 && M[13] == 0.0 && M[14] == 0.0 && M[15] == 1.0)) return B2K_OK;
+    if (index < 0) b2k_set_error("%s: %s is not an SE(3)/affine matrix (bottom row must be 0 0 0 1)", fn, name);
+    else b2k_set_error("%s: %s %d is not an SE(3)/affine matrix (bottom row must be 0 0 0 1)", fn, name, index);
+    return B2K_ERR_INVALID;
 }
 
 int b2k_cuda_fail(cudaError_t e, const char *what)
@@ -99,53 +126,18 @@ extern "C" const char *b2k_last_error(void) { return g_err; }
 extern "C" int b2k_version(void) { return B2K_VERSION; }
 extern "C" int64_t b2k_launch_count(void) { return (int64_t)g_launches.load(); }
 
-// ------------------------------------------------------------------ validation helpers
-// q_on_device: the pointer is read by a kernel (element-wise at worst: only the natural alignment of the element
-// type is needed); host pointers of the *_host front ends only go through cudaMemcpy and need none.
-static int check_common(const char *fn, const b2k_chain_s *c, int dtype, const void *q, int64_t N, int64_t ldq,
-                        bool q_on_device = true)
-{
-    if (!c) { b2k_set_error("%s: chain handle is NULL", fn); return B2K_ERR_INVALID; }
-    if (dtype != B2K_F32 && dtype != B2K_F64) { b2k_set_error("%s: dtype must be B2K_F32 or B2K_F64", fn); return B2K_ERR_INVALID; }
-    if (N < 0) { b2k_set_error("%s: N = %lld is negative", fn, (long long)N); return B2K_ERR_INVALID; }
-    if (N > 0 && !q) { b2k_set_error("%s: q is NULL", fn); return B2K_ERR_INVALID; }
-    if (ldq < c->q_width || ldq > B2K_MAX_QWIDTH) {
-        b2k_set_error("%s: q row width %lld outside [%d, %d] (chain reads columns up to %d)", fn, (long long)ldq,
-                      c->q_width, B2K_MAX_QWIDTH, c->q_width - 1);
-        return B2K_ERR_INVALID;
-    }
-    const unsigned es = dtype == B2K_F64 ? 8u : 4u;
-    if (q_on_device && (((uintptr_t)q) & (es - 1))) { b2k_set_error("%s: q must be %u-byte aligned", fn, es); return B2K_ERR_INVALID; }
-    return B2K_OK;
-}
-
-static int check_out(const char *fn, const char *name, const void *p, int64_t N, unsigned align = 8)
-{
-    if (N > 0 && !p) { b2k_set_error("%s: %s is NULL", fn, name); return B2K_ERR_INVALID; }
-    if (align > 1 && (((uintptr_t)p) & (align - 1))) { b2k_set_error("%s: %s must be %u-byte aligned", fn, name, align); return B2K_ERR_INVALID; }
-    return B2K_OK;
-}
-
-static int check_affine(const char *fn, const char *name, const double *M)
-{
-    if (M && (M[12] != 0.0 || M[13] != 0.0 || M[14] != 0.0 || M[15] != 1.0)) {
-        b2k_set_error("%s: %s is not an SE(3)/affine matrix (bottom row must be 0 0 0 1)", fn, name);
-        return B2K_ERR_INVALID;
-    }
-    return B2K_OK;
-}
-
+// ------------------------------------------------------------------ forward kinematics and Jacobians
 static int fkj_dispatch(const char *fn, b2k_chain_t c, int dtype, int mode, const void *q, int64_t N, int64_t ldq,
                         const double *base, const double *tool, void *T, void *J, void *stream)
 {
-    int rc = check_common(fn, c, dtype, q, N, ldq);
-    if (rc) return rc;
+    int rc;
+    if ((rc = b2k_check_chain(fn, c, dtype, q, N, ldq)) || (rc = b2k_check_affine(fn, "base", base)) ||
+        (rc = b2k_check_affine(fn, "tool", tool)))
+        return rc;
     // T is stored in 32-byte pieces; J leaves through a shared-memory stage of 6n-element rows (TileStage in b2k_fkj.cuh)
-    const unsigned es = dtype == B2K_F64 ? 8u : 4u;
-    const unsigned jub = b2k_stage_unit(6 * c->n * (int)es);
-    if ((mode & FKJ_T) && (rc = check_out(fn, "T", T, N, 32))) return rc;
-    if ((mode & (FKJ_J0 | FKJ_JE)) && (rc = check_out(fn, "J", J, N, jub))) return rc;
-    if ((rc = check_affine(fn, "base", base)) || (rc = check_affine(fn, "tool", tool))) return rc;
+    const int es = dtype == B2K_F64 ? 8 : 4;
+    if ((mode & FKJ_T) && (rc = b2k_check_array(fn, "T", T, N, 32))) return rc;
+    if ((mode & (FKJ_J0 | FKJ_JE)) && (rc = b2k_check_array(fn, "J", J, N, b2k_stage_unit(6 * c->n * es)))) return rc;
     if (N == 0) return B2K_OK;
     B2K_ON_DEVICE_OF(q);
     cudaStream_t st = (cudaStream_t)stream;
@@ -183,31 +175,6 @@ extern "C" int b2k_fkine_jacobe(b2k_chain_t c, int dtype, const void *q, int64_t
     return fkj_dispatch("b2k_fkine_jacobe", c, dtype, FKJ_T | FKJ_JE, q, N, ldq, base, tool, T, J, stream);
 }
 
-// ------------------------------------------------------------------ planar chains (b2k_planar.cu)
-int b2k_planar_check(const char *fn, const b2k_chain_s *c, const double *base, const double *tool);
-int b2k_planar_launch(const b2k_chain_s *c, int dtype, const double *base, const double *tool, int frame, const void *q,
-                      long long nrows, long long ldq, void *T, void *J, cudaStream_t st);
-
-extern "C" int b2k_fkine_planar(b2k_chain_t c, int dtype, const void *q, int64_t N, int64_t ldq, const double *base,
-                                const double *tool, int frame, void *T, void *J, void *stream)
-{
-    const char *fn = "b2k_fkine_planar";
-    if (!c) { b2k_set_error("%s: chain handle is NULL", fn); return B2K_ERR_INVALID; }
-    if (dtype != B2K_F32 && dtype != B2K_F64) { b2k_set_error("%s: dtype must be B2K_F32 or B2K_F64", fn); return B2K_ERR_INVALID; }
-    if (c->n < 1 || c->n > B2K_MAX_JOINTS) { b2k_set_error("%s: unsupported joint count %d", fn, c->n); return B2K_ERR_INVALID; }
-    if (frame != 0 && frame != 1) { b2k_set_error("%s: frame must be 0 (jacob0) or 1 (jacobe), got %d", fn, frame); return B2K_ERR_INVALID; }
-    if (!T && !J) { b2k_set_error("%s: T and J are both NULL; nothing to compute", fn); return B2K_ERR_INVALID; }
-    int rc = b2k_planar_check(fn, c, base, tool);
-    if (rc) return rc;
-    if ((rc = check_common(fn, c, dtype, q, N, ldq))) return rc;
-    const unsigned es = dtype == B2K_F64 ? 8u : 4u;
-    if ((T && (rc = check_out(fn, "T", T, N, b2k_stage_unit(9 * es)))) || (J && (rc = check_out(fn, "J", J, N, b2k_stage_unit(3 * c->n * es)))))
-        return rc;
-    if (N == 0) return B2K_OK;
-    B2K_ON_DEVICE_OF(q);
-    return b2k_planar_launch(c, dtype, base, tool, frame, q, N, ldq, T, J, (cudaStream_t)stream);
-}
-
 // ------------------------------------------------------------------ operations on an rne handle
 // the generic kernels (b2k_rne.cuh), one translation unit per family of operations and dtype
 typedef int RneGenericFn(const b2k_rne_s *, int op, int dtype, const b2k_rne_args &, cudaStream_t);
@@ -227,10 +194,10 @@ static int rne_dispatch(const char *fn, int op, b2k_rne_t r, int dtype, b2k_rne_
     int rc;
     const int es = dtype == B2K_F64 ? 8 : 4;
     for (int i = 0; i < d.nin; i++)
-        if ((rc = check_out(fn, d.in[i], a.in[i], a.nrows, es))) return rc;
+        if ((rc = b2k_check_array(fn, d.in[i], a.in[i], a.nrows, es))) return rc;
     // each output leaves through a per-warp stage of its rows, copied in b2k_stage_unit(row bytes) pieces (b2k_rne.cuh)
     for (int o = 0; o < d.nout; o++)
-        if ((rc = check_out(fn, d.out[o], a.out[o], a.nrows, b2k_stage_unit(d.out_row(o, r->n) * es)))) return rc;
+        if ((rc = b2k_check_array(fn, d.out[o], a.out[o], a.nrows, b2k_stage_unit(d.out_row(o, r->n) * es)))) return rc;
     if (a.nrows == 0) return B2K_OK;
     B2K_ON_DEVICE_OF(a.in[0]);
     cudaStream_t st = (cudaStream_t)stream;
@@ -417,40 +384,36 @@ int run_pipeline(int device, long long N, int n_in, const void *const *h_in, con
 }
 } // namespace
 
-extern "C" int b2k_fkine_jacob0_host(b2k_chain_t c, int dtype, const void *q, int64_t N, int64_t ldq, const double *base,
-                                     const double *tool, void *T, void *J, int device)
+// b2k_fkine_host and b2k_fkine_jacob0_host (jacob: also J (N, 6, n))
+static int fkine_host(const char *fn, b2k_chain_t c, int dtype, const void *q, int64_t N, int64_t ldq, const double *base,
+                      const double *tool, void *T, bool jacob, void *J, int device)
 {
-    const char *fn = "b2k_fkine_jacob0_host";
-    int rc = check_common(fn, c, dtype, q, N, ldq, false);
-    if (rc) return rc;
-    if ((rc = check_out(fn, "T", T, N, 1)) || (rc = check_out(fn, "J", J, N, 1))) return rc;
+    int rc;
+    if ((rc = b2k_check_chain(fn, c, dtype, q, N, ldq, false)) || (rc = b2k_check_array(fn, "T", T, N, 1)) ||
+        (jacob && (rc = b2k_check_array(fn, "J", J, N, 1))))
+        return rc;
     if (N == 0) return B2K_OK;
     const size_t es = dtype == B2K_F64 ? 8 : 4;
     const void *h_in[1] = {q};
     size_t in_b[1] = {(size_t)ldq * es};
     void *h_out[2] = {T, J};
     size_t out_b[2] = {16 * es, (size_t)6 * c->n * es};
-    return run_pipeline(device, N, 1, h_in, in_b, 2, h_out, out_b, [&](Slot &s, long long rows) {
-        return b2k_fkine_jacob0(c, dtype, s.d_in[0], rows, ldq, base, tool, s.d_out[0], s.d_out[1], s.st);
+    return run_pipeline(device, N, 1, h_in, in_b, jacob ? 2 : 1, h_out, out_b, [&](Slot &s, long long rows) {
+        if (jacob) return b2k_fkine_jacob0(c, dtype, s.d_in[0], rows, ldq, base, tool, s.d_out[0], s.d_out[1], s.st);
+        return b2k_fkine(c, dtype, s.d_in[0], rows, ldq, base, tool, s.d_out[0], s.st);
     });
+}
+
+extern "C" int b2k_fkine_jacob0_host(b2k_chain_t c, int dtype, const void *q, int64_t N, int64_t ldq, const double *base,
+                                     const double *tool, void *T, void *J, int device)
+{
+    return fkine_host("b2k_fkine_jacob0_host", c, dtype, q, N, ldq, base, tool, T, true, J, device);
 }
 
 extern "C" int b2k_fkine_host(b2k_chain_t c, int dtype, const void *q, int64_t N, int64_t ldq, const double *base,
                               const double *tool, void *T, int device)
 {
-    const char *fn = "b2k_fkine_host";
-    int rc = check_common(fn, c, dtype, q, N, ldq, false);
-    if (rc) return rc;
-    if ((rc = check_out(fn, "T", T, N, 1))) return rc;
-    if (N == 0) return B2K_OK;
-    const size_t es = dtype == B2K_F64 ? 8 : 4;
-    const void *h_in[1] = {q};
-    size_t in_b[1] = {(size_t)ldq * es};
-    void *h_out[1] = {T};
-    size_t out_b[1] = {16 * es};
-    return run_pipeline(device, N, 1, h_in, in_b, 1, h_out, out_b, [&](Slot &s, long long rows) {
-        return b2k_fkine(c, dtype, s.d_in[0], rows, ldq, base, tool, s.d_out[0], s.st);
-    });
+    return fkine_host("b2k_fkine_host", c, dtype, q, N, ldq, base, tool, T, false, nullptr, device);
 }
 
 // b2k_rne_host and b2k_rne_wrench_host (wrench: also the base wrench wbase (N, 6))
@@ -462,7 +425,7 @@ static int rne_host(const char *fn, b2k_rne_t r, int dtype, const void *q, const
     if (N < 0 || (N > 0 && (!q || !qd || !qdd || !tau || !grav))) { b2k_set_error("%s: NULL argument", fn); return B2K_ERR_INVALID; }
     const size_t es = dtype == B2K_F64 ? 8 : 4;
     int rc;
-    if (wrench && (rc = check_out(fn, "wbase", wbase, N, (unsigned)es))) return rc;
+    if (wrench && (rc = b2k_check_array(fn, "wbase", wbase, N, (unsigned)es))) return rc;
     if (N == 0) return B2K_OK;
     const void *h_in[3] = {q, qd, qdd};
     size_t in_b[3] = {r->n * es, r->n * es, r->n * es};
@@ -552,9 +515,11 @@ static int ik_dispatch(const char *fn, int variant, b2k_chain_t c, int dtype, Ik
         return B2K_ERR_INVALID;
     }
     int rc;
-    if ((rc = check_out(fn, "Tep", a.Tep, a.N)) || (rc = check_out(fn, "q_out", a.q_out, a.N)) ||
-        (rc = check_out(fn, "success", a.success, a.N)) || (rc = check_out(fn, "iterations", a.iterations, a.N)) ||
-        (rc = check_out(fn, "searches", a.searches, a.N)) || (rc = check_out(fn, "residual", a.residual, a.N)))
+    if ((rc = b2k_check_array(fn, "Tep", a.Tep, a.N, 8)) || (rc = b2k_check_array(fn, "q_out", a.q_out, a.N, 8)) ||
+        (rc = b2k_check_array(fn, "success", a.success, a.N, 8)) ||
+        (rc = b2k_check_array(fn, "iterations", a.iterations, a.N, 8)) ||
+        (rc = b2k_check_array(fn, "searches", a.searches, a.N, 8)) ||
+        (rc = b2k_check_array(fn, "residual", a.residual, a.N, 8)))
         return rc;
     const bool pinv = variant != IK_QP && (a.method == B2K_IK_NR || a.method == B2K_IK_GN);
     if (pinv && a.lambda < 0) { b2k_set_error("%s: pinv_damping is negative", fn); return B2K_ERR_INVALID; }

@@ -120,6 +120,9 @@ struct IkArgs {
     } gains;
 };
 
+// what an fkj call (b2k_fkj.cuh) writes: the pose T, the Jacobian in the start frame, or in the end-effector frame
+enum { FKJ_T = 1, FKJ_J0 = 2, FKJ_JE = 4 };
+
 // the unit a per-warp output stage of rows of `row_bytes` is copied in (TileStage<real, n>::UB in b2k_fkj.cuh): 16 bytes
 // when a row is a whole number of 16-byte units, else 8, else 4.  An output array must be aligned to it.
 constexpr int b2k_stage_unit(int row_bytes) { return row_bytes % 16 == 0 ? 16 : (row_bytes % 8 == 0 ? 8 : 4); }
@@ -176,8 +179,17 @@ void b2k_rne_spec_detach(b2k_rne_s *r);
 long long b2k_rne_spec_launch(const b2k_rne_s *r, int mode, int dtype, const void *in0, const void *in1, const void *in2,
                               long long nrows, const double *grav, const double *fext, void *out, void *out2, cudaStream_t st);
 
-// ---- error plumbing (b2k_api.cu)
+// ---- error plumbing and argument checks (b2k_api.cu)
 void b2k_set_error(const char *fmt, ...);
+// The arguments every entry point that walks a chain shares, in this order: handle, dtype, joint count, N >= 0, q not
+// NULL when N > 0, q row width ldq in [q_width, B2K_MAX_QWIDTH], and, when q_on_device, q aligned to its element size
+// (a kernel reads it element-wise at worst; the host pointers of the *_host front ends only go through cudaMemcpy).
+int b2k_check_chain(const char *fn, const b2k_chain_s *c, int dtype, const void *q, int64_t N, int64_t ldq,
+                    bool q_on_device = true);
+// an array of N rows: not NULL when N > 0, and aligned to `align` bytes (1: any address)
+int b2k_check_array(const char *fn, const char *name, const void *p, int64_t N, unsigned align);
+// a host 4x4 row-major matrix, NULL or with the bottom row 0 0 0 1; index >= 0 is printed after the name
+int b2k_check_affine(const char *fn, const char *name, const double *M, int index = -1);
 int b2k_cuda_fail(cudaError_t e, const char *what);
 void b2k_count_launch(int n = 1);
 int b2k_num_sms(int *device_out = nullptr);
@@ -186,6 +198,27 @@ int b2k_num_sms(int *device_out = nullptr);
 int b2k_blocks_per_sm(const void *func, int threads, size_t smem);
 // once per device: keep freed stream-ordered allocations cached in the default memory pool
 void b2k_keep_mempool();
+
+// Calls go(std::integral_constant<int, N>()) for the joint count n = N in 1..10: the kernels are unrolled per N.
+template <typename F>
+int b2k_for_joints(int n, F &&go)
+{
+    static_assert(B2K_MAX_JOINTS == 10, "one case per joint count");
+    switch (n) {
+    case 1: return go(std::integral_constant<int, 1>());
+    case 2: return go(std::integral_constant<int, 2>());
+    case 3: return go(std::integral_constant<int, 3>());
+    case 4: return go(std::integral_constant<int, 4>());
+    case 5: return go(std::integral_constant<int, 5>());
+    case 6: return go(std::integral_constant<int, 6>());
+    case 7: return go(std::integral_constant<int, 7>());
+    case 8: return go(std::integral_constant<int, 8>());
+    case 9: return go(std::integral_constant<int, 9>());
+    case 10: return go(std::integral_constant<int, 10>());
+    }
+    b2k_set_error("unsupported joint count %d", n);
+    return B2K_ERR_INVALID;
+}
 
 #define B2K_CUDA(call)                                   \
     do {                                                 \

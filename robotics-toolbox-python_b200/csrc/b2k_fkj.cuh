@@ -836,8 +836,6 @@ k_fkj_backward(const __grid_constant__ ChainP<real, N> P, const real *__restrict
 }
 
 // ------------------------------------------------------------------ launcher
-enum { FKJ_T = 1, FKJ_J0 = 2, FKJ_JE = 4 };
-
 inline int b2k_gcd(int a, int b) { return b ? b2k_gcd(b, a % b) : a; }
 
 // can the q tile be kept as an exact image in shared memory (16-byte cp.async path)?
@@ -926,14 +924,7 @@ template <typename real>
 int fkj_launch(const b2k_chain_s *c, int mode, const void *q, long long nrows, long long ldq, const double *base,
                const double *tool, void *T, void *J, cudaStream_t st)
 {
-#define B2K_CASE(NN) \
-    case NN: return fkj_launch_n<real, NN>(c, mode, (const real *)q, nrows, (int)ldq, base, tool, (real *)T, (real *)J, st);
-    switch (c->n) {
-        B2K_CASE(1) B2K_CASE(2) B2K_CASE(3) B2K_CASE(4) B2K_CASE(5)
-        B2K_CASE(6) B2K_CASE(7) B2K_CASE(8) B2K_CASE(9) B2K_CASE(10)
-    default:
-        b2k_set_error("fkj: unsupported joint count %d", c->n);
-        return B2K_ERR_INVALID;
-    }
-#undef B2K_CASE
+    return b2k_for_joints(c->n, [&](auto n) {
+        return fkj_launch_n<real, n.value>(c, mode, (const real *)q, nrows, (int)ldq, base, tool, (real *)T, (real *)J, st);
+    });
 }

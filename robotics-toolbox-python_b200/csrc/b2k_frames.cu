@@ -82,13 +82,8 @@ extern "C" int b2k_fkine_frames(b2k_chain_t c, int dtype, const void *q, int64_t
                                 void *stream)
 {
     const char *fn = "b2k_fkine_frames";
-    if (!c) { b2k_set_error("%s: chain handle is NULL", fn); return B2K_ERR_INVALID; }
-    if (dtype != B2K_F32 && dtype != B2K_F64) { b2k_set_error("%s: dtype must be B2K_F32 or B2K_F64", fn); return B2K_ERR_INVALID; }
-    if (N < 0 || (N > 0 && (!q || !out))) { b2k_set_error("%s: bad N / q / out", fn); return B2K_ERR_INVALID; }
-    if (ldq < c->q_width || ldq > B2K_MAX_QWIDTH) {
-        b2k_set_error("%s: q row width %lld outside [%d, %d]", fn, (long long)ldq, c->q_width, B2K_MAX_QWIDTH);
-        return B2K_ERR_INVALID;
-    }
+    int rc;
+    if ((rc = b2k_check_chain(fn, c, dtype, q, N, ldq)) || (rc = b2k_check_affine(fn, "base", base))) return rc;
     if (nframes < 1 || !after || !slot || !tails || nslots < 1) { b2k_set_error("%s: bad frame table", fn); return B2K_ERR_INVALID; }
     for (int k = 0; k < nframes; k++) {
         if (after[k] < -1 || after[k] >= c->n || (k > 0 && after[k] < after[k - 1])) {
@@ -96,28 +91,16 @@ extern "C" int b2k_fkine_frames(b2k_chain_t c, int dtype, const void *q, int64_t
             return B2K_ERR_INVALID;
         }
         if (slot[k] < 0 || slot[k] >= nslots) { b2k_set_error("%s: slot[%d] = %d outside [0, %lld)", fn, k, slot[k], (long long)nslots); return B2K_ERR_INVALID; }
-        const double *M = tails + (size_t)k * 16;
-        if (M[12] != 0.0 || M[13] != 0.0 || M[14] != 0.0 || M[15] != 1.0) { b2k_set_error("%s: tail %d is not an SE(3)/affine matrix", fn, k); return B2K_ERR_INVALID; }
+        if ((rc = b2k_check_affine(fn, "tail", tails + (size_t)k * 16, k))) return rc;
     }
-    if (base && (base[12] != 0.0 || base[13] != 0.0 || base[14] != 0.0 || base[15] != 1.0)) { b2k_set_error("%s: base is not an SE(3)/affine matrix", fn); return B2K_ERR_INVALID; }
-    const unsigned es = dtype == B2K_F64 ? 8u : 4u;
-    if ((uintptr_t)q & (es - 1)) { b2k_set_error("%s: q must be %u-byte aligned", fn, es); return B2K_ERR_INVALID; }
-    if ((uintptr_t)out & 31) { b2k_set_error("%s: out must be 32-byte aligned", fn); return B2K_ERR_INVALID; }
+    if ((rc = b2k_check_array(fn, "out", out, N, 32))) return rc;
     if (N == 0) return B2K_OK;
     B2K_ON_DEVICE_OF(q);
     cudaStream_t st = (cudaStream_t)stream;
-#define B2K_CASE(NN)                                                                                                          \
-    case NN:                                                                                                                  \
-        return dtype == B2K_F64 ? frames_launch_n<double, NN>(c, (const double *)q, N, (int)ldq, base, nframes, after, slot,  \
-                                                              tails, (double *)out, nslots, st)                               \
-                                : frames_launch_n<float, NN>(c, (const float *)q, N, (int)ldq, base, nframes, after, slot,    \
-                                                             tails, (float *)out, nslots, st);
-    switch (c->n) {
-        B2K_CASE(1) B2K_CASE(2) B2K_CASE(3) B2K_CASE(4) B2K_CASE(5)
-        B2K_CASE(6) B2K_CASE(7) B2K_CASE(8) B2K_CASE(9) B2K_CASE(10)
-    default:
-        b2k_set_error("%s: unsupported joint count %d", fn, c->n);
-        return B2K_ERR_INVALID;
-    }
-#undef B2K_CASE
+    return b2k_for_joints(c->n, [&](auto n) {
+        return dtype == B2K_F64 ? frames_launch_n<double, n.value>(c, (const double *)q, N, (int)ldq, base, nframes, after, slot,
+                                                                   tails, (double *)out, nslots, st)
+                                : frames_launch_n<float, n.value>(c, (const float *)q, N, (int)ldq, base, nframes, after, slot,
+                                                                  tails, (float *)out, nslots, st);
+    });
 }

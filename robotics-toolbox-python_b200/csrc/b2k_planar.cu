@@ -240,27 +240,9 @@ int planar_launch_n(const b2k_chain_s *c, const double *base, const double *tool
     return frame ? launch(k_planar<real, N, false, true, 1>, false, true) : launch(k_planar<real, N, false, true, 0>, false, true);
 }
 
-template <typename real>
-int planar_launch(const b2k_chain_s *c, const double *base, const double *tool, int frame, const void *q, long long nrows,
-                  long long ldq, void *T, void *J, cudaStream_t st)
-{
-#define B2K_CASE(NN) \
-    case NN: return planar_launch_n<real, NN>(c, base, tool, frame, (const real *)q, nrows, (int)ldq, (real *)T, (real *)J, st);
-    switch (c->n) {
-        B2K_CASE(1) B2K_CASE(2) B2K_CASE(3) B2K_CASE(4) B2K_CASE(5)
-        B2K_CASE(6) B2K_CASE(7) B2K_CASE(8) B2K_CASE(9) B2K_CASE(10)
-    default:
-        b2k_set_error("b2k_fkine_planar: unsupported joint count %d", c->n);
-        return B2K_ERR_INVALID;
-    }
-#undef B2K_CASE
-}
-
-} // namespace
-
 // B2K_OK when the chain (and the base / tool, row-major 3x3, either may be NULL) is planar; otherwise an error naming the
 // first transform, in chain order, that leaves the plane.  Host only.
-int b2k_planar_check(const char *fn, const b2k_chain_s *c, const double *base, const double *tool)
+int planar_check(const char *fn, const b2k_chain_s *c, const double *base, const double *tool)
 {
     const double *M[2] = {base, tool};
     const char *names[2] = {"base", "tool"};
@@ -288,9 +270,29 @@ int b2k_planar_check(const char *fn, const b2k_chain_s *c, const double *base, c
     return B2K_OK;
 }
 
-int b2k_planar_launch(const b2k_chain_s *c, int dtype, const double *base, const double *tool, int frame, const void *q,
-                      long long nrows, long long ldq, void *T, void *J, cudaStream_t st)
+} // namespace
+
+extern "C" int b2k_fkine_planar(b2k_chain_t c, int dtype, const void *q, int64_t N, int64_t ldq, const double *base,
+                                const double *tool, int frame, void *T, void *J, void *stream)
 {
-    if (dtype == B2K_F64) return planar_launch<double>(c, base, tool, frame, q, nrows, ldq, T, J, st);
-    return planar_launch<float>(c, base, tool, frame, q, nrows, ldq, T, J, st);
+    const char *fn = "b2k_fkine_planar";
+    int rc = b2k_check_chain(fn, c, dtype, q, N, ldq);
+    if (rc) return rc;
+    if (frame != 0 && frame != 1) { b2k_set_error("%s: frame must be 0 (jacob0) or 1 (jacobe), got %d", fn, frame); return B2K_ERR_INVALID; }
+    if (!T && !J) { b2k_set_error("%s: T and J are both NULL; nothing to compute", fn); return B2K_ERR_INVALID; }
+    if ((rc = planar_check(fn, c, base, tool))) return rc;
+    // T and J leave through per-warp stages of 9- and 3n-element rows (TileStage in b2k_fkj.cuh)
+    const int es = dtype == B2K_F64 ? 8 : 4;
+    if ((T && (rc = b2k_check_array(fn, "T", T, N, b2k_stage_unit(9 * es)))) ||
+        (J && (rc = b2k_check_array(fn, "J", J, N, b2k_stage_unit(3 * c->n * es)))))
+        return rc;
+    if (N == 0) return B2K_OK;
+    B2K_ON_DEVICE_OF(q);
+    cudaStream_t st = (cudaStream_t)stream;
+    return b2k_for_joints(c->n, [&](auto n) {
+        return dtype == B2K_F64 ? planar_launch_n<double, n.value>(c, base, tool, frame, (const double *)q, N, (int)ldq,
+                                                                   (double *)T, (double *)J, st)
+                                : planar_launch_n<float, n.value>(c, base, tool, frame, (const float *)q, N, (int)ldq,
+                                                                  (float *)T, (float *)J, st);
+    });
 }

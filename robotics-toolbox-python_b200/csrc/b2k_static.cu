@@ -232,85 +232,43 @@ __global__ void __launch_bounds__(256) k_friction(const __grid_constant__ Fricti
 }
 
 // ------------------------------------------------------------------ host side
+// One call of b2k_gravjac (mass, grav; tau = taug, J = J0), b2k_pay (w, w_stride, frame; tau) or b2k_paycap (mass, grav,
+// w, w_stride, frame, tauR; tau = wmax, joint), as passed; what the mode does not read is NULL or 0.
+struct StaticArgs {
+    const void *q;
+    long long nrows, ldq;
+    const double *mass, *grav;
+    const void *w;
+    long long w_stride;
+    int frame;
+    const double *tauR;
+    void *tau, *J;
+    int *joint;
+};
+
 template <typename real, int N, int MODE>
-static int static_launch_n(const b2k_chain_s *c, const real *q, long long nrows, int ldq, const double *mass, const double *grav,
-                           const real *w, int w_stride, int frame, const double *tauR, real *tau, real *J, int *joint,
-                           cudaStream_t st)
+static int static_launch_n(const b2k_chain_s *c, const StaticArgs &a, cudaStream_t st)
 {
     ChainP<real, N> P;
     b2k_fill_chain<real, N>(c, nullptr, nullptr, true, P);
     StaticP<real, N> S;
     double suf = 0.0;
     for (int j = N - 1; j >= 0; j--) {
-        const double *mj = mass ? mass + 4 * j : nullptr;
+        const double *mj = a.mass ? a.mass + 4 * j : nullptr;
         S.m[j] = mj ? (real)mj[0] : (real)0;
         for (int i = 0; i < 3; i++) S.c[j][i] = mj ? (real)mj[1 + i] : (real)0;
         suf += mj ? mj[0] : 0.0;
         S.msuf[j] = (real)suf;
-        S.tauR[j][0] = tauR ? (real)tauR[2 * j] : (real)0;
-        S.tauR[j][1] = tauR ? (real)tauR[2 * j + 1] : (real)0;
+        S.tauR[j][0] = a.tauR ? (real)a.tauR[2 * j] : (real)0;
+        S.tauR[j][1] = a.tauR ? (real)a.tauR[2 * j + 1] : (real)0;
     }
-    for (int i = 0; i < 3; i++) S.g[i] = grav ? (real)grav[i] : (real)0;
-    S.frame = frame;
-    const unsigned blocks = (unsigned)((nrows + B2K_STATIC_THREADS - 1) / B2K_STATIC_THREADS);
-    k_static<real, N, MODE><<<blocks, B2K_STATIC_THREADS, 0, st>>>(P, S, q, nrows, ldq, w, w_stride, tau, J, joint);
+    for (int i = 0; i < 3; i++) S.g[i] = a.grav ? (real)a.grav[i] : (real)0;
+    S.frame = a.frame;
+    const unsigned blocks = (unsigned)((a.nrows + B2K_STATIC_THREADS - 1) / B2K_STATIC_THREADS);
+    k_static<real, N, MODE><<<blocks, B2K_STATIC_THREADS, 0, st>>>(P, S, (const real *)a.q, a.nrows, (int)a.ldq, (const real *)a.w,
+                                                                 (int)a.w_stride, (real *)a.tau, (real *)a.J, a.joint);
     b2k_count_launch();
     B2K_CUDA(cudaGetLastError());
-    return B2K_OK;
-}
-
-template <int MODE>
-static int static_dispatch(const b2k_chain_s *c, int dtype, const void *q, long long N, int ldq, const double *mass,
-                           const double *grav, const void *w, int w_stride, int frame, const double *tauR, void *tau, void *J,
-                           int *joint, cudaStream_t st)
-{
-#define B2K_CASE(NN)                                                                                                          \
-    case NN:                                                                                                                  \
-        return dtype == B2K_F64                                                                                               \
-                   ? static_launch_n<double, NN, MODE>(c, (const double *)q, N, ldq, mass, grav, (const double *)w, w_stride, \
-                                                       frame, tauR, (double *)tau, (double *)J, joint, st)                    \
-                   : static_launch_n<float, NN, MODE>(c, (const float *)q, N, ldq, mass, grav, (const float *)w, w_stride,    \
-                                                      frame, tauR, (float *)tau, (float *)J, joint, st);
-    switch (c->n) {
-        B2K_CASE(1) B2K_CASE(2) B2K_CASE(3) B2K_CASE(4) B2K_CASE(5)
-        B2K_CASE(6) B2K_CASE(7) B2K_CASE(8) B2K_CASE(9) B2K_CASE(10)
-    default:
-        b2k_set_error("unsupported joint count %d", c->n);
-        return B2K_ERR_INVALID;
-    }
-#undef B2K_CASE
-}
-
-static bool misaligned(const void *p, unsigned bytes) { return ((uintptr_t)p & (bytes - 1)) != 0; }
-
-// the checks every chain entry point shares: handle, dtype, N, q and its row width
-static int check_chain_args(const char *fn, b2k_chain_t c, int dtype, const void *q, int64_t N, int64_t ldq)
-{
-    if (!c) { b2k_set_error("%s: chain handle is NULL", fn); return B2K_ERR_INVALID; }
-    if (dtype != B2K_F32 && dtype != B2K_F64) { b2k_set_error("%s: dtype must be B2K_F32 or B2K_F64", fn); return B2K_ERR_INVALID; }
-    if (c->n < 1 || c->n > B2K_MAX_JOINTS) { b2k_set_error("%s: joint count %d outside [1, %d]", fn, c->n, B2K_MAX_JOINTS); return B2K_ERR_INVALID; }
-    if (N < 0) { b2k_set_error("%s: N is negative", fn); return B2K_ERR_INVALID; }
-    if (N > 0 && !q) { b2k_set_error("%s: q is NULL", fn); return B2K_ERR_INVALID; }
-    if (ldq < c->q_width || ldq > B2K_MAX_QWIDTH) {
-        b2k_set_error("%s: q row width %lld outside [%d, %d]", fn, (long long)ldq, c->q_width, B2K_MAX_QWIDTH);
-        return B2K_ERR_INVALID;
-    }
-    if (misaligned(q, dtype == B2K_F64 ? 8u : 4u)) { b2k_set_error("%s: q is not aligned to its element size", fn); return B2K_ERR_INVALID; }
-    return B2K_OK;
-}
-
-static int check_wrench(const char *fn, int dtype, const void *W, int64_t w_stride, int64_t N)
-{
-    if (N > 0 && !W) { b2k_set_error("%s: the wrench is NULL", fn); return B2K_ERR_INVALID; }
-    if (w_stride != 0 && w_stride != 6) { b2k_set_error("%s: w_stride must be 0 (one wrench) or 6 (one per row)", fn); return B2K_ERR_INVALID; }
-    if (misaligned(W, dtype == B2K_F64 ? 8u : 4u)) { b2k_set_error("%s: the wrench is not aligned to its element size", fn); return B2K_ERR_INVALID; }
-    return B2K_OK;
-}
-
-static int check_out(const char *fn, const char *name, int dtype, const void *p, int64_t N)
-{
-    if (N > 0 && !p) { b2k_set_error("%s: %s is NULL", fn, name); return B2K_ERR_INVALID; }
-    if (misaligned(p, dtype == B2K_F64 ? 8u : 4u)) { b2k_set_error("%s: %s is not aligned to its element size", fn, name); return B2K_ERR_INVALID; }
     return B2K_OK;
 }
 
@@ -324,56 +282,60 @@ static int check_mass(const char *fn, const b2k_chain_s *c, const double *mass, 
     return B2K_OK;
 }
 
-#define B2K_TRY(x)              \
-    do {                        \
-        const int _rc = (x);    \
-        if (_rc) return _rc;    \
-    } while (0)
+static int check_w_stride(const char *fn, int64_t w_stride)
+{
+    if (w_stride != 0 && w_stride != 6) { b2k_set_error("%s: w_stride must be 0 (one wrench) or 6 (one per row)", fn); return B2K_ERR_INVALID; }
+    return B2K_OK;
+}
+
+// Every argument is checked before any CUDA call: the chain, then the host tables and scalars the mode reads, then the
+// device arrays, each aligned to its element size.
+template <int MODE>
+static int static_dispatch(const char *fn, b2k_chain_t c, int dtype, const StaticArgs &a, void *stream)
+{
+    const bool mass = MODE != ST_PAY, wrench = MODE != ST_GRAVJAC;
+    int rc;
+    if ((rc = b2k_check_chain(fn, c, dtype, a.q, a.nrows, a.ldq))) return rc;
+    if (mass && (rc = check_mass(fn, c, a.mass, a.grav))) return rc;
+    if (wrench) {
+        if ((rc = check_w_stride(fn, a.w_stride))) return rc;
+        if (a.frame != 0 && a.frame != 1) { b2k_set_error("%s: frame must be 0 (world) or 1 (end effector)", fn); return B2K_ERR_INVALID; }
+    }
+    if (MODE == ST_PAYCAP && !a.tauR) { b2k_set_error("%s: tauR is NULL", fn); return B2K_ERR_INVALID; }
+    const unsigned es = dtype == B2K_F64 ? 8 : 4;
+    const long long N = a.nrows;
+    if ((wrench && (rc = b2k_check_array(fn, MODE == ST_PAY ? "W" : "w", a.w, N, es))) ||
+        (rc = b2k_check_array(fn, MODE == ST_GRAVJAC ? "taug" : MODE == ST_PAY ? "tau" : "wmax", a.tau, N, es)) ||
+        (MODE == ST_GRAVJAC && (rc = b2k_check_array(fn, "J0", a.J, N, es))) ||
+        (MODE == ST_PAYCAP && (rc = b2k_check_array(fn, "joint", a.joint, N, 4))))
+        return rc;
+    if (N == 0) return B2K_OK;
+    B2K_ON_DEVICE_OF(a.q);
+    cudaStream_t st = (cudaStream_t)stream;
+    return b2k_for_joints(c->n, [&](auto n) {
+        return dtype == B2K_F64 ? static_launch_n<double, n.value, MODE>(c, a, st) : static_launch_n<float, n.value, MODE>(c, a, st);
+    });
+}
 
 extern "C" int b2k_gravjac(b2k_chain_t c, int dtype, const void *q, int64_t N, int64_t ldq, const double *mass, const double *grav,
                            void *taug, void *J0, void *stream)
 {
-    const char *fn = "b2k_gravjac";
-    B2K_TRY(check_chain_args(fn, c, dtype, q, N, ldq));
-    B2K_TRY(check_mass(fn, c, mass, grav));
-    B2K_TRY(check_out(fn, "taug", dtype, taug, N));
-    B2K_TRY(check_out(fn, "J0", dtype, J0, N));
-    if (N == 0) return B2K_OK;
-    B2K_ON_DEVICE_OF(q);
-    return static_dispatch<ST_GRAVJAC>(c, dtype, q, N, (int)ldq, mass, grav, nullptr, 0, 0, nullptr, taug, J0, nullptr,
-                                       (cudaStream_t)stream);
+    return static_dispatch<ST_GRAVJAC>("b2k_gravjac", c, dtype, {q, N, ldq, mass, grav, nullptr, 0, 0, nullptr, taug, J0, nullptr},
+                                       stream);
 }
 
 extern "C" int b2k_pay(b2k_chain_t c, int dtype, const void *q, int64_t N, int64_t ldq, const void *W, int64_t w_stride, int frame,
                        void *tau, void *stream)
 {
-    const char *fn = "b2k_pay";
-    B2K_TRY(check_chain_args(fn, c, dtype, q, N, ldq));
-    B2K_TRY(check_wrench(fn, dtype, W, w_stride, N));
-    if (frame != 0 && frame != 1) { b2k_set_error("%s: frame must be 0 (world) or 1 (end effector)", fn); return B2K_ERR_INVALID; }
-    B2K_TRY(check_out(fn, "tau", dtype, tau, N));
-    if (N == 0) return B2K_OK;
-    B2K_ON_DEVICE_OF(q);
-    return static_dispatch<ST_PAY>(c, dtype, q, N, (int)ldq, nullptr, nullptr, W, (int)w_stride, frame, nullptr, tau, nullptr, nullptr,
-                                   (cudaStream_t)stream);
+    return static_dispatch<ST_PAY>("b2k_pay", c, dtype, {q, N, ldq, nullptr, nullptr, W, w_stride, frame, nullptr, tau, nullptr, nullptr},
+                                   stream);
 }
 
 extern "C" int b2k_paycap(b2k_chain_t c, int dtype, const void *q, int64_t N, int64_t ldq, const double *mass, const double *grav,
                           const void *w, int64_t w_stride, int frame, const double *tauR, void *wmax, int32_t *joint, void *stream)
 {
-    const char *fn = "b2k_paycap";
-    B2K_TRY(check_chain_args(fn, c, dtype, q, N, ldq));
-    B2K_TRY(check_mass(fn, c, mass, grav));
-    B2K_TRY(check_wrench(fn, dtype, w, w_stride, N));
-    if (frame != 0 && frame != 1) { b2k_set_error("%s: frame must be 0 (world) or 1 (end effector)", fn); return B2K_ERR_INVALID; }
-    if (!tauR) { b2k_set_error("%s: tauR is NULL", fn); return B2K_ERR_INVALID; }
-    B2K_TRY(check_out(fn, "wmax", dtype, wmax, N));
-    if (N > 0 && !joint) { b2k_set_error("%s: joint is NULL", fn); return B2K_ERR_INVALID; }
-    if (misaligned(joint, 4u)) { b2k_set_error("%s: joint is not 4-byte aligned", fn); return B2K_ERR_INVALID; }
-    if (N == 0) return B2K_OK;
-    B2K_ON_DEVICE_OF(q);
-    return static_dispatch<ST_PAYCAP>(c, dtype, q, N, (int)ldq, mass, grav, w, (int)w_stride, frame, tauR, wmax, nullptr, joint,
-                                      (cudaStream_t)stream);
+    return static_dispatch<ST_PAYCAP>("b2k_paycap", c, dtype, {q, N, ldq, mass, grav, w, w_stride, frame, tauR, wmax, nullptr, joint},
+                                      stream);
 }
 
 extern "C" int b2k_pay_jacobian(int dtype, int n, const void *J, const void *W, int64_t w_stride, int64_t N, void *tau, void *stream)
@@ -382,9 +344,11 @@ extern "C" int b2k_pay_jacobian(int dtype, int n, const void *J, const void *W, 
     if (dtype != B2K_F32 && dtype != B2K_F64) { b2k_set_error("%s: dtype must be B2K_F32 or B2K_F64", fn); return B2K_ERR_INVALID; }
     if (n < 1 || n > B2K_MAX_JOINTS) { b2k_set_error("%s: n = %d outside [1, %d]", fn, n, B2K_MAX_JOINTS); return B2K_ERR_INVALID; }
     if (N < 0) { b2k_set_error("%s: N is negative", fn); return B2K_ERR_INVALID; }
-    B2K_TRY(check_out(fn, "J", dtype, J, N));
-    B2K_TRY(check_wrench(fn, dtype, W, w_stride, N));
-    B2K_TRY(check_out(fn, "tau", dtype, tau, N));
+    const unsigned es = dtype == B2K_F64 ? 8 : 4;
+    int rc;
+    if ((rc = check_w_stride(fn, w_stride)) || (rc = b2k_check_array(fn, "J", J, N, es)) ||
+        (rc = b2k_check_array(fn, "W", W, N, es)) || (rc = b2k_check_array(fn, "tau", tau, N, es)))
+        return rc;
     if (N == 0) return B2K_OK;
     B2K_ON_DEVICE_OF(J);
     const long long total = (long long)N * n;
@@ -423,8 +387,9 @@ extern "C" int b2k_friction(int dtype, int n, const double *params, const void *
     for (int k = 0; k < 4 * n; k++)
         if (!isfinite(params[k])) { b2k_set_error("%s: params[%d] is not finite", fn, k); return B2K_ERR_INVALID; }
     if (N < 0) { b2k_set_error("%s: N is negative", fn); return B2K_ERR_INVALID; }
-    B2K_TRY(check_out(fn, "qd", dtype, qd, N));
-    B2K_TRY(check_out(fn, "tau", dtype, tau, N));
+    const unsigned es = dtype == B2K_F64 ? 8 : 4;
+    int rc;
+    if ((rc = b2k_check_array(fn, "qd", qd, N, es)) || (rc = b2k_check_array(fn, "tau", tau, N, es))) return rc;
     if (N == 0) return B2K_OK;
     B2K_ON_DEVICE_OF(qd);
     const long long total = (long long)N * n;
