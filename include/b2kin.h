@@ -318,6 +318,19 @@ int b2k_tree_rne(b2k_tree_t tree, int dtype, const void *q, const void *qd, cons
 #define B2K_DYN_ACCEL 5
 int b2k_tree_dyn(b2k_tree_t tree, int op, int dtype, const void *in0, const void *in1, const void *in2, int64_t N,
                  const double *grav, void *out, void *stream);
+/* Exact first derivatives of the tree's dynamics (forward-mode tangents of the generated recursion, never differences),
+ * for linearising about a batch of states (MPC, iLQR / DDP, LQR):
+ *   op B2K_DYN_RNE_DERIV   x = qdd     out0 = dtau_dq (N,n,n), out1 = dtau_dqd (N,n,n); out2 must be NULL
+ *      B2K_DYN_ACCEL_DERIV x = torque  out0 = dqdd_dq, out1 = dqdd_dqd, out2 = dqdd_dtau (N,n,n) each
+ * Entry [i, k] = d out_i / d x_k: i in group order as b2k_tree_rne returns tau (op 7) or in the order of B2K_DYN_ACCEL's
+ * output (op 8), k in q order.  Op 8 differentiates qdd* = accel(q, qd, torque) with accel's M and solve:
+ * dqdd_dx = -M^-1 dtau_dx at qdd*, dqdd_dtau = M^-1.  grav = MINUS the robot's gravity, as for b2k_tree_rne.  Arrays are
+ * device, 16-byte aligned.  b2k_tree_dyn rejects these two op codes; b2k_tree_codegen / b2k_tree_info take them (op 8
+ * generates two functions: rne_row, the ACCEL row, and rne_deriv_row, the op 7 row evaluated at qdd*). */
+#define B2K_DYN_RNE_DERIV 7
+#define B2K_DYN_ACCEL_DERIV 8
+int b2k_tree_derivatives(b2k_tree_t tree, int op, int dtype, const void *q, const void *qd, const void *x, int64_t N,
+                         const double *grav, void *out0, void *out1, void *out2, void *stream);
 int b2k_tree_codegen(b2k_tree_t tree, int op, int grav_mask, char *src, int64_t src_cap, double *consts, int32_t consts_cap,
                      int32_t *n_consts, int32_t *counts);
 int b2k_tree_info(b2k_tree_t tree, int op, int dtype, const double *grav, char *buf, int64_t cap);

@@ -495,7 +495,8 @@ class Robot:
             tau = B.to_host(tau)
         return tau[0] if single else tau
 
-    _DYN_OPS = {"rne": 0, "inertia": 1, "gravload": 2, "itorque": 3, "coriolis": 4, "accel": 5}
+    _DYN_OPS = {"rne": 0, "inertia": 1, "gravload": 2, "itorque": 3, "coriolis": 4, "accel": 5, "rne_derivatives": 7,
+                "accel_derivatives": 8}
 
     def rne_kernel_info(self, dtype=np.float64, gravity=None, op="rne") -> str:
         g = self._gravity if gravity is None else np.asarray(gravity, dtype=np.float64).reshape(3)
@@ -506,7 +507,9 @@ class Robot:
 
     # ---- dynamics built on the recursion (reference DynamicsMixin, Dynamics.py, which BaseRobot inherits: each method
     #      there is a Python loop of self.rne calls; here one generated kernel per operation, b2k_tree_dyn)
-    def _tree_dyn(self, op, ins, names, out_tail, gravity=None, dtype=None):
+    def _tree_dyn(self, op, ins, names, out_tail, gravity=None, dtype=None, nout=1):
+        """One generated kernel over rows of `ins`; returns one array of shape (N,) + out_tail, or a tuple of `nout` of
+        them (the derivative operations, b2k_tree_derivatives)."""
         for x, nm in zip(ins, names):
             B.check_numeric(x, nm)
         n = self.n
@@ -525,13 +528,19 @@ class Robot:
             raise ValueError(", ".join(names) + " must have the same number of rows")
         g = self._gravity if gravity is None else np.asarray(gravity, dtype=np.float64).reshape(3)
         ag = np.ascontiguousarray(-g)
-        out = B.empty((N,) + tuple(out_tail), dt, like=dev[0])
+        outs = [B.empty((N,) + tuple(out_tail), dt, like=dev[0]) for _ in range(nout)]
         ptrs = [B.ptr(t) for t in dev] + [None] * (3 - len(dev))
-        _lib.check(_lib.lib().b2k_tree_dyn(self._tree_handle(), self._DYN_OPS[op], B.code(dt), ptrs[0], ptrs[1], ptrs[2], N,
-                                           _lib.dptr(ag), B.ptr(out), B.stream_ptr(dev[0])))
+        if op in ("rne_derivatives", "accel_derivatives"):
+            optrs = [B.ptr(o) for o in outs] + [None] * (3 - nout)
+            _lib.check(_lib.lib().b2k_tree_derivatives(self._tree_handle(), self._DYN_OPS[op], B.code(dt), ptrs[0], ptrs[1],
+                                                       ptrs[2], N, _lib.dptr(ag), *optrs, B.stream_ptr(dev[0])))
+        else:
+            _lib.check(_lib.lib().b2k_tree_dyn(self._tree_handle(), self._DYN_OPS[op], B.code(dt), ptrs[0], ptrs[1], ptrs[2], N,
+                                               _lib.dptr(ag), B.ptr(outs[0]), B.stream_ptr(dev[0])))
         if host:
-            out = B.to_host(out)
-        return out[0] if single else out
+            outs = [B.to_host(o) for o in outs]
+        outs = [o[0] if single else o for o in outs]
+        return tuple(outs) if nout > 1 else outs[0]
 
     def inertia(self, q, dtype=None):
         """Joint-space inertia matrix M(q), (n,n) or (N,n,n) (Dynamics.py:700-758: n rne calls per row there)."""
@@ -553,6 +562,25 @@ class Robot:
         """Forward dynamics qdd = M(q)^-1 (torque - rne(q, qd, 0)) (Dynamics.py:424-503: n + 1 rne calls and a numpy
         solve per row there)."""
         return self._tree_dyn("accel", (q, qd, torque), ("q", "qd", "torque"), (self.n,), gravity=gravity, dtype=dtype)
+
+    def rne_derivatives(self, q, qd, qdd, gravity=None, dtype=None):
+        """Exact first derivatives of inverse dynamics: ``(dtau_dq, dtau_dqd)``, each (n,n) for one state or (N,n,n) for a
+        batch, with ``[i, k] = d tau_i / d x_k`` of ``tau = self.rne(q, qd, qdd, gravity=gravity)``: i in joint-group order
+        as ``rne`` returns tau, k in q order.  The derivative of exactly that function, flipped joints included (their
+        motion subspace ignores the flip, the joint transform does not).  Forward-mode tangents of the recursion generated
+        for this robot, exact to rounding (no step size).  ``d tau / d qdd = inertia(q)`` is not returned.  The
+        linearisation MPC, iLQR / DDP rollouts and LQR about sampled operating points need."""
+        return self._tree_dyn("rne_derivatives", (q, qd, qdd), ("q", "qd", "qdd"), (self.n, self.n), gravity=gravity, dtype=dtype,
+                              nout=2)
+
+    def accel_derivatives(self, q, qd, torque, gravity=None, dtype=None):
+        """Exact first derivatives of forward dynamics ``qdd = self.accel(q, qd, torque, gravity=gravity)``:
+        ``(dqdd_dq, dqdd_dqd, dqdd_dtau)``, each (n,n) or (N,n,n), ``[i, k] = d qdd_i / d x_k`` in the index order of
+        ``accel``.  ``dqdd_dx = -M^-1 d rne(q, qd, qdd*) / dx`` at ``qdd* = accel(q, qd, torque)`` (qdd* held fixed in the
+        rne derivative) and ``dqdd_dtau = M^-1``, with the M and the solve of ``accel``, computed once per state.  A
+        singular M (a point mass on its own joint axis) gives non-finite rows, as ``accel`` does."""
+        return self._tree_dyn("accel_derivatives", (q, qd, torque), ("q", "qd", "torque"), (self.n, self.n), gravity=gravity,
+                              dtype=dtype, nout=3)
 
     # ---- operational-space dynamics (reference DynamicsMixin, Dynamics.py between gravload and itorque): _opspace.py
     def _opspace_robot(self):

@@ -135,11 +135,13 @@ struct b2k_rne_s {
 
 // Operations on an rne handle.  B2K_GEN_RNE..B2K_GEN_RNE_WRENCH are served by the robot-specialised kernels
 // (b2k_rne_gen.cpp, b2k_rne_spec.cu) on the full 32-row tiles and by the generic ones (b2k_rne.cuh) on the rest; the
-// derivatives only by the generic ones.  RNE..ACCEL are also the public B2K_DYN_* codes of the tree entry points.
+// derivatives of DH arms only by the generic ones, those of trees by the generated kernels.  RNE..ACCEL, RNE_DERIV and
+// ACCEL_DERIV are also the public B2K_DYN_* codes of the tree entry points.
 enum { B2K_GEN_RNE = 0, B2K_GEN_INERTIA = 1, B2K_GEN_GRAVLOAD = 2, B2K_GEN_ITORQUE = 3, B2K_GEN_CORIOLIS = 4, B2K_GEN_ACCEL = 5,
        B2K_GEN_RNE_WRENCH = 6, B2K_GEN_RNE_DERIV = 7, B2K_GEN_ACCEL_DERIV = 8, B2K_GEN_NOPS = 9 };
 static_assert(B2K_GEN_RNE == B2K_DYN_RNE && B2K_GEN_INERTIA == B2K_DYN_INERTIA && B2K_GEN_GRAVLOAD == B2K_DYN_GRAVLOAD &&
-                  B2K_GEN_ITORQUE == B2K_DYN_ITORQUE && B2K_GEN_CORIOLIS == B2K_DYN_CORIOLIS && B2K_GEN_ACCEL == B2K_DYN_ACCEL,
+                  B2K_GEN_ITORQUE == B2K_DYN_ITORQUE && B2K_GEN_CORIOLIS == B2K_DYN_CORIOLIS && B2K_GEN_ACCEL == B2K_DYN_ACCEL &&
+                  B2K_GEN_RNE_DERIV == B2K_DYN_RNE_DERIV && B2K_GEN_ACCEL_DERIV == B2K_DYN_ACCEL_DERIV,
               "B2K_DYN_* (b2kin.h) are the B2K_GEN_* codes of the tree operations");
 
 // What an operation reads and writes.  Every input is an (N, n) array; every output has rows of n or n * n reals, except

@@ -40,21 +40,31 @@ struct Sym {
     Opd x, y;
 };
 
+// How an emitted variable was computed, kept so that its derivatives can be emitted afterwards (tangent()):
+// a * b, fma(a, b, c), a + b (signs in the operands), or a leaf -- a named input or a term with no derivative rule.
+struct Def {
+    enum Op { LEAF, MUL, FMA, ADD } op = LEAF;
+    Opd a, b, c;
+};
+
 struct Gen {
     std::vector<std::string> code;
     std::vector<std::string> names; // variable id -> spelling
+    std::vector<Def> defs;          // variable id -> how it was computed
     std::vector<double> consts;     // constant bank
     std::map<unsigned long long, int> cslot;
     int n_mul = 0, n_fma = 0, n_add = 0;
 
-    int new_var()
+    int new_var(const Def &d = Def())
     {
         names.push_back("t" + std::to_string((int)names.size()));
+        defs.push_back(d);
         return (int)names.size() - 1;
     }
     int named_var(const std::string &s)
     {
         names.push_back(s);
+        defs.push_back(Def());
         return (int)names.size() - 1;
     }
     static Sym zero() { return Sym(); }
@@ -87,9 +97,9 @@ struct Gen {
         }
         return std::string(neg ? "-" : "") + names[o.id];
     }
-    Sym emit(const std::string &rhs)
+    Sym emit(const std::string &rhs, const Def &d = Def())
     {
-        int id = new_var();
+        int id = new_var(d);
         code.push_back("    const real " + names[id] + " = " + rhs + ";");
         Sym s;
         s.k = Sym::O; s.x.id = id;
@@ -99,7 +109,9 @@ struct Gen {
     Opd operand(const Sym &a)
     {
         if (a.k == Sym::O) return a.x;
-        Sym m = emit(spell(a.x) + " * " + spell(a.y));
+        Def d;
+        d.op = Def::MUL; d.a = a.x; d.b = a.y;
+        Sym m = emit(spell(a.x) + " * " + spell(a.y), d);
         n_mul++;
         return m.x;
     }
@@ -156,7 +168,9 @@ struct Gen {
         if (!plain.empty()) { acc = plain[0]; ai = 1; }
         else { acc = operand(prods[0]); pi = 1; }
         for (; pi < prods.size(); pi++) {
-            acc = emit("fma(" + spell(prods[pi].x) + ", " + spell(prods[pi].y) + ", " + spell(acc) + ")").x;
+            Def d;
+            d.op = Def::FMA; d.a = prods[pi].x; d.b = prods[pi].y; d.c = acc;
+            acc = emit("fma(" + spell(prods[pi].x) + ", " + spell(prods[pi].y) + ", " + spell(acc) + ")", d).x;
             n_fma++;
         }
         for (; ai < plain.size(); ai++) {
@@ -167,7 +181,9 @@ struct Gen {
             if (babs.isc) babs.c = fabs(babs.c);
             std::string rhs;
             rhs = spell(acc) + (bneg ? " - " : " + ") + spell(babs);
-            acc = emit(rhs).x;
+            Def d;
+            d.op = Def::ADD; d.a = acc; d.b = b;
+            acc = emit(rhs, d).x;
             n_add++;
         }
         Sym s; s.k = Sym::O; s.x = acc;
@@ -181,6 +197,40 @@ struct Gen {
         if (a.k != Sym::P) return a;
         Sym s; s.k = Sym::O; s.x = operand(a);
         return s;
+    }
+    static Sym val(const Opd &o)
+    {
+        if (o.isc) return cst(o.neg ? -o.c : o.c);
+        Sym s; s.k = Sym::O; s.x = o;
+        return s;
+    }
+    // Forward-mode derivative of the variables emitted so far along one direction.  seed[id] is the derivative of the
+    // leaf variable id (zero when unset); returns the derivative of every variable below `upto`.  The product rule
+    // runs through mul / sum, so a factor whose derivative is structurally zero drops out: no instruction is emitted
+    // for a variable that does not depend on the direction.
+    std::vector<Sym> tangent(int upto, const std::vector<Sym> &seed)
+    {
+        std::vector<Sym> T(seed);
+        T.resize(upto);
+        auto dt = [&](const Opd &o) { // the derivative of an operand (a pending product is read as a plain variable)
+            if (o.isc) return zero();
+            return o.neg ? neg(T[o.id]) : T[o.id];
+        };
+        auto dtf = [&](const Opd &o) { // ... when it becomes a factor: multiplied out once, then reused
+            if (o.isc) return zero();
+            T[o.id] = fix(T[o.id]);
+            return o.neg ? neg(T[o.id]) : T[o.id];
+        };
+        for (int id = 0; id < upto; id++) {
+            const Def &d = defs[id];
+            switch (d.op) {
+            case Def::LEAF: break;
+            case Def::MUL: T[id] = sum({mul(dtf(d.a), val(d.b)), mul(val(d.a), dtf(d.b))}); break;
+            case Def::FMA: T[id] = sum({mul(dtf(d.a), val(d.b)), mul(val(d.a), dtf(d.b)), dt(d.c)}); break;
+            case Def::ADD: T[id] = sum({dt(d.a), dt(d.b)}); break;
+            }
+        }
+        return T;
     }
 };
 
@@ -519,6 +569,40 @@ int assemble(Gen &g, int N, const b2k_gen_opts &o, const RecFn &rec, std::vector
             std::vector<Sym> tau = rec(in);
             for (int k = 0; k < N; k++) tail.push_back(assign(g, "out[" + std::to_string(i * N + k) + "]", tau[k]));
         }
+    } else if (o.mode == B2K_GEN_RNE_DERIV) {
+        // tau = rne(q, qd, qdd, g) once, then one tangent pass per direction q_0..q_{n-1}, qd_0..qd_{n-1}:
+        // dq[i * n + k] = d tau_i / d q_k, dqd[i * n + k] = d tau_i / d qd_k.  Each column is stored as soon as its pass
+        // ends, so that only one direction's tangents are live at a time.
+        sig = "rne_deriv_row(const real *C, const real *grav, const real *fext, const real *st, const real *ct, const real *qq, "
+              "const real *qd, const real *qdd, real *dq, real *dqd)";
+        in.qd = jvec("qd"); in.qdd = jvec("qdd");
+        in.grav = gvec();
+        std::vector<Sym> tau = rec(in);
+        for (Sym &s : tau) s = g.fix(s);
+        const int upto = (int)g.names.size();
+        std::map<std::string, int> leaf; // the inputs of this function (the latest leaf of each name)
+        for (int id = 0; id < upto; id++)
+            if (g.defs[id].op == Def::LEAF && g.names[id].find('[') != std::string::npos) leaf[g.names[id]] = id;
+        auto id_of = [&](const char *a, int k) {
+            auto it = leaf.find(std::string(a) + "[" + std::to_string(k) + "]");
+            return it == leaf.end() ? -1 : it->second;
+        };
+        auto leafsym = [&](int id) { Opd x; x.id = id; return Gen::val(x); };
+        for (int dir = 0; dir < 2 * N; dir++) {
+            const int k = dir % N;
+            std::vector<Sym> seed(upto);
+            if (dir < N) { // st = sin q -> cos q, ct = cos q -> -sin q, qq = q -> 1 (a flipped joint's sign is in the recursion)
+                const int is = id_of("st", k), ic = id_of("ct", k), iq = id_of("qq", k);
+                if (is >= 0 && ic >= 0) { seed[is] = leafsym(ic); seed[ic] = g.neg(leafsym(is)); }
+                if (iq >= 0) seed[iq] = Gen::cst(1.0);
+            } else if (id_of("qd", k) >= 0) seed[id_of("qd", k)] = Gen::cst(1.0);
+            const std::vector<Sym> T = g.tangent(upto, seed);
+            for (int i = 0; i < N; i++) {
+                Sym d = Gen::zero();
+                if (tau[i].k == Sym::O && !tau[i].x.isc) d = tau[i].x.neg ? g.neg(T[tau[i].x.id]) : T[tau[i].x.id];
+                g.code.push_back(assign(g, std::string(dir < N ? "dq[" : "dqd[") + std::to_string(i * N + k) + "]", d));
+            }
+        }
     } else {
         err = "unknown generator mode";
         return -1;
@@ -530,6 +614,10 @@ int assemble(Gen &g, int N, const b2k_gen_opts &o, const RecFn &rec, std::vector
 
 int b2k_rne_generate(const b2k_rne_s *r, const b2k_gen_opts &o, b2k_gen_out &out)
 {
+    if (o.mode == B2K_GEN_RNE_DERIV || o.mode == B2K_GEN_ACCEL_DERIV) {
+        out.error = "the derivatives of DH arms are served by the generic kernel";
+        return -1;
+    }
     const int N = r->n;
     Gen g;
     std::vector<Link> L(N);
@@ -634,11 +722,14 @@ int b2k_tree_generate(const b2k_tree_s *t, const b2k_gen_opts &o, b2k_gen_out &o
     TreeOps T(g);
     Vops &v = T.v;
     std::vector<Sym> st(N), ct(N), qq(N);
-    for (int j = 0; j < N; j++) {
-        const std::string k = "[" + std::to_string(t->jindex[j]) + "]";
-        st[j] = g.var("st" + k); ct[j] = g.var("ct" + k); qq[j] = g.var("qq" + k);
-        if (t->flip[j]) { st[j] = g.neg(st[j]); qq[j] = g.neg(qq[j]); } // eta = -q
-    }
+    auto joint_inputs = [&]() { // the joint angle / offset arguments of one generated function
+        for (int j = 0; j < N; j++) {
+            const std::string k = "[" + std::to_string(t->jindex[j]) + "]";
+            st[j] = g.var("st" + k); ct[j] = g.var("ct" + k); qq[j] = g.var("qq" + k);
+            if (t->flip[j]) { st[j] = g.neg(st[j]); qq[j] = g.neg(qq[j]); } // eta = -q
+        }
+    };
+    joint_inputs();
     auto unit = [&](int axis, const Sym &x) { // x * e_axis
         V3 u = v.zero();
         (axis % 3 == 0 ? u.x : (axis % 3 == 1 ? u.y : u.z)) = x;
@@ -708,8 +799,23 @@ int b2k_tree_generate(const b2k_tree_s *t, const b2k_gen_opts &o, b2k_gen_out &o
     const char *sig = nullptr;
     b2k_gen_opts oo = o;
     oo.has_fext = 0; // Robot.rne has no tip wrench
+    std::string src;
+    if (o.mode == B2K_GEN_ACCEL_DERIV) {
+        // two functions over one constant bank: rne_row, the ACCEL row (M and torque - rne(q, qd, 0)), and rne_deriv_row,
+        // the RNE_DERIV row that the kernel evaluates at the solved qdd* with the same gravity
+        oo.mode = B2K_GEN_ACCEL;
+        if (assemble(g, N, oo, rec, tail, sig, out.error)) return -1;
+        src = std::string("__device__ __forceinline__ void ") + sig + "\n{\n";
+        for (const std::string &s : g.code) src += s + "\n";
+        for (const std::string &s : tail) src += s + "\n";
+        src += "}\n";
+        g.code.clear();
+        tail.clear();
+        joint_inputs();
+        oo.mode = B2K_GEN_RNE_DERIV;
+    }
     if (assemble(g, N, oo, rec, tail, sig, out.error)) return -1;
-    std::string src = std::string("__device__ __forceinline__ void ") + sig + "\n{\n";
+    src += std::string("__device__ __forceinline__ void ") + sig + "\n{\n";
     for (const std::string &s : g.code) src += s + "\n";
     for (const std::string &s : tail) src += s + "\n";
     src += "}\n";

@@ -36,4 +36,7 @@ int b2k_tree_generate(const b2k_tree_s *t, const b2k_gen_opts &o, b2k_gen_out &o
 // outputs of the generated function: RNE / GRAVLOAD / ITORQUE n values; INERTIA / CORIOLIS n*n; ACCEL n*n + n
 // (rows of M followed by torque - rne(q, qd, 0), the wrapper solves the system); RNE_WRENCH n + 6 (tau, then the wrench
 // [f; m] the base exerts on link 1, in frame 0, moment about its origin).  Trees (b2k_tree_generate) reject RNE_WRENCH.
+// Trees only: RNE_DERIV generates `rne_deriv_row(C, grav, fext, st, ct, qq, qd, qdd, dq, dqd)`, dq / dqd the n x n blocks
+// d tau_i / d q_k and d tau_i / d qd_k (i group order, k q order); ACCEL_DERIV generates the ACCEL `rne_row` followed by
+// that `rne_deriv_row` over one constant bank.
 int b2k_rne_generate(const b2k_rne_s *r, const b2k_gen_opts &o, b2k_gen_out &out);

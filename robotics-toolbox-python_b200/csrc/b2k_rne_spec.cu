@@ -17,6 +17,7 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <algorithm>
 #include <functional>
 #include <map>
 #include <mutex>
@@ -33,6 +34,7 @@ namespace {
 // (B2K_GEN_*), NIN (input arrays), NOUT (reals written per row), NRES (reals the row function returns),
 // PADIN (1: padded input rows, element-wise tile load), MINB (resident blocks per SM to aim for); NOUT2 (only for
 // B2K_GEN_RNE_WRENCH: reals per row of a second output array, res[NOUT..NOUT+NOUT2), staged and copied on its own).
+// WPB: warps per block of the derivative kernels (kDeriv), chosen from n so that their output stage fits.
 const char *kPrologue = R"B2KSRC(
 typedef REAL real;
 typedef unsigned long long u64;
@@ -123,17 +125,49 @@ __device__ __forceinline__ void sincos_batch(const real *x, const TrigC &t, real
 #endif
     }
 }
+
+// M (NJ x NJ, row-major, symmetric positive definite; only the lower triangle is read) = L D L^T without pivoting, in
+// place: L below the diagonal of M, D in d.  The accel kernels, the forward-dynamics integrator and the accel derivatives
+// all solve with this one factorisation.
+__device__ __forceinline__ void ldlt_factor(real *M, real *d)
+{
+#pragma unroll
+    for (int c = 0; c < NJ; c++) {
+        real dc = M[c * NJ + c];
+#pragma unroll
+        for (int k = 0; k < c; k++) dc = fma(-M[c * NJ + k] * d[k], M[c * NJ + k], dc);
+        d[c] = dc;
+        const real inv = (real)1 / dc;
+#pragma unroll
+        for (int r = c + 1; r < NJ; r++) {
+            real v = M[r * NJ + c];
+#pragma unroll
+            for (int k = 0; k < c; k++) v = fma(-M[r * NJ + k] * d[k], M[c * NJ + k], v);
+            M[r * NJ + c] = v * inv; // L[r][c]
+        }
+    }
+}
+
+// y <- M^-1 y with the factors of ldlt_factor
+__device__ __forceinline__ void ldlt_solve(const real *L, const real *d, real *y)
+{
+#pragma unroll
+    for (int r = 0; r < NJ; r++)
+#pragma unroll
+        for (int k = 0; k < r; k++) y[r] = fma(-L[r * NJ + k], y[k], y[r]);
+#pragma unroll
+    for (int r = 0; r < NJ; r++) y[r] = y[r] / d[r];
+#pragma unroll
+    for (int r = NJ - 1; r >= 0; r--)
+#pragma unroll
+        for (int k = r + 1; k < NJ; k++) y[r] = fma(-L[k * NJ + r], y[k], y[r]);
+}
 )B2KSRC";
 
-const char *kKernel = R"B2KSRC(
+// the input tiles of the row kernels: 32 rows of NJ reals per array
+const char *kTileIn = R"B2KSRC(
 #define LDI (PADIN ? (NJ | 1) : NJ)                  /* smem row stride of the input tiles, in reals */
 #define IN_BYTES ((32 * LDI * (int)sizeof(real) + 15) & ~15)
-#define OUT_BYTES (32 * NOUT * (int)sizeof(real))
-#ifndef NOUT2
-#define NOUT2 0
-#endif
-#define NBUF (TPW > 1 ? 2 : 1)                        /* input buffers per warp */
-#define WARP_BYTES (NBUF * NIN * IN_BYTES + OUT_BYTES + 32 * NOUT2 * (int)sizeof(real))
 
 __device__ __forceinline__ void load_tile(real *s, const real *g, int lane)
 {
@@ -153,6 +187,15 @@ __device__ __forceinline__ void load_tile(real *s, const real *g, int lane)
             asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"(sa + 512u * (unsigned)k), "l"(gg + 32 * k));
 #endif
 }
+)B2KSRC";
+
+const char *kKernel = R"B2KSRC(
+#define OUT_BYTES (32 * NOUT * (int)sizeof(real))
+#ifndef NOUT2
+#define NOUT2 0
+#endif
+#define NBUF (TPW > 1 ? 2 : 1)                        /* input buffers per warp */
+#define WARP_BYTES (NBUF * NIN * IN_BYTES + OUT_BYTES + 32 * NOUT2 * (int)sizeof(real))
 
 // A warp owns TPW consecutive tiles of 32 rows (one-shot grid of full tiles; the ragged tail of a batch goes to the
 // generic kernel).  The input tiles are double-buffered: the cp.async loads of tile t+1 are issued before tile t is
@@ -212,32 +255,9 @@ k_rne_spec(const __grid_constant__ SpecP P, const real *__restrict__ in0, const 
         // accel: res = [M (NJ x NJ, row i = torques for a unit acceleration of joint i) | torque - rne(q, qd, 0)].
         // M is the joint-space inertia matrix (symmetric positive definite): LDL^T without pivoting, in registers.
         real d[NJ];
-#pragma unroll
-        for (int c = 0; c < NJ; c++) {
-            real dc = res[c * NJ + c];
-#pragma unroll
-            for (int k = 0; k < c; k++) dc = fma(-res[c * NJ + k] * d[k], res[c * NJ + k], dc);
-            d[c] = dc;
-            const real inv = (real)1 / dc;
-#pragma unroll
-            for (int r = c + 1; r < NJ; r++) {
-                real v = res[r * NJ + c];
-#pragma unroll
-                for (int k = 0; k < c; k++) v = fma(-res[r * NJ + k] * d[k], res[c * NJ + k], v);
-                res[r * NJ + c] = v * inv; // L[r][c]
-            }
-        }
+        ldlt_factor(res, d);
         real *y = res + NJ * NJ;
-#pragma unroll
-        for (int r = 0; r < NJ; r++)
-#pragma unroll
-            for (int k = 0; k < r; k++) y[r] = fma(-res[r * NJ + k], y[k], y[r]);
-#pragma unroll
-        for (int r = 0; r < NJ; r++) y[r] = y[r] / d[r];
-#pragma unroll
-        for (int r = NJ - 1; r >= 0; r--)
-#pragma unroll
-            for (int k = r + 1; k < NJ; k++) y[r] = fma(-res[k * NJ + r], y[k], y[r]);
+        ldlt_solve(res, d, y);
         const real *o = y;
 #else
         const real *o = res;
@@ -273,6 +293,105 @@ k_rne_spec(const __grid_constant__ SpecP P, const real *__restrict__ in0, const 
 )B2KSRC";
 
 
+// ------------------------------------------------------------------ derivatives of the dynamics of a tree (MODE 7, 8)
+// A row writes 2 (RNE_DERIV: dtau_dq, dtau_dqd) or 3 (ACCEL_DERIV: dqdd_dq, dqdd_dqd, dqdd_dtau) blocks of NJ x NJ reals.
+// The generated derivative row stores its columns straight into the warp's shared stage, one exact-image n x n tile per
+// output (32 rows), copied out by one TMA bulk copy each; the number of warps per block (WPB) is chosen from n so that
+// the stage fits (fp64 n = 16, three outputs: 197 KB for one warp).
+const char *kDeriv = R"B2KSRC(
+#define NSQ (NJ * NJ)
+#define NBLK (MODE == 8 ? 3 : 2)
+#define BLK_BYTES (32 * NSQ * (int)sizeof(real))
+#define WARP_BYTES (NIN * IN_BYTES + NBLK * BLK_BYTES)
+
+extern "C" __global__ void __launch_bounds__(32 * WPB, MINB)
+k_rne_deriv_spec(const __grid_constant__ SpecP P, const real *__restrict__ in0, const real *__restrict__ in1,
+                 const real *__restrict__ in2, real *__restrict__ out0, real *__restrict__ out1, real *__restrict__ out2,
+                 long long ntiles)
+{
+    extern __shared__ __align__(16) unsigned char smem[];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const long long tile = (long long)blockIdx.x * WPB + warp;
+    if (tile >= ntiles) return;
+    unsigned char *wb = smem + (size_t)warp * WARP_BYTES;
+    real *so = reinterpret_cast<real *>(wb + NIN * IN_BYTES);
+    const size_t row0 = (size_t)tile * 32;
+    load_tile(reinterpret_cast<real *>(wb), in0 + row0 * NJ, lane);
+    load_tile(reinterpret_cast<real *>(wb + IN_BYTES), in1 + row0 * NJ, lane);
+    load_tile(reinterpret_cast<real *>(wb + 2 * IN_BYTES), in2 + row0 * NJ, lane);
+#if !PADIN
+    asm volatile("cp.async.commit_group;\n" ::: "memory");
+    asm volatile("cp.async.wait_group 0;\n" ::: "memory");
+#endif
+    __syncwarp();
+    const real *s0 = reinterpret_cast<const real *>(wb);
+    const real *s1 = reinterpret_cast<const real *>(wb + IN_BYTES);
+    const real *s2 = reinterpret_cast<const real *>(wb + 2 * IN_BYTES);
+    real th[NJ], st[NJ], ct[NJ], a1[NJ], a2[NJ];
+#pragma unroll
+    for (int j = 0; j < NJ; j++) {
+        th[j] = s0[lane * LDI + j] + P.offset[j];
+        a1[j] = s1[lane * LDI + j];
+        a2[j] = s2[lane * LDI + j];
+    }
+    sincos_batch(th, P.trig, st, ct);
+    real *d0 = so + lane * NSQ, *d1 = so + 32 * NSQ + lane * NSQ;
+#if MODE == 8
+    // qdd* = M^-1 (torque - rne(q, qd, 0)) as accel computes it; dqdd_dtau = M^-1 from the same factorisation, staged
+    // before the derivative row so that the factors are dead while it runs; then the derivatives of rne(q, qd, qdd*)
+    // with qdd* held fixed, mapped in the stage: dqdd_dx = -M^-1 dtau_dx
+    real *d2 = so + 64 * NSQ + lane * NSQ, qdd[NJ];
+    {
+        real res[NJ * NJ + NJ], d[NJ];
+        rne_row(P.C, P.grav, P.fext, st, ct, th, a1, a2, res);
+        ldlt_factor(res, d);
+        ldlt_solve(res, d, res + NSQ);
+#pragma unroll
+        for (int i = 0; i < NJ; i++) qdd[i] = res[NSQ + i];
+#pragma unroll 1
+        for (int c = 0; c < NJ; c++) {
+            real y[NJ];
+#pragma unroll
+            for (int i = 0; i < NJ; i++) y[i] = (real)(i == c);
+            ldlt_solve(res, d, y);
+#pragma unroll
+            for (int i = 0; i < NJ; i++) d2[i * NJ + c] = y[i];
+        }
+    }
+    rne_deriv_row(P.C, P.grav, P.fext, st, ct, th, a1, qdd, d0, d1);
+#pragma unroll 1
+    for (int k = 0; k < 2 * NJ; k++) {
+        real *blk = k < NJ ? d0 : d1;
+        const int c = k < NJ ? k : k - NJ;
+        real x[NJ];
+#pragma unroll
+        for (int i = 0; i < NJ; i++) x[i] = blk[i * NJ + c];
+#pragma unroll
+        for (int i = 0; i < NJ; i++) {
+            real y = (real)0;
+#pragma unroll
+            for (int j = 0; j < NJ; j++) y = fma(-d2[i * NJ + j], x[j], y);
+            blk[i * NJ + c] = y;
+        }
+    }
+#else
+    rne_deriv_row(P.C, P.grav, P.fext, st, ct, th, a1, a2, d0, d1);
+#endif
+    // the staged tiles are the exact images of the output blocks: one TMA bulk copy (shared -> global) each, by lane 0
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    __syncwarp();
+    if (lane == 0) {
+        real *outs[3] = {out0, out1, out2};
+#pragma unroll
+        for (int b = 0; b < NBLK; b++)
+            asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(outs[b] + row0 * NSQ),
+                         "r"((unsigned)__cvta_generic_to_shared(so + b * 32 * NSQ)), "r"((unsigned)BLK_BYTES) : "memory");
+        asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+        asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); // the copies read this warp's shared memory
+    }
+}
+)B2KSRC";
+
 // ------------------------------------------------------------------ forward-dynamics integrator (DynamicsMixin.fdyn)
 // The reference integrates ONE state with scipy's RK45, calling accel() -- n + 1 Python rne loops and a numpy solve --
 // for every stage (Dynamics.py:185-422).  Here one lane integrates one trajectory of an ensemble entirely on the device:
@@ -305,32 +424,9 @@ __device__ __forceinline__ void fd_accel(const SpecP &P, const FdynP &F, const r
     sincos_batch(th, P.trig, st, ct);
     rne_row(P.C, P.grav, P.fext, st, ct, th, y + NJ, tq, res);
     real d[NJ];
-#pragma unroll
-    for (int c = 0; c < NJ; c++) {
-        real dc = res[c * NJ + c];
-#pragma unroll
-        for (int k = 0; k < c; k++) dc = fma(-res[c * NJ + k] * d[k], res[c * NJ + k], dc);
-        d[c] = dc;
-        const real inv = (real)1 / dc;
-#pragma unroll
-        for (int r = c + 1; r < NJ; r++) {
-            real v = res[r * NJ + c];
-#pragma unroll
-            for (int k = 0; k < c; k++) v = fma(-res[r * NJ + k] * d[k], res[c * NJ + k], v);
-            res[r * NJ + c] = v * inv;
-        }
-    }
+    ldlt_factor(res, d);
     real *x = res + NJ * NJ;
-#pragma unroll
-    for (int r = 0; r < NJ; r++)
-#pragma unroll
-        for (int k = 0; k < r; k++) x[r] = fma(-res[r * NJ + k], x[k], x[r]);
-#pragma unroll
-    for (int r = 0; r < NJ; r++) x[r] = x[r] / d[r];
-#pragma unroll
-    for (int r = NJ - 1; r >= 0; r--)
-#pragma unroll
-        for (int k = r + 1; k < NJ; k++) x[r] = fma(-res[k * NJ + r], x[k], x[r]);
+    ldlt_solve(res, d, x);
 #pragma unroll
     for (int j = 0; j < NJ; j++) qdd[j] = x[j];
 }
@@ -548,6 +644,8 @@ struct Program {
     std::string cubin;        // sm_90a image
     std::vector<double> consts;
     int nin = 1, nout = 0, nout2 = 0, nres = 0, nc = 1, tpw = 1;
+    int wpb = 4;    // warps per block
+    int nblk = 0;   // derivative kernels: output blocks of n x n reals (2 or 3), each its own array
     const char *entry = "k_rne_spec";
     int n_mul = 0, n_fma = 0, n_add = 0, regs = 0;
     size_t smem = 0;
@@ -588,6 +686,7 @@ std::string build_source(const GenFn &gen, int n, int mode, int dtype, Program &
     p.n_mul = g.n_mul; p.n_fma = g.n_fma; p.n_add = g.n_add;
     const b2k_rne_op_s &op = B2K_RNE_OPS[mode];
     p.nin = op.nin;
+    const bool deriv = mode == B2K_GEN_RNE_DERIV || mode == B2K_GEN_ACCEL_DERIV;
     p.nout = op.out_row(0, n);
     p.nout2 = op.nout > 1 ? op.out_row(1, n) : 0; // tau (N, n) and the base wrench (N, 6)
     p.nres = mode == B2K_GEN_ACCEL ? n * n + n : p.nout + p.nout2;
@@ -608,10 +707,18 @@ std::string build_source(const GenFn &gen, int n, int mode, int dtype, Program &
     const int tpw = (dtype == B2K_F32 && light) ? 2 : 1;
     p.tpw = tpw;
     p.smem = 4 * ((tpw > 1 ? 2 : 1) * p.nin * in_bytes + (size_t)32 * (p.nout + p.nout2) * es);
+    if (deriv) { // one stage of 32 x n x n reals per output block and warp; as many warps per block as fit, up to 4
+        p.nblk = op.nout;
+        p.nout = n * n; p.nout2 = 0;
+        p.nres = n * n + n;
+        const size_t warp_bytes = p.nin * in_bytes + (size_t)p.nblk * 32 * n * n * es;
+        p.wpb = (int)std::min<size_t>(4, (220 * 1024) / warp_bytes);
+        p.smem = (size_t)std::max(p.wpb, 1) * warp_bytes;
+    }
     if (p.smem > 220 * 1024) { p.why = "a tile of this operation does not fit the shared memory of an SM (" + std::to_string(p.smem) + " B)"; return std::string(); }
     int minb = (int)((200 * 1024) / (p.smem + 1024));
     // resident blocks to aim for (swept: fp64 96 registers / 5 blocks, fp32 64 registers / 8 blocks)
-    const int want = light ? (es == 8 ? 5 : 8) : (es == 8 ? 2 : 3);
+    const int want = deriv ? 1 : light ? (es == 8 ? 5 : 8) : (es == 8 ? 2 : 3);
     if (minb > want) minb = want;
     if (minb < 1) minb = 1;
     auto D = [&](const char *k, long long v) { defs.push_back(std::string("-D") + k + "=" + std::to_string(v)); };
@@ -619,8 +726,9 @@ std::string build_source(const GenFn &gen, int n, int mode, int dtype, Program &
     D("REAL_IS_F64", es == 8);
     D("NJ", n); D("NC", p.nc); D("MODE", mode); D("NIN", p.nin); D("NOUT", p.nout); D("NRES", p.nres); D("PADIN", padin); D("MINB", minb); D("TPW", tpw);
     if (p.nout2) D("NOUT2", p.nout2);
+    if (deriv) D("WPB", p.wpb);
     // in1 / in2 of the generated function are the second / third input rows; the RNE proper names them qd / qdd
-    return std::string(kPrologue) + g.source + (kernel_text ? kernel_text : kKernel);
+    return std::string(kPrologue) + g.source + (kernel_text ? kernel_text : std::string(kTileIn) + (deriv ? kDeriv : kKernel));
 }
 
 void compile(const GenFn &gen, int n, const Key &key, Program &p)
@@ -631,6 +739,7 @@ void compile(const GenFn &gen, int n, const Key &key, Program &p)
     std::vector<std::string> defs;
     const bool fdyn = std::get<0>(key) / 100 == 2;
     if (fdyn) p.entry = "k_fdyn";
+    else if (mode == B2K_GEN_RNE_DERIV || mode == B2K_GEN_ACCEL_DERIV) p.entry = "k_rne_deriv_spec";
     const std::string src = build_source(gen, n, mode, dtype, p, defs, fdyn ? kFdyn : nullptr);
     if (src.empty()) return;
     std::vector<std::string> opts = {"--gpu-architecture=sm_90a", "--std=c++17"};
@@ -758,15 +867,16 @@ std::vector<unsigned char> spec_params(Program *p, int n, int dtype, const doubl
 }
 
 int launch_tiles(Program *p, CUfunction fn, int n, int dtype, const double *offset, const void *in0, const void *in1, const void *in2,
-                 void *out, void *out2, long long ntiles, const double *grav, const double *fext, cudaStream_t st)
+                 void *out, void *out2, long long ntiles, const double *grav, const double *fext, cudaStream_t st, void *out3 = nullptr)
 {
     std::vector<unsigned char> pb = spec_params(p, n, dtype, offset, grav, fext);
     long long nt = ntiles;
-    void *args[7] = {pb.data(), (void *)&in0, (void *)&in1, (void *)&in2, (void *)&out, (void *)&nt, nullptr};
-    if (p->nout2) { args[5] = (void *)&out2; args[6] = (void *)&nt; } // k_rne_spec(..., out, out2, ntiles)
-    const long long per_block = 4LL * p->tpw;
+    void *args[8] = {pb.data(), (void *)&in0, (void *)&in1, (void *)&in2, (void *)&out, (void *)&nt, nullptr, nullptr};
+    if (p->nblk) { args[5] = (void *)&out2; args[6] = (void *)&out3; args[7] = (void *)&nt; } // k_rne_deriv_spec(..., out0, out1, out2, ntiles)
+    else if (p->nout2) { args[5] = (void *)&out2; args[6] = (void *)&nt; } // k_rne_spec(..., out, out2, ntiles)
+    const long long per_block = (long long)p->wpb * p->tpw;
     const unsigned grid = (unsigned)((ntiles + per_block - 1) / per_block);
-    CUresult rc = driver()->LaunchKernel(fn, grid, 1, 1, 128, 1, 1, (unsigned)p->smem, (CUstream)st, args, nullptr);
+    CUresult rc = driver()->LaunchKernel(fn, grid, 1, 1, 32 * p->wpb, 1, 1, (unsigned)p->smem, (CUstream)st, args, nullptr);
     if (rc != CUDA_SUCCESS) {
         const char *es2 = nullptr;
         driver()->GetErrorString(rc, &es2);
@@ -930,19 +1040,30 @@ static Program *tree_program(b2k_tree_t t, int mode, int dtype, int gmask)
     }, t->n, key);
 }
 
-// Robot.rne (mode 0) and the operations DynamicsMixin builds on it (modes 1-5: inertia, gravload, itorque, coriolis, accel)
-// for a rigid-body tree: the generated kernel on the full tiles, one padded tile for the ragged tail.
-static int tree_run(const char *fn, b2k_tree_t t, int mode, int dtype, const void *in0, const void *in1, const void *in2, int64_t N,
-                    const double *grav, void *out, void *stream)
+// Robot.rne (mode 0), the operations DynamicsMixin builds on it (modes 1-5: inertia, gravload, itorque, coriolis, accel) and
+// their derivatives (modes 7, 8; `derivs`: the b2k_tree_derivatives entry point) for a rigid-body tree: the generated kernel
+// on the full tiles, one padded tile for the ragged tail.  out[0..nout) are the operation's output arrays.
+static int tree_run(const char *fn, b2k_tree_t t, int mode, bool derivs, int dtype, const void *in0, const void *in1, const void *in2,
+                    int64_t N, const double *grav, void *const out[3], void *stream)
 {
     if (!t) { b2k_set_error("%s: tree handle is NULL", fn); return B2K_ERR_INVALID; }
-    if (mode < B2K_GEN_RNE || mode > B2K_GEN_ACCEL) { b2k_set_error("%s: operation %d is not one of B2K_DYN_*", fn, mode); return B2K_ERR_INVALID; }
+    if (derivs ? (mode != B2K_GEN_RNE_DERIV && mode != B2K_GEN_ACCEL_DERIV) : (mode < B2K_GEN_RNE || mode > B2K_GEN_ACCEL)) {
+        if (derivs) b2k_set_error("%s: operation %d is not B2K_DYN_RNE_DERIV or B2K_DYN_ACCEL_DERIV", fn, mode);
+        else b2k_set_error("%s: operation %d is not one of B2K_DYN_*", fn, mode);
+        return B2K_ERR_INVALID;
+    }
     if (dtype != B2K_F32 && dtype != B2K_F64) { b2k_set_error("%s: dtype must be B2K_F32 or B2K_F64", fn); return B2K_ERR_INVALID; }
-    const int nin = B2K_RNE_OPS[mode].nin;
-    if (N < 0 || (N > 0 && (!in0 || (nin >= 2 && !in1) || (nin >= 3 && !in2) || !out))) { b2k_set_error("%s: bad arguments", fn); return B2K_ERR_INVALID; }
-    const bool ug = B2K_RNE_OPS[mode].grav;
+    const b2k_rne_op_s &op = B2K_RNE_OPS[mode];
+    const int nin = op.nin, nout = op.nout;
+    bool missing = false;
+    for (int o = 0; o < nout; o++) missing |= !out[o];
+    if (N < 0 || (N > 0 && (!in0 || (nin >= 2 && !in1) || (nin >= 3 && !in2) || missing))) { b2k_set_error("%s: bad arguments", fn); return B2K_ERR_INVALID; }
+    for (int o = nout; o < 3; o++)
+        if (out[o]) { b2k_set_error("%s: operation %d has %d outputs: %s must be NULL", fn, mode, nout, o == 2 ? "out2" : "out1"); return B2K_ERR_INVALID; }
+    const bool ug = op.grav;
     if (ug && !grav) { b2k_set_error("%s: grav is NULL (pass MINUS the robot's gravity: a_grav of Robot.rne)", fn); return B2K_ERR_INVALID; }
-    const uintptr_t al = (uintptr_t)in0 | (uintptr_t)(nin >= 2 ? in1 : in0) | (uintptr_t)(nin >= 3 ? in2 : in0) | (uintptr_t)out;
+    uintptr_t al = (uintptr_t)in0 | (uintptr_t)(nin >= 2 ? in1 : in0) | (uintptr_t)(nin >= 3 ? in2 : in0);
+    for (int o = 0; o < nout; o++) al |= (uintptr_t)out[o];
     if (al & 15) { b2k_set_error("%s: arrays must be 16-byte aligned", fn); return B2K_ERR_INVALID; }
     if (N == 0) return B2K_OK;
     B2K_ON_DEVICE_OF(in0);
@@ -963,18 +1084,20 @@ static int tree_run(const char *fn, b2k_tree_t t, int mode, int dtype, const voi
     const long long ntiles = N / 32, tail = N - ntiles * 32;
     const double *gv = ug ? grav : nullptr;
     int rc = B2K_OK;
-    if (ntiles) rc = launch_tiles(p, f, n, dtype, nullptr, in0, in1, in2, out, nullptr, ntiles, gv, nullptr, st);
+    if (ntiles) rc = launch_tiles(p, f, n, dtype, nullptr, in0, in1, in2, out[0], out[1], ntiles, gv, nullptr, st, out[2]);
     if (rc == B2K_OK && tail) { // ragged tail: one padded tile through stream-ordered scratch
         b2k_keep_mempool();
         char *scr = nullptr;
-        B2K_CUDA(cudaMallocAsync((void **)&scr, 3 * 32 * rowb + 32 * orowb, st));
+        B2K_CUDA(cudaMallocAsync((void **)&scr, 3 * 32 * rowb + nout * 32 * orowb, st));
         cudaMemsetAsync(scr, 0, 3 * 32 * rowb, st);
         const size_t off = (size_t)ntiles * 32 * rowb;
         const void *src[3] = {in0, in1, in2};
         for (int i = 0; i < nin; i++) cudaMemcpyAsync(scr + i * 32 * rowb, (const char *)src[i] + off, tail * rowb, cudaMemcpyDeviceToDevice, st);
-        char *so = scr + 3 * 32 * rowb;
-        rc = launch_tiles(p, f, n, dtype, nullptr, scr, scr + 32 * rowb, scr + 2 * 32 * rowb, so, nullptr, 1, gv, nullptr, st);
-        cudaMemcpyAsync((char *)out + (size_t)ntiles * 32 * orowb, so, tail * orowb, cudaMemcpyDeviceToDevice, st);
+        char *so[3] = {nullptr, nullptr, nullptr};
+        for (int o = 0; o < nout; o++) so[o] = scr + 3 * 32 * rowb + o * 32 * orowb;
+        rc = launch_tiles(p, f, n, dtype, nullptr, scr, scr + 32 * rowb, scr + 2 * 32 * rowb, so[0], so[1], 1, gv, nullptr, st, so[2]);
+        for (int o = 0; o < nout; o++)
+            cudaMemcpyAsync((char *)out[o] + (size_t)ntiles * 32 * orowb, so[o], tail * orowb, cudaMemcpyDeviceToDevice, st);
         cudaFreeAsync(scr, st);
         cudaError_t e = cudaGetLastError();
         if (rc == B2K_OK && e != cudaSuccess) rc = b2k_cuda_fail(e, "tail tile of a tree kernel");
@@ -985,13 +1108,22 @@ static int tree_run(const char *fn, b2k_tree_t t, int mode, int dtype, const voi
 extern "C" int b2k_tree_rne(b2k_tree_t t, int dtype, const void *q, const void *qd, const void *qdd, int64_t N, const double *grav,
                             void *tau, void *stream)
 {
-    return tree_run("b2k_tree_rne", t, B2K_GEN_RNE, dtype, q, qd, qdd, N, grav, tau, stream);
+    void *const out[3] = {tau, nullptr, nullptr};
+    return tree_run("b2k_tree_rne", t, B2K_GEN_RNE, false, dtype, q, qd, qdd, N, grav, out, stream);
 }
 
 extern "C" int b2k_tree_dyn(b2k_tree_t t, int op, int dtype, const void *in0, const void *in1, const void *in2, int64_t N,
                             const double *grav, void *out, void *stream)
 {
-    return tree_run("b2k_tree_dyn", t, op, dtype, in0, in1, in2, N, grav, out, stream);
+    void *const outs[3] = {out, nullptr, nullptr};
+    return tree_run("b2k_tree_dyn", t, op, false, dtype, in0, in1, in2, N, grav, outs, stream);
+}
+
+extern "C" int b2k_tree_derivatives(b2k_tree_t t, int op, int dtype, const void *q, const void *qd, const void *x, int64_t N,
+                                    const double *grav, void *out0, void *out1, void *out2, void *stream)
+{
+    void *const outs[3] = {out0, out1, out2};
+    return tree_run("b2k_tree_derivatives", t, op, true, dtype, q, qd, x, N, grav, outs, stream);
 }
 
 extern "C" int b2k_tree_codegen(b2k_tree_t t, int op, int grav_mask, char *src, int64_t src_cap, double *consts, int32_t consts_cap,
@@ -1018,12 +1150,19 @@ extern "C" int b2k_tree_codegen(b2k_tree_t t, int op, int grav_mask, char *src, 
 extern "C" int b2k_tree_info(b2k_tree_t t, int op, int dtype, const double *grav, char *buf, int64_t cap)
 {
     if (!t || !buf || cap < 1) { b2k_set_error("b2k_tree_info: bad arguments"); return B2K_ERR_INVALID; }
-    if (op < B2K_GEN_RNE || op > B2K_GEN_ACCEL) { b2k_set_error("b2k_tree_info: operation %d is not one of B2K_DYN_*", op); return B2K_ERR_INVALID; }
+    if (op < B2K_GEN_RNE || op > B2K_GEN_ACCEL_DERIV || op == B2K_GEN_RNE_WRENCH) {
+        b2k_set_error("b2k_tree_info: operation %d is not one of B2K_DYN_*", op);
+        return B2K_ERR_INVALID;
+    }
     Program *p = tree_program(t, op, dtype, B2K_RNE_OPS[op].grav ? grav_mask_of(grav) : 0);
     if (!p || !p->ok) snprintf(buf, (size_t)cap, "unavailable (%s)", p ? p->why.c_str() : "no cache");
     else if (op == B2K_GEN_RNE)
         snprintf(buf, (size_t)cap, "k_rne_spec<%s,tree n=%d>: %d mul + %d fma + %d add per row, %d constants, %d regs, %zu B smem/block",
                  dtype == B2K_F64 ? "double" : "float", t->n, p->n_mul, p->n_fma, p->n_add, p->nc, p->regs, p->smem);
+    else if (p->nblk)
+        snprintf(buf, (size_t)cap, "%s<%s,tree n=%d,mode=%d>: %d mul + %d fma + %d add per row, %d constants, %d regs, %zu B smem/block, "
+                 "%d warps/block",
+                 p->entry, dtype == B2K_F64 ? "double" : "float", t->n, op, p->n_mul, p->n_fma, p->n_add, p->nc, p->regs, p->smem, p->wpb);
     else
         snprintf(buf, (size_t)cap, "k_rne_spec<%s,tree n=%d,mode=%d>: %d mul + %d fma + %d add per row, %d constants, %d regs, %zu B smem/block",
                  dtype == B2K_F64 ? "double" : "float", t->n, op, p->n_mul, p->n_fma, p->n_add, p->nc, p->regs, p->smem);

@@ -292,6 +292,69 @@ if want("tree_"):
                        Nd, (6 * nin + nout) * es, {"recursions_per_row": recs, "kernel": trob.rne_kernel_info(dt, op=op)})
                 del out
         del bufs, tau
+    # Exact derivatives of the same tree (generated tangent recursion, b2k_tree_derivatives), N rows.  Algorithmic bytes
+    # per row: rne_derivatives (3n + 2n^2) es, accel_derivatives (3n + 3n^2) es.  fd_route is what a user has without
+    # them, timed in the same call on the same rows: one-sided differences, 2n + 1 b2k_tree_rne launches (inverse mode) and
+    # 3n + 1 b2k_tree_dyn(ACCEL) launches (forward mode: the base point and one perturbation of each q, qd, torque entry).
+    # The card's name and power limit are read in the same run.
+    TD_CASES = [f"tree_{op}_derivs_puma_{t}" for op in ("rne", "accel") for t in ("f64", "f32")]
+    if any(want(c) for c in TD_CASES):
+        import subprocess
+
+        try:
+            plim = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True,
+                                  text=True, timeout=30).stdout.strip()
+        except Exception as e:  # the figure is context, the timing does not depend on it
+            plim = f"unavailable ({type(e).__name__})"
+        card = {"gpu": torch.cuda.get_device_name(0), "power_limit": plim}
+        L = rtb._lib.lib()
+        h = trob._tree_handle()
+        st = torch.cuda.current_stream().cuda_stream
+        ag = np.ascontiguousarray(-trob.gravity)
+        n = 6
+        rngt = np.random.default_rng(14)
+        for dt in (np.float64, np.float32):
+            tag = "f64" if dt == np.float64 else "f32"
+            c_rne, c_acc = f"tree_rne_derivs_puma_{tag}", f"tree_accel_derivs_puma_{tag}"
+            if not (want(c_rne) or want(c_acc)):
+                continue
+            es = np.dtype(dt).itemsize
+            code = rtb._lib.F64 if dt == np.float64 else rtb._lib.F32
+            tt = torch.float64 if dt == np.float64 else torch.float32
+            q0, qd0, x0 = (torch.from_numpy(rngt.uniform(-2, 2, (N, n)).astype(dt)).to(dev) for _ in range(3))
+            o = [torch.empty((N, n, n), dtype=tt, device=dev) for _ in range(3)]
+            hstep = 1e-6 if dt == np.float64 else 1e-2
+            for case, op, npert in ((c_rne, 7, 2), (c_acc, 8, 3)):
+                if not want(case):
+                    continue
+                pert = []
+                for k in range(n):
+                    e = torch.zeros(n, dtype=tt, device=dev)
+                    e[k] = hstep
+                    pert += [(q0 + e, qd0, x0), (q0, qd0 + e, x0)] + ([(q0, qd0, x0 + e)] if npert == 3 else [])
+                pert.append((q0, qd0, x0))
+                outs = [torch.empty((N, n), dtype=tt, device=dev) for _ in pert]
+
+                def fd_route(i, op=op, pert=pert, outs=outs):
+                    for (a, b, c), t in zip(pert, outs):
+                        if op == 7:
+                            rtb._lib.check(L.b2k_tree_rne(h, code, a.data_ptr(), b.data_ptr(), c.data_ptr(), N, rtb._lib.dptr(ag), t.data_ptr(), st))
+                        else:
+                            rtb._lib.check(L.b2k_tree_dyn(h, 5, code, a.data_ptr(), b.data_ptr(), c.data_ptr(), N, rtb._lib.dptr(ag), t.data_ptr(), st))
+
+                # alternate the two routes, so that both see the same clocks
+                ms_fd, ms = [], []
+                for _ in range(2):
+                    ms_fd.append(timeit(fd_route, 1))
+                    ms.append(timeit(lambda i, op=op: rtb._lib.check(L.b2k_tree_derivatives(
+                        h, op, code, q0.data_ptr(), qd0.data_ptr(), x0.data_ptr(), N, rtb._lib.dptr(ag), o[0].data_ptr(), o[1].data_ptr(),
+                        o[2].data_ptr() if op == 8 else None, st)), 1))
+                ms_fd, ms = min(ms_fd), min(ms)
+                report(case, ms, N, (3 * n + npert * n * n) * es,
+                       dict(card, frac_of_3p35TBps=round((3 * n + npert * n * n) * es * N / (ms * 1e-3) / 3.35e12, 4), fd_route_ms=round(ms_fd, 4), fd_route_launches=len(pert), speedup_vs_fd_route=round(ms_fd / ms, 2),
+                            kernel=trob.rne_kernel_info(dt, op="rne_derivatives" if op == 7 else "accel_derivatives")))
+                del pert, outs
+            del q0, qd0, x0, o
 
 # forward-dynamics ensemble: friction-free Puma falling from qn for 0.5 s, rtol 1e-6, one lane per trajectory
 if want("fdyn_"):
