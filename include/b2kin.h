@@ -455,6 +455,16 @@ int b2k_opspace_xdd(int dtype, int n, const void *Ja, const void *qdd, const voi
  * any CUDA call, and N = 0 returns without touching the device. */
 int b2k_ikine_6s(int dtype, const double *dh, const double *base, const double *tool, const void *T, int64_t N, int nconf,
                  const int32_t *conf, void *q, int32_t *ok, void *stream);
+/* b2k_ikine_ur is the same for UR-type arms (DHRobot.ikine_ur; the reference has no counterpart): the analytic joint
+ * solution of a standard-DH 6R arm whose axes 2, 3 and 4 are parallel, one pose per row, no iteration.
+ *   dh   the pattern, each condition to 1e-9: alpha = (+pi/2, 0, 0, +pi/2, -pi/2, any), a1 = a4 = a5 = 0, a2 != 0,
+ *        a3 != 0.  d2, d3 and d4 enter only through their sum.  Anything else is B2K_ERR_INVALID.
+ *   conf bit 0 set = shoulder right ("r": O5 . x1 >= 0), bit 1 set = elbow down ("d"; "u" = the elbow above the
+ *        shoulder-O4 line, base z up), bit 2 set = wrist flipped ("f"; "n" = sin(theta5) >= 0)
+ *   base, tool, T, q, ok, the validation and the N = 0 rule as for b2k_ikine_6s.  A row is out of reach when its O5 is
+ *        nearer the first axis than |d2 + d3 + d4| or when the elbow cosine exceeds 1 by more than 64 eps of dtype. */
+int b2k_ikine_ur(int dtype, const double *dh, const double *base, const double *tool, const void *T, int64_t N, int nconf,
+                 const int32_t *conf, void *q, int32_t *ok, void *stream);
 
 /* ---------------------------------------------------------------- pure functions of the Jacobian
  * The six functions below take a batch of Jacobians J (N,6,n), n = 1..B2K_MAX_JOINTS.  J, qd and the output must be

@@ -4,7 +4,8 @@ through the batched RNE kernel.
 Mirrors the hot-path part of the reference's ``DHRobot`` (reference
 src/roboticstoolbox/robot/DHRobot.py): ``ets()`` 878-918, ``fkine`` 920-979, ``jacobe`` 1066-1140,
 ``jacob0`` 1142-1198, ``rne`` 1373-1456 with its parameter packing ``_init_rne`` 1340-1361 and
-dirty tracking (DHLink.py:24-51), ``ikine_LM`` 2454-2474, and the closed-form ``ikine_6s`` as ``ikine_a``.
+dirty tracking (DHLink.py:24-51), ``ikine_LM`` 2454-2474, and the closed-form ``ikine_6s`` as ``ikine_a``; ``ikine_ur``
+is the closed form of UR-type arms, which the reference lacks.
 """
 from __future__ import annotations
 
@@ -187,7 +188,8 @@ class DHRobot:
         q1, q2 = self.ikine_LM(T1, **kwargs), self.ikine_LM(T2, **kwargs)
         return _jtraj(q1.q, q2.q, t, device=device)
 
-    # ---- closed-form inverse kinematics (reference DHRobot.ikine_6s, which Puma560.ikine_a calls): csrc/b2k_ik6s.cu
+    # ---- closed-form inverse kinematics (reference DHRobot.ikine_6s, which Puma560.ikine_a calls; and UR-type arms):
+    # csrc/b2k_ik6s.cu
     _IKINE_A_LETTERS = ("lr", "ud", "nf")
 
     @staticmethod
@@ -209,17 +211,18 @@ class DHRobot:
             out += given.pop() if given else pair[0]
         return out
 
-    def _ikine_a_table(self) -> np.ndarray:
-        """(6,4) rows of (d, a, alpha, offset) for b2k_ikine_6s, after the checks its table cannot express"""
+    def _ikine_a_table(self, method="ikine_a") -> np.ndarray:
+        """(6,4) rows of (d, a, alpha, offset) for b2k_ikine_6s / b2k_ikine_ur, after the checks their tables cannot
+        express; ``method`` names the caller in the messages"""
         if self.n != 6:
-            raise ValueError(f"ikine_a: the closed form serves 6-joint arms; this robot has {self.n} joints")
+            raise ValueError(f"{method}: the closed form serves 6-joint arms; this robot has {self.n} joints")
         if self.mdh:
-            raise ValueError("ikine_a: the closed form serves standard DH; this robot uses modified DH")
+            raise ValueError(f"{method}: the closed form serves standard DH; this robot uses modified DH")
         for j, l in enumerate(self.links):
             if not l.isrevolute:
-                raise ValueError(f"ikine_a: joint {j + 1} is prismatic; the closed form needs revolute joints")
+                raise ValueError(f"{method}: joint {j + 1} is prismatic; the closed form needs revolute joints")
             if l.flip:
-                raise ValueError(f"ikine_a: joint {j + 1} is flipped; the closed form needs unflipped joints")
+                raise ValueError(f"{method}: joint {j + 1} is flipped; the closed form needs unflipped joints")
         return np.ascontiguousarray([[l.d, l.a, l.alpha, l.offset] for l in self.links], dtype=np.float64)
 
     def ikine_a(self, T, config="lun", dtype=None) -> IKSolution:
@@ -233,22 +236,39 @@ class DHRobot:
         One pose gives ``IKSolution(q (6,), success, reason="Success" | "Out of reach")``; a batch q (N,6) with NaN
         rows where the pose is out of reach, success = every row reachable.  A sequence of configurations makes q
         (k,6) / (N,k,6).  numpy in gives numpy out, a CUDA tensor gives q on its device.  Joint limits are not applied."""
+        return self._ikine_closed(T, config, dtype, "b2k_ikine_6s", "ikine_a")
+
+    def ikine_ur(self, T, config="lun", dtype=None) -> IKSolution:
+        """Analytic inverse kinematics of a UR-type 6R arm (Universal Robots UR3 / UR5 / UR10 and any arm of their link
+        pattern): the exact joint solution for a shoulder (l / r), elbow (u / d) and wrist (n / f) configuration, up to
+        eight per pose, with no iteration.
+
+        The robot must be a standard-DH, all-revolute, unflipped 6-joint arm with alpha = (pi/2, 0, 0, pi/2, -pi/2, any),
+        a1 = a4 = a5 = 0, a2 != 0 and a3 != 0; any other robot raises ValueError naming what breaks the pattern.  d1 ..
+        d6, a6, alpha6, the offsets, the base and the tool are free.  The letters are predicates of the solution, in the
+        frame of link 1 with X = a2 c2 + a3 c23 and Y = a2 s2 + a3 s23 the position of the wrist's first joint (O4):
+        ``r`` iff O5 . x1 >= 0 (as for Puma arms), ``u`` iff the elbow lies above the shoulder-O4 line with the base z
+        axis up, sign(X) (X a2 s2 - Y a2 c2) > 0, and ``n`` iff sin(theta5) >= 0.  Inputs, outputs, shapes, dtypes,
+        placement and the reason strings are those of :meth:`ikine_a`.  Joint limits are not applied."""
+        return self._ikine_closed(T, config, dtype, "b2k_ikine_ur", "ikine_ur")
+
+    def _ikine_closed(self, T, config, dtype, entry, method) -> IKSolution:
+        """The body of ikine_a and ikine_ur: ``entry`` is the C entry point, ``method`` names the caller in messages"""
         configs = [config] if isinstance(config, str) else list(config)
         if not 1 <= len(configs) <= 8:
-            raise ValueError(f"ikine_a: give 1 to 8 configurations, got {len(configs)}")
+            raise ValueError(f"{method}: give 1 to 8 configurations, got {len(configs)}")
         codes = []
         for c in configs:
             v = self.config_validate(c, self._IKINE_A_LETTERS)
             codes.append(int(v[0] == "r") | int(v[1] == "d") << 1 | int(v[2] == "f") << 2)
         conf = np.array(codes, dtype=np.int32)
-        dh = self._ikine_a_table()
+        dh = self._ikine_a_table(method)
         base = None if np.array_equal(self._base, np.eye(4)) else np.ascontiguousarray(self._base)
         tool = None if np.array_equal(self._tool, np.eye(4)) else np.ascontiguousarray(self._tool)
-        L = _lib.lib()
+        solve = getattr(_lib.lib(), entry)
         cp = conf.ctypes.data_as(_lib.ip)
         # the link pattern is checked by the C entry point; N = 0 validates without touching a device
-        _lib.check(L.b2k_ikine_6s(_lib.F64, _lib.dptr(dh), _lib.dptr(base), _lib.dptr(tool), None, 0, len(conf), cp, None,
-                                  None, None))
+        _lib.check(solve(_lib.F64, _lib.dptr(dh), _lib.dptr(base), _lib.dptr(tool), None, 0, len(conf), cp, None, None, None))
         T = getattr(T, "A", T)
         B.check_numeric(T, "T")
         if not B.is_tensor(T):
@@ -261,8 +281,8 @@ class DHRobot:
         N, k = Td.shape[0], len(conf)
         q = B.empty((N, k, 6), dt, like=Td)
         ok = B.empty_i32((N, k), like=Td)
-        _lib.check(L.b2k_ikine_6s(B.code(dt), _lib.dptr(dh), _lib.dptr(base), _lib.dptr(tool), B.ptr(Td), N, k, cp, B.ptr(q),
-                                  B.ptr(ok), B.stream_ptr(Td)))
+        _lib.check(solve(B.code(dt), _lib.dptr(dh), _lib.dptr(base), _lib.dptr(tool), B.ptr(Td), N, k, cp, B.ptr(q), B.ptr(ok),
+                         B.stream_ptr(Td)))
         reached = B.to_host(ok).astype(bool)
         if not B.is_tensor(T):
             q = B.to_host(q)

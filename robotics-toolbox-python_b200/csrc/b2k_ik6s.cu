@@ -1,13 +1,20 @@
-// b2k_ik6s.cu -- closed-form inverse kinematics of a Puma-type 6R arm: the reference's DHRobot.ikine_6s (Puma560.ikine_a)
-// over a batch of poses, every requested shoulder / elbow / wrist configuration from one read of each pose.
+// b2k_ik6s.cu -- closed-form inverse kinematics of 6R arms over a batch of poses, every requested shoulder / elbow /
+// wrist configuration from one read of each pose: Puma-type arms with a spherical wrist (k_ikine_6s, the reference's
+// DHRobot.ikine_6s / Puma560.ikine_a) and UR-type arms with three parallel axes (k_ikine_ur, DHRobot.ikine_ur).
 //
 // One lane per row, 64-thread blocks.  Each warp stages its 32 poses through shared memory with 16-byte loads (odd row
 // pitch, so the lanes then read their own rows without bank conflicts), and the same stage then collects the (nconf, 6)
-// joint rows and the ok flags so that they leave coalesced.  Per row the wrist centre W = base^-1 T tool^-1 Tt^-1, its
-// distance r from the first axis and atan2(Py, Px) are formed once; per shoulder theta1, V, the elbow cosine and
-// Rz(theta1)^T R(W); per configuration the rest.  With the pattern's twists R(A1 A2 A3) = Rz(theta1) Ry(-(theta2 +
-// theta3)), so R(A1 A2 A3)^T R(W) is two plane rotations of R(W), not three link products.  DESIGN (f-6) states the
-// algorithm and what the configuration letters mean.
+// joint rows and the ok flags so that they leave coalesced (ik6_tile).  Both arms work in the folded frame
+// W = base^-1 T tool^-1 Tt^-1, Tt = transl(a6, 0, d6) Rx(alpha6), folded on the host into two constant 3x4 matrices.
+//
+// Puma: per row the wrist centre W, its distance r from the first axis and atan2(Py, Px) are formed once; per shoulder
+// theta1, V, the elbow cosine and Rz(theta1)^T R(W); per configuration the rest.  With the pattern's twists
+// R(A1 A2 A3) = Rz(theta1) Ry(-(theta2 + theta3)), so R(A1 A2 A3)^T R(W) is two plane rotations of R(W), not three link
+// products.  DESIGN (f-6) states the algorithm and what the configuration letters mean.
+//
+// UR: W = A1 ... A5 Rz(theta6), so W's origin is O5.  Per row r and atan2(Py, Px); per shoulder theta1 and the first
+// joint axis z1 in W's columns, (u, v, w) = (s5 c6, -s5 s6, c5); per configuration theta5 and theta6 from (u, v, w),
+// then O4 and the axis x4, which reduce the parallel axes 2, 3 and 4 to a planar two-link problem.  DESIGN (f-15).
 #include <math.h>
 
 #include "b2k_common.cuh"
@@ -27,6 +34,19 @@ struct Ik6sP {
     int wrist_neg; // alpha4 > 0: theta5 is the negated tr2eul theta
     int conf[8];
     int vec;       // T is 16-byte aligned
+    long long nrows;
+};
+
+template <typename real>
+struct IkurP {
+    real Bi[12];           // base^-1, 3x4 row-major
+    real Ei[12];           // tool^-1 Tt^-1, Tt = transl(a6, 0, d6) Rx(alpha6)
+    real d1, D, d5;        // D = d2 + d3 + d4
+    real a2, a3, k3, inv3; // k3 = a2^2 + a3^2, inv3 = 1 / (2 a2 a3)
+    real sign_a23;         // sign(a2 a3)
+    real off[6];
+    int conf[8];
+    int vec;               // T is 16-byte aligned
     long long nrows;
 };
 
@@ -59,7 +79,7 @@ __device__ __forceinline__ real ik6_wrap(real x)
     return w - pi;
 }
 
-// sin and cos of the angles this kernel forms, all below 8 pi in magnitude (or NaN on a row that is out of reach):
+// sin and cos of the angles these kernels form, all below 8 pi in magnitude (or NaN on a row that is out of reach):
 // sincospi needs no Payne-Hanek reduction, whose local array would give the kernel a stack frame
 struct Ik6SinCos {
     __device__ __forceinline__ void operator()(double x, double &s, double &c) const { sincospi(x * 0.31830988618379067, &s, &c); }
@@ -78,9 +98,12 @@ template <> __device__ __forceinline__ void ik6_ld16<float>(const float *p, floa
     o[0] = v.x; o[1] = v.y; o[2] = v.z; o[3] = v.w;
 }
 
-template <typename real, int NC>
-__global__ void __launch_bounds__(32 * B2K_IK6_WARPS) k_ikine_6s(const __grid_constant__ Ik6sP<real> P, const real *__restrict__ T,
-                                                                  real *__restrict__ q, int *__restrict__ ok)
+// One warp's tile of 32 rows: stage the poses, hand each lane the top 3x4 of its pose, let solve(t, qs, oks) write the
+// row's NC joint vectors to qs[6 k + j] and its NC flags to oks[k] in the stage, then store both coalesced.  Idle lanes
+// of a ragged tile solve row 0 into their own stage slots, which are never stored.
+template <typename real, int NC, typename Solve>
+__device__ __forceinline__ void ik6_tile(int vec, long long nrows, const real *__restrict__ T, real *__restrict__ q,
+                                         int *__restrict__ ok, const Solve &solve)
 {
     constexpr int TS = 17;                  // odd pitch of a staged pose row
     constexpr int QW = 6 * NC, QS = QW + 1; // a row of q, and its odd pitch in the stage
@@ -90,13 +113,13 @@ __global__ void __launch_bounds__(32 * B2K_IK6_WARPS) k_ikine_6s(const __grid_co
     __shared__ int okst[B2K_IK6_WARPS][32 * OS];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const long long row0 = ((long long)blockIdx.x * B2K_IK6_WARPS + warp) * 32;
-    if (row0 >= P.nrows) return;
-    const int rows = (int)(P.nrows - row0 < 32 ? P.nrows - row0 : 32);
+    if (row0 >= nrows) return;
+    const int rows = (int)(nrows - row0 < 32 ? nrows - row0 : 32);
     real *st = stage[warp];
     int *so = okst[warp];
 
     const real *src = T + row0 * 16;
-    if (P.vec) {
+    if (vec) {
         constexpr int U = 16 / sizeof(real), UPR = 16 / U; // reals per 16-byte unit, units per pose
         for (int u = lane; u < rows * UPR; u += 32) {
             real v[U];
@@ -109,73 +132,12 @@ __global__ void __launch_bounds__(32 * B2K_IK6_WARPS) k_ikine_6s(const __grid_co
         for (int e = lane; e < rows * 16; e += 32) st[(e >> 4) * TS + (e & 15)] = src[e];
     }
     __syncwarp();
-    const int lr = lane < rows ? lane : 0; // idle lanes of a ragged tile recompute row 0 and store nothing
-    real t[12], M[12], W[12];
+    const int lr = lane < rows ? lane : 0;
+    real t[12];
 #pragma unroll
     for (int k = 0; k < 12; k++) t[k] = st[lr * TS + k];
     __syncwarp(); // the stage now collects the output
-
-    // wrist centre and the quantities every configuration shares
-    ik6_mul34<real>(P.Bi, t, M);
-    ik6_mul34<real>(M, P.Ei, W);
-    const real pi = (real)3.14159265358979323846;
-    const Ik6SinCos sc;
-    const real Px = W[3], Py = W[7], Z = W[11] - P.d1;
-    const real r = hypot(Px, Py);
-    const bool reach = fabs(P.D) <= r;
-    const real phi = r_atan2<real>(Py, Px), s = asin(P.D / r);
-    // per shoulder (index 0 = l, 1 = r): theta1, V, atan2(Z, V), acos of the elbow cosine, Rz(theta1)^T R(W) rows 0 and 1
-    real th1[2], V[2], base2[2], ac[2], m0[2][3], m1[2][3];
-    bool elbow_ok[2];
-#pragma unroll
-    for (int sh = 0; sh < 2; sh++) {
-        th1[sh] = phi + (sh ? s : pi - s);
-        real s1, c1;
-        sc(th1[sh], s1, c1);
-        V[sh] = Px * c1 + Py * s1;
-        const real rho2 = V[sh] * V[sh] + Z * Z;
-        const real c = (P.k2 + rho2) / (P.two_a2 * sqrt(rho2));
-        elbow_ok[sh] = fabs(c) <= 1; // false for NaN and infinity too
-        ac[sh] = P.sign_a2 * acos(c); // so that "u" is the elbow above the shoulder-wrist line for either sign of a2
-        base2[sh] = r_atan2<real>(Z, V[sh]);
-#pragma unroll
-        for (int j = 0; j < 3; j++) {
-            m0[sh][j] = c1 * W[j] + s1 * W[4 + j];
-            m1[sh][j] = c1 * W[4 + j] - s1 * W[j];
-        }
-    }
-
-#pragma unroll 1
-    for (int k = 0; k < NC; k++) {
-        const int code = P.conf[k];
-        const bool right = code & 1, down = code & 2, flip = code & 4;
-        // ternaries, not a run-time index, keep the per-shoulder values in registers
-        const real t1 = right ? th1[1] : th1[0], v = right ? V[1] : V[0];
-        const real th2 = (right ? base2[1] : base2[0]) + (down != right ? (real)1 : (real)-1) * (right ? ac[1] : ac[0]);
-        real s2, c2;
-        sc(th2, s2, c2);
-        const real num = c2 * v + s2 * Z - P.a2, den = c2 * Z - s2 * v;
-        const real th3 = P.beta3 - r_atan2<real>(num, den);
-        real sb, cb;
-        sc(th2 + th3, sb, cb);
-        // R = Ry(theta2 + theta3) Rz(theta1)^T R(W)
-        real R[3][3];
-#pragma unroll
-        for (int j = 0; j < 3; j++) {
-            const real a0 = right ? m0[1][j] : m0[0][j];
-            R[0][j] = cb * a0 + sb * W[8 + j];
-            R[1][j] = right ? m1[1][j] : m1[0][j];
-            R[2][j] = cb * W[8 + j] - sb * a0;
-        }
-        real g[3];
-        if (flip) rot_to_eul<real, true, Ik6SinCos>(R, g);
-        else rot_to_eul<real, false, Ik6SinCos>(R, g);
-        const real th[6] = {t1, th2, th3, g[0], P.wrist_neg ? -g[1] : g[1], g[2]};
-        const bool good = reach && (right ? elbow_ok[1] : elbow_ok[0]);
-#pragma unroll
-        for (int j = 0; j < 6; j++) st[lane * QS + k * 6 + j] = good ? ik6_wrap<real>(th[j] - P.off[j]) : (real)NAN;
-        so[lane * OS + k] = good;
-    }
+    solve(t, st + lane * QS, so + lane * OS);
     __syncwarp();
     real *qd = q + row0 * QW;
     for (int e = lane; e < rows * QW; e += 32) {
@@ -189,6 +151,144 @@ __global__ void __launch_bounds__(32 * B2K_IK6_WARPS) k_ikine_6s(const __grid_co
     }
 }
 
+template <typename real, int NC>
+__global__ void __launch_bounds__(32 * B2K_IK6_WARPS) k_ikine_6s(const __grid_constant__ Ik6sP<real> P, const real *__restrict__ T,
+                                                                  real *__restrict__ q, int *__restrict__ ok)
+{
+    ik6_tile<real, NC>(P.vec, P.nrows, T, q, ok, [&](const real *t, real *qs, int *oks) {
+        real M[12], W[12];
+        // wrist centre and the quantities every configuration shares
+        ik6_mul34<real>(P.Bi, t, M);
+        ik6_mul34<real>(M, P.Ei, W);
+        const real pi = (real)3.14159265358979323846;
+        const Ik6SinCos sc;
+        const real Px = W[3], Py = W[7], Z = W[11] - P.d1;
+        const real r = hypot(Px, Py);
+        const bool reach = fabs(P.D) <= r;
+        const real phi = r_atan2<real>(Py, Px), s = asin(P.D / r);
+        // per shoulder (index 0 = l, 1 = r): theta1, V, atan2(Z, V), acos of the elbow cosine, Rz(theta1)^T R(W) rows 0 and 1
+        real th1[2], V[2], base2[2], ac[2], m0[2][3], m1[2][3];
+        bool elbow_ok[2];
+#pragma unroll
+        for (int sh = 0; sh < 2; sh++) {
+            th1[sh] = phi + (sh ? s : pi - s);
+            real s1, c1;
+            sc(th1[sh], s1, c1);
+            V[sh] = Px * c1 + Py * s1;
+            const real rho2 = V[sh] * V[sh] + Z * Z;
+            const real c = (P.k2 + rho2) / (P.two_a2 * sqrt(rho2));
+            elbow_ok[sh] = fabs(c) <= 1; // false for NaN and infinity too
+            ac[sh] = P.sign_a2 * acos(c); // so that "u" is the elbow above the shoulder-wrist line for either sign of a2
+            base2[sh] = r_atan2<real>(Z, V[sh]);
+#pragma unroll
+            for (int j = 0; j < 3; j++) {
+                m0[sh][j] = c1 * W[j] + s1 * W[4 + j];
+                m1[sh][j] = c1 * W[4 + j] - s1 * W[j];
+            }
+        }
+
+#pragma unroll 1
+        for (int k = 0; k < NC; k++) {
+            const int code = P.conf[k];
+            const bool right = code & 1, down = code & 2, flip = code & 4;
+            // ternaries, not a run-time index, keep the per-shoulder values in registers
+            const real t1 = right ? th1[1] : th1[0], v = right ? V[1] : V[0];
+            const real th2 = (right ? base2[1] : base2[0]) + (down != right ? (real)1 : (real)-1) * (right ? ac[1] : ac[0]);
+            real s2, c2;
+            sc(th2, s2, c2);
+            const real num = c2 * v + s2 * Z - P.a2, den = c2 * Z - s2 * v;
+            const real th3 = P.beta3 - r_atan2<real>(num, den);
+            real sb, cb;
+            sc(th2 + th3, sb, cb);
+            // R = Ry(theta2 + theta3) Rz(theta1)^T R(W)
+            real R[3][3];
+#pragma unroll
+            for (int j = 0; j < 3; j++) {
+                const real a0 = right ? m0[1][j] : m0[0][j];
+                R[0][j] = cb * a0 + sb * W[8 + j];
+                R[1][j] = right ? m1[1][j] : m1[0][j];
+                R[2][j] = cb * W[8 + j] - sb * a0;
+            }
+            real g[3];
+            if (flip) rot_to_eul<real, true, Ik6SinCos>(R, g);
+            else rot_to_eul<real, false, Ik6SinCos>(R, g);
+            const real th[6] = {t1, th2, th3, g[0], P.wrist_neg ? -g[1] : g[1], g[2]};
+            const bool good = reach && (right ? elbow_ok[1] : elbow_ok[0]);
+#pragma unroll
+            for (int j = 0; j < 6; j++) qs[k * 6 + j] = good ? ik6_wrap<real>(th[j] - P.off[j]) : (real)NAN;
+            oks[k] = good;
+        }
+    });
+}
+
+// |c3| up to 1 + B2K_IKUR_ELBOW_BAND eps of the compute type counts as reached and is clamped to 1: a straight elbow
+// (UR10's qz and qr) has c3 = +-1 only up to the rounding of the fold and of X^2 + Y^2
+#define B2K_IKUR_ELBOW_BAND 64
+
+template <typename real, int NC>
+__global__ void __launch_bounds__(32 * B2K_IK6_WARPS) k_ikine_ur(const __grid_constant__ IkurP<real> P, const real *__restrict__ T,
+                                                                  real *__restrict__ q, int *__restrict__ ok)
+{
+    ik6_tile<real, NC>(P.vec, P.nrows, T, q, ok, [&](const real *t, real *qs, int *oks) {
+        real M[12], W[12]; // W = A1 ... A5 Rz(theta6): columns x', y', z', origin O5
+        ik6_mul34<real>(P.Bi, t, M);
+        ik6_mul34<real>(M, P.Ei, W);
+        const real pi = (real)3.14159265358979323846, eps = r_eps<real>();
+        const Ik6SinCos sc;
+        const real px = W[3], py = W[7], pz = W[11];
+        const real r = hypot(px, py);
+        const bool reach = fabs(P.D) <= r;
+        const real phi = r_atan2<real>(py, px), s = asin(P.D / r);
+        // per shoulder (index 0 = l, 1 = r): theta1, x1 = (c1, s1, 0), and z1 = (s1, -c1, 0) against W's columns
+        real th1[2], c1[2], s1[2], uu[2], vv[2], ww[2];
+#pragma unroll
+        for (int sh = 0; sh < 2; sh++) {
+            th1[sh] = phi + (sh ? s : pi - s);
+            sc(th1[sh], s1[sh], c1[sh]);
+            uu[sh] = W[0] * s1[sh] - W[4] * c1[sh];
+            vv[sh] = W[1] * s1[sh] - W[5] * c1[sh];
+            ww[sh] = W[2] * s1[sh] - W[6] * c1[sh];
+        }
+
+#pragma unroll 1
+        for (int k = 0; k < NC; k++) {
+            const int code = P.conf[k];
+            const bool right = code & 1, down = code & 2, flip = code & 4;
+            // ternaries, not a run-time index, keep the per-shoulder values in registers
+            const real t1 = right ? th1[1] : th1[0], ca = right ? c1[1] : c1[0], sa = right ? s1[1] : s1[0];
+            const real u = right ? uu[1] : uu[0], v = right ? vv[1] : vv[0], w = right ? ww[1] : ww[0];
+            // wrist: (u, v, w) = (s5 c6, -s5 s6, c5), sigma = sign(s5) = +1 for "n", -1 for "f"
+            const real sg = flip ? (real)-1 : (real)1, h = hypot(u, v);
+            const bool sing = fabs(u) < 10 * eps && fabs(v) < 10 * eps; // theta6 = 0, as tr2eul's singular rule
+            const real th5 = r_atan2<real>(sg * h, w), th6 = sing ? (real)0 : r_atan2<real>(-sg * v, sg * u);
+            const real ih = sg / h;
+            const real s5 = sg * h, c5 = w, c6 = sing ? (real)1 : u * ih, s6 = sing ? (real)0 : -v * ih;
+            // the planar problem: O4 = O5 + d5 (s6 x' + c6 y'), X = O4 . x1, Y = O4z - d1; x4 = c5 (c6 x' - s6 y') - s5 z'
+            const real o0 = px + P.d5 * (s6 * W[0] + c6 * W[1]);
+            const real o1 = py + P.d5 * (s6 * W[4] + c6 * W[5]);
+            const real o2 = pz + P.d5 * (s6 * W[8] + c6 * W[9]);
+            const real X = o0 * ca + o1 * sa, Y = o2 - P.d1;
+            const real x40 = c5 * (c6 * W[0] - s6 * W[1]) - s5 * W[2];
+            const real x41 = c5 * (c6 * W[4] - s6 * W[5]) - s5 * W[6];
+            const real x42 = c5 * (c6 * W[8] - s6 * W[9]) - s5 * W[10];
+            const real th234 = r_atan2<real>(x42, x40 * ca + x41 * sa);
+            // elbow: theta3 = -+sign(X) sign(a2 a3) acos(c3) for u / d, with sign(0) = +1
+            const real c3r = (X * X + Y * Y - P.k3) * P.inv3;
+            const bool good = reach && fabs(c3r) <= 1 + B2K_IKUR_ELBOW_BAND * eps; // false for NaN too
+            const real c3 = fmin(fmax(c3r, (real)-1), (real)1);
+            const real sgn3 = ((X >= 0) == down ? (real)1 : (real)-1) * P.sign_a23;
+            const real th3 = sgn3 * acos(c3), s3 = sgn3 * sqrt((1 - c3) * (1 + c3));
+            // theta2 = atan2(Y, X) - atan2(a3 s3, a2 + a3 c3), as one atan2 of the difference
+            const real ex = fma(P.a3, c3, P.a2), ey = P.a3 * s3;
+            const real th2 = r_atan2<real>(Y * ex - X * ey, X * ex + Y * ey);
+            const real th[6] = {t1, th2, th3, th234 - th2 - th3, th5, th6};
+#pragma unroll
+            for (int j = 0; j < 6; j++) qs[k * 6 + j] = good ? ik6_wrap<real>(th[j] - P.off[j]) : (real)NAN;
+            oks[k] = good;
+        }
+    });
+}
+
 // inverse of a rigid 3x4 transform: [R^T | -R^T t]
 void ik6_inv_rigid(const double *A, double *X)
 {
@@ -198,43 +298,10 @@ void ik6_inv_rigid(const double *A, double *X)
     }
 }
 
-template <typename real>
-int ik6_launch(const double *Bi, const double *Ei, const double *dh, const void *T, long long N, int nconf, const int32_t *conf,
-               void *q, int32_t *ok, cudaStream_t st)
+// The checks both entry points make before their link pattern, in this order.  B2K_OK or B2K_ERR_INVALID.
+int ik6_check(const char *fn, int dtype, const double *dh, const void *T, int64_t N, int nconf, const int32_t *conf,
+              const void *q, const int32_t *ok)
 {
-    Ik6sP<real> P;
-    for (int k = 0; k < 12; k++) { P.Bi[k] = (real)Bi[k]; P.Ei[k] = (real)Ei[k]; }
-    const double a2 = dh[1 * 4 + 1], a3 = dh[2 * 4 + 1], d4 = dh[3 * 4 + 0];
-    P.d1 = (real)dh[0];
-    P.D = (real)(dh[1 * 4 + 0] + dh[2 * 4 + 0]);
-    P.a2 = (real)a2;
-    P.k2 = (real)(a2 * a2 - a3 * a3 - d4 * d4);
-    P.two_a2 = (real)(2 * a2);
-    P.beta3 = (real)atan2(a3, d4);
-    P.sign_a2 = a2 > 0 ? (real)1 : (real)-1;
-    for (int j = 0; j < 6; j++) P.off[j] = (real)dh[j * 4 + 3];
-    P.wrist_neg = dh[3 * 4 + 2] > 0;
-    for (int k = 0; k < 8; k++) P.conf[k] = k < nconf ? conf[k] : 0;
-    P.vec = ((uintptr_t)T & 15) == 0;
-    P.nrows = N;
-    const unsigned blocks = (unsigned)((N + 32 * B2K_IK6_WARPS - 1) / (32 * B2K_IK6_WARPS));
-    switch (nconf) {
-#define B2K_CASE(NC) \
-    case NC: k_ikine_6s<real, NC><<<blocks, 32 * B2K_IK6_WARPS, 0, st>>>(P, (const real *)T, (real *)q, (int *)ok); break;
-        B2K_CASE(1) B2K_CASE(2) B2K_CASE(3) B2K_CASE(4) B2K_CASE(5) B2K_CASE(6) B2K_CASE(7) B2K_CASE(8)
-#undef B2K_CASE
-    }
-    b2k_count_launch();
-    B2K_CUDA(cudaGetLastError());
-    return B2K_OK;
-}
-
-} // namespace
-
-extern "C" int b2k_ikine_6s(int dtype, const double *dh, const double *base, const double *tool, const void *T, int64_t N, int nconf,
-                            const int32_t *conf, void *q, int32_t *ok, void *stream)
-{
-    const char *fn = "b2k_ikine_6s";
     if (dtype != B2K_F32 && dtype != B2K_F64) { b2k_set_error("%s: bad dtype", fn); return B2K_ERR_INVALID; }
     if (N < 0) { b2k_set_error("%s: bad N", fn); return B2K_ERR_INVALID; }
     if (nconf < 1 || nconf > 8) { b2k_set_error("%s: nconf must be 1..8, got %d", fn, nconf); return B2K_ERR_INVALID; }
@@ -244,10 +311,113 @@ extern "C" int b2k_ikine_6s(int dtype, const double *dh, const double *base, con
         if (conf[k] < 0 || conf[k] > 7) { b2k_set_error("%s: configuration code %d of slot %d is not 0..7", fn, conf[k], k); return B2K_ERR_INVALID; }
     for (int e = 0; e < 24; e++)
         if (!isfinite(dh[e])) { b2k_set_error("%s: dh[%d][%d] is not finite", fn, e / 4, e % 4); return B2K_ERR_INVALID; }
+    return B2K_OK;
+}
+
+struct Ik6Rule {
+    bool bad;
+    const char *what;
+    double got;
+};
+
+// the first broken rule of a link pattern as "<fn>: not a <arm>-type arm: <what> (got <value>); <needs>"
+template <size_t R>
+int ik6_pattern(const char *fn, const Ik6Rule (&rules)[R], const char *arm, const char *needs)
+{
+    for (const auto &p : rules)
+        if (p.bad) {
+            b2k_set_error("%s: not a %s-type arm: %s (got %.17g); the closed form needs %s", fn, arm, p.what, p.got, needs);
+            return B2K_ERR_INVALID;
+        }
+    return B2K_OK;
+}
+
+// fold the constants on the host in fp64: Bi = base^-1, Ei = tool^-1 Tt^-1 = (Tt tool)^-1, Tt = transl(a6, 0, d6) Rx(alpha6)
+void ik6_fold(const double *dh, const double *base, const double *tool, double *Bi, double *Ei)
+{
+    double Bt[12], E[12], tl[12];
+    b2k_ident34(Bt);
+    if (base) b2k_mat_to34(base, Bt);
+    const double a6 = dh[20 + 1], d6 = dh[20], ca = cos(dh[20 + 2]), sa = sin(dh[20 + 2]);
+    const double Tt[12] = {1, 0, 0, a6, 0, ca, -sa, 0, 0, sa, ca, d6};
+    b2k_ident34(tl);
+    if (tool) b2k_mat_to34(tool, tl);
+    b2k_mul34(Tt, tl, E);
+    ik6_inv_rigid(Bt, Bi);
+    ik6_inv_rigid(E, Ei);
+}
+
+// the fields both parameter blocks have, then one launch of kern[nconf - 1], the instantiation for nconf configurations
+template <typename real, typename Prm>
+int ik6_launch(void (*const kern[8])(Prm, const real *, real *, int *), Prm &P, const double *Bi, const double *Ei,
+               const double *dh, const void *T, long long N, int nconf, const int32_t *conf, void *q, int32_t *ok,
+               cudaStream_t st)
+{
+    for (int k = 0; k < 12; k++) { P.Bi[k] = (real)Bi[k]; P.Ei[k] = (real)Ei[k]; }
+    for (int j = 0; j < 6; j++) P.off[j] = (real)dh[j * 4 + 3];
+    for (int k = 0; k < 8; k++) P.conf[k] = k < nconf ? conf[k] : 0;
+    P.vec = ((uintptr_t)T & 15) == 0;
+    P.nrows = N;
+    const unsigned blocks = (unsigned)((N + 32 * B2K_IK6_WARPS - 1) / (32 * B2K_IK6_WARPS));
+    kern[nconf - 1]<<<blocks, 32 * B2K_IK6_WARPS, 0, st>>>(P, (const real *)T, (real *)q, (int *)ok);
+    b2k_count_launch();
+    B2K_CUDA(cudaGetLastError());
+    return B2K_OK;
+}
+
+template <typename real>
+int ik6s_launch(const double *Bi, const double *Ei, const double *dh, const void *T, long long N, int nconf, const int32_t *conf,
+                void *q, int32_t *ok, cudaStream_t st)
+{
+    static void (*const kern[8])(Ik6sP<real>, const real *, real *, int *) = {
+        k_ikine_6s<real, 1>, k_ikine_6s<real, 2>, k_ikine_6s<real, 3>, k_ikine_6s<real, 4>,
+        k_ikine_6s<real, 5>, k_ikine_6s<real, 6>, k_ikine_6s<real, 7>, k_ikine_6s<real, 8>};
+    Ik6sP<real> P;
+    const double a2 = dh[1 * 4 + 1], a3 = dh[2 * 4 + 1], d4 = dh[3 * 4 + 0];
+    P.d1 = (real)dh[0];
+    P.D = (real)(dh[1 * 4 + 0] + dh[2 * 4 + 0]);
+    P.a2 = (real)a2;
+    P.k2 = (real)(a2 * a2 - a3 * a3 - d4 * d4);
+    P.two_a2 = (real)(2 * a2);
+    P.beta3 = (real)atan2(a3, d4);
+    P.sign_a2 = a2 > 0 ? (real)1 : (real)-1;
+    P.wrist_neg = dh[3 * 4 + 2] > 0;
+    return ik6_launch<real>(kern, P, Bi, Ei, dh, T, N, nconf, conf, q, ok, st);
+}
+
+template <typename real>
+int ikur_launch(const double *Bi, const double *Ei, const double *dh, const void *T, long long N, int nconf, const int32_t *conf,
+                void *q, int32_t *ok, cudaStream_t st)
+{
+    static void (*const kern[8])(IkurP<real>, const real *, real *, int *) = {
+        k_ikine_ur<real, 1>, k_ikine_ur<real, 2>, k_ikine_ur<real, 3>, k_ikine_ur<real, 4>,
+        k_ikine_ur<real, 5>, k_ikine_ur<real, 6>, k_ikine_ur<real, 7>, k_ikine_ur<real, 8>};
+    IkurP<real> P;
+    const double a2 = dh[1 * 4 + 1], a3 = dh[2 * 4 + 1];
+    P.d1 = (real)dh[0];
+    P.D = (real)(dh[1 * 4 + 0] + dh[2 * 4 + 0] + dh[3 * 4 + 0]);
+    P.d5 = (real)dh[4 * 4 + 0];
+    P.a2 = (real)a2;
+    P.a3 = (real)a3;
+    P.k3 = (real)(a2 * a2 + a3 * a3);
+    P.inv3 = (real)(1 / (2 * a2 * a3));
+    P.sign_a23 = a2 * a3 > 0 ? (real)1 : (real)-1;
+    return ik6_launch<real>(kern, P, Bi, Ei, dh, T, N, nconf, conf, q, ok, st);
+}
+
+const double kHalfPi = 1.5707963267948966, kPatternTol = 1e-9;
+
+} // namespace
+
+extern "C" int b2k_ikine_6s(int dtype, const double *dh, const double *base, const double *tool, const void *T, int64_t N, int nconf,
+                            const int32_t *conf, void *q, int32_t *ok, void *stream)
+{
+    const char *fn = "b2k_ikine_6s";
+    if (int rc = ik6_check(fn, dtype, dh, T, N, nconf, conf, q, ok)) return rc;
     // the Puma link pattern, link by link; NaN-safe comparisons
-    const double h = 1.5707963267948966, tol = 1e-9;
+    const double h = kHalfPi, tol = kPatternTol;
     const double *d = dh, *a = dh + 1, *al = dh + 2; // stride 4
-    const struct { bool bad; const char *what; double got; } pattern[] = {
+    const Ik6Rule pattern[] = {
         {!(fabs(al[0] - h) <= tol), "alpha1 must be +pi/2", al[0]},
         {!(fabs(a[0]) <= tol), "a1 must be 0", a[0]},
         {!(fabs(al[4]) <= tol), "alpha2 must be 0", al[4]},
@@ -259,27 +429,44 @@ extern "C" int b2k_ikine_6s(int dtype, const double *dh, const double *base, con
         {!(fabs(a[16]) <= tol), "a5 must be 0", a[16]},
         {!(fabs(d[16]) <= tol), "d5 must be 0", d[16]},
     };
-    for (const auto &p : pattern)
-        if (p.bad) {
-            b2k_set_error("%s: not a Puma-type arm: %s (got %.17g); the closed form needs alpha = (pi/2, 0, -pi/2, +-pi/2, "
-                          "-+pi/2, any), a1 = a4 = a5 = 0, d5 = 0, a2 != 0", fn, p.what, p.got);
-            return B2K_ERR_INVALID;
-        }
+    if (int rc = ik6_pattern(fn, pattern, "Puma", "alpha = (pi/2, 0, -pi/2, +-pi/2, -+pi/2, any), a1 = a4 = a5 = 0, d5 = 0, a2 != 0"))
+        return rc;
     if (N == 0) return B2K_OK;
     B2K_ON_DEVICE_OF(T);
-    // fold the constants on the host in fp64: Bi = base^-1, Ei = tool^-1 Tt^-1 = (Tt tool)^-1
-    double Bt[12], Tt[12], E[12], Bi[12], Ei[12], tl[12];
-    b2k_ident34(Bt);
-    if (base) b2k_mat_to34(base, Bt);
-    const double a6 = a[20], d6 = d[20], ca = cos(al[20]), sa = sin(al[20]);
-    const double Tt_[12] = {1, 0, 0, a6, 0, ca, -sa, 0, 0, sa, ca, d6};
-    for (int k = 0; k < 12; k++) Tt[k] = Tt_[k];
-    b2k_ident34(tl);
-    if (tool) b2k_mat_to34(tool, tl);
-    b2k_mul34(Tt, tl, E);
-    ik6_inv_rigid(Bt, Bi);
-    ik6_inv_rigid(E, Ei);
+    double Bi[12], Ei[12];
+    ik6_fold(dh, base, tool, Bi, Ei);
     cudaStream_t st = (cudaStream_t)stream;
-    return dtype == B2K_F64 ? ik6_launch<double>(Bi, Ei, dh, T, N, nconf, conf, q, ok, st)
-                            : ik6_launch<float>(Bi, Ei, dh, T, N, nconf, conf, q, ok, st);
+    return dtype == B2K_F64 ? ik6s_launch<double>(Bi, Ei, dh, T, N, nconf, conf, q, ok, st)
+                            : ik6s_launch<float>(Bi, Ei, dh, T, N, nconf, conf, q, ok, st);
+}
+
+extern "C" int b2k_ikine_ur(int dtype, const double *dh, const double *base, const double *tool, const void *T, int64_t N, int nconf,
+                            const int32_t *conf, void *q, int32_t *ok, void *stream)
+{
+    const char *fn = "b2k_ikine_ur";
+    if (int rc = ik6_check(fn, dtype, dh, T, N, nconf, conf, q, ok)) return rc;
+    // the UR link pattern, link by link; NaN-safe comparisons
+    const double h = kHalfPi, tol = kPatternTol;
+    const double *a = dh + 1, *al = dh + 2; // stride 4
+    const Ik6Rule pattern[] = {
+        {!(fabs(al[0] - h) <= tol), "alpha1 must be +pi/2", al[0]},
+        {!(fabs(a[0]) <= tol), "a1 must be 0", a[0]},
+        {!(fabs(al[4]) <= tol), "alpha2 must be 0", al[4]},
+        {!(fabs(a[4]) > tol), "a2 must not be 0", a[4]},
+        {!(fabs(al[8]) <= tol), "alpha3 must be 0", al[8]},
+        {!(fabs(a[8]) > tol), "a3 must not be 0", a[8]},
+        {!(fabs(al[12] - h) <= tol), "alpha4 must be +pi/2", al[12]},
+        {!(fabs(a[12]) <= tol), "a4 must be 0", a[12]},
+        {!(fabs(al[16] + h) <= tol), "alpha5 must be -pi/2", al[16]},
+        {!(fabs(a[16]) <= tol), "a5 must be 0", a[16]},
+    };
+    if (int rc = ik6_pattern(fn, pattern, "UR", "alpha = (pi/2, 0, 0, pi/2, -pi/2, any), a1 = a4 = a5 = 0, a2 != 0, a3 != 0"))
+        return rc;
+    if (N == 0) return B2K_OK;
+    B2K_ON_DEVICE_OF(T);
+    double Bi[12], Ei[12];
+    ik6_fold(dh, base, tool, Bi, Ei);
+    cudaStream_t st = (cudaStream_t)stream;
+    return dtype == B2K_F64 ? ikur_launch<double>(Bi, Ei, dh, T, N, nconf, conf, q, ok, st)
+                            : ikur_launch<float>(Bi, Ei, dh, T, N, nconf, conf, q, ok, st);
 }

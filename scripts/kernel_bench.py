@@ -501,6 +501,43 @@ if want("ikine_a_"):
             del qi, oki
     del Tq, T64
 
+# Closed-form IK of UR-type arms (b2k_ikine_ur) of UR10 on device-resident poses, with the bytes per row and the card
+# context of the ikine_a_ block above, so that `--only ikine_` times both kernels in one run.
+if want("ikine_ur_"):
+    import subprocess
+
+    try:
+        plim = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True,
+                              text=True, timeout=30).stdout.strip()
+    except Exception as e:  # the figure is context, the timing does not depend on it
+        plim = f"unavailable ({type(e).__name__})"
+    card = {"gpu": torch.cuda.get_device_name(0), "power_limit": plim}
+    ur10 = rtb.models.UR10()
+    NI = args.rows
+    Tq = torch.from_numpy(rng.uniform(-np.pi, np.pi, (NI, 6))).to(dev)
+    T64 = ur10.ets().eval(Tq)
+    Li = rtb._lib.lib()
+    sti = torch.cuda.current_stream().cuda_stream
+    dhi = np.ascontiguousarray([[l.d, l.a, l.alpha, l.offset] for l in ur10.links], dtype=np.float64)
+    for dt, tag in ((np.float64, "f64"), (np.float32, "f32")):
+        Ti = T64 if dt == np.float64 else T64.float()
+        sz = np.dtype(dt).itemsize
+        for nc, bpr in ((1, (16 + 6) * sz + 4), (8, 16 * sz + 8 * (6 * sz + 4))):
+            case = f"ikine_ur_ur10_{nc}conf_{tag}"
+            if not want(case):
+                continue
+            conf = np.arange(nc, dtype=np.int32)
+            qi = torch.empty((NI, nc, 6), dtype=Ti.dtype, device=dev)
+            oki = torch.empty((NI, nc), dtype=torch.int32, device=dev)
+            code = rtb._lib.F64 if dt == np.float64 else rtb._lib.F32
+            ms = timeit(lambda i: rtb._lib.check(Li.b2k_ikine_ur(code, rtb._lib.dptr(dhi), None, None, Ti.data_ptr(), NI, nc,
+                                                                 conf.ctypes.data_as(rtb._lib.ip), qi.data_ptr(), oki.data_ptr(),
+                                                                 sti)), 1)
+            report(case, ms, NI, bpr, dict(card, api="C ABI, poses on the device", frac_of_3350=round(bpr * NI / (ms * 1e-3) / 3.35e12, 4),
+                                           solved=float(oki.float().mean())))
+            del qi, oki
+    del Tq, T64
+
 # IK (config 4): reachable targets, chan
 if want("ik_"):
     panda = rtb.models.Panda().ets()
