@@ -365,6 +365,28 @@ int b2k_rne_derivatives(b2k_rne_t rne, int dtype, const void *q, const void *qd,
 int b2k_rne_accel_derivatives(b2k_rne_t rne, int dtype, const void *q, const void *qd, const void *torque, int64_t N,
                               const double *grav, void *dqdd_dq, void *dqdd_dqd, void *dqdd_dtau, void *stream);
 
+/* The dynamics regressor, for identifying a DH arm's link parameters from logged (q, qd, qdd, tau):
+ * tau = Y(q, qd, qdd; g) pi with no tip wrench, for every link table rne serves (prismatic joints through d = q + offset,
+ * the modified-DH prismatic first joint as rne treats it, flip ignored).  pi has p = 14 n entries, link-major, 14 per
+ * link j:  pi[14j .. 14j+13] = [m, m rx, m ry, m rz, Ixx, Iyy, Izz, Ixy, Iyz, Ixz, Jm, B, Tc+, Tc-]
+ * r is the link's centre of mass in its frame (as rne takes it); the six inertia entries, in the order of the 6-vector
+ * form of a link's I, are those of I_o = I + m (r.r E - r r^T), the inertia about the link-frame origin.  The gear ratio
+ * G is a known constant: the columns of Jm_j, B_j, Tc+_j, Tc-_j are G_j^2 qdd_j, G_j^2 qd_j, |G_j| [qd_j > 0],
+ * |G_j| [qd_j < 0] in row j and 0 elsewhere; Y[j, 14i + k] = 0 for i < j.  These zeros are written as exact 0.
+ *   b2k_rne_regressor       Y (N, n, 14n) row-major, one launch; grav = MINUS the robot's gravity, as b2k_rne.
+ *                           The arrays follow the rules above (Y's row is 14 n^2 reals).
+ *   b2k_rne_regressor_gram  the normal equations without Y existing in full, always in fp64:
+ *                           G (p, p) = sum Y^T W Y, b (p) = sum Y^T W tau, s (1) = sum tau^T W tau over the N rows,
+ *                           W = diag(weights) (host, n values, finite and >= 0; NULL = all 1).  tau (N, n) has the
+ *                           compute type.  G is exactly symmetric, and no atomics are used: equal calls give equal bits.
+ *                           G, b, s are device arrays, 8-byte aligned, written also for N = 0 (zeros, no kernel).
+ * Every argument is checked before any CUDA call.  No reference counterpart. */
+int b2k_rne_regressor(b2k_rne_t rne, int dtype, const void *q, const void *qd, const void *qdd, int64_t N,
+                      const double *grav, void *Y, void *stream);
+int b2k_rne_regressor_gram(b2k_rne_t rne, int dtype, const void *q, const void *qd, const void *qdd, const void *tau,
+                           int64_t N, const double *grav, const double *weights, double *G, double *b, double *s,
+                           void *stream);
+
 /* ---------------------------------------------------------------- static forces (DynamicsMixin, robot/Dynamics.py)
  * One forward walk over a compiled chain per row (base and tool as the chain has them, as for b2k_jacob0); q is (N, ldq)
  * with the joint coordinates at the chain's joint indices.  Unlike b2k_rne, `grav` is the world-frame gravity AS THE

@@ -10,6 +10,7 @@ is the closed form of UR-type arms, which the reference lacks.
 from __future__ import annotations
 
 import ctypes as C
+from collections import namedtuple
 from typing import List, Optional
 
 import numpy as np
@@ -23,6 +24,9 @@ from .DHLink import DHLink
 from .ET import ET
 from .ETS import ETS, _mat44
 from .IK import IKSolution
+
+
+IdentifyResult = namedtuple("IdentifyResult", "pi rank rms")
 
 
 class DHRobot:
@@ -502,11 +506,13 @@ class DHRobot:
         """Which kernel serves `op` for this robot: the robot-specialised one (generated from the link table and
         compiled with NVRTC at first use; the line lists its multiply / FMA / add count per row, registers and
         shared memory) or the pre-compiled generic one, with the reason."""
-        if op in self._DERIV_OPS:
+        if op in self._DERIV_OPS or op == "rne_regressor":
             allrev = all(l.sigma == 0 for l in self.links)
-            return (f"generic k_rne_deriv<{'double' if np.dtype(dtype) == np.float64 else 'float'}, n={self.n}, {'MDH' if self.mdh else 'DH'}, "
-                    f"{'all-revolute' if allrev else 'prismatic'}, {self._DERIV_OPS[op]}> (the robot-specialised path "
-                    "generates no derivative kernels)")
+            shape = (f"{'double' if np.dtype(dtype) == np.float64 else 'float'}, n={self.n}, {'MDH' if self.mdh else 'DH'}, "
+                     f"{'all-revolute' if allrev else 'prismatic'}")
+            if op == "rne_regressor":
+                return f"generic k_rne_regressor<{shape}> (the robot-specialised path generates no regressor kernels)"
+            return f"generic k_rne_deriv<{shape}, {self._DERIV_OPS[op]}> (the robot-specialised path generates no derivative kernels)"
         h = self._rne_handle()
         g = self._kernel_gravity(gravity)
         buf = C.create_string_buffer(2048)
@@ -515,10 +521,9 @@ class DHRobot:
         return buf.value.decode()
 
     # ---- dynamics built on the recursion (reference DynamicsMixin, Dynamics.py; SURVEY 8f-1)
-    def _dyn(self, fn_name, ins, out_tail, gravity=None, use_gravity=False, dtype=None, fext=None, use_fext=False, n_out=1):
-        """Shared front end of the fan-out kernels: every input (N,n) or (n,), one launch.  With n_out > 1 the kernel
-        writes that many outputs of the same shape, returned as a tuple."""
-        h = self._rne_handle()
+    def _dyn_inputs(self, ins, dtype):
+        """The inputs of a batched dynamics call as contiguous (N, n) device tensors of one dtype: returns (dtype,
+        whether the inputs were host arrays, whether they were single (n,) states, the tensors, N)."""
         n = self.n
         for x in ins:
             B.check_numeric(x)
@@ -534,6 +539,14 @@ class DHRobot:
         for t in dev:
             if t.dim() != 2 or tuple(t.shape) != (N, n):
                 raise ValueError(f"inputs must have shape ({n},) or (N,{n}); got {tuple(t.shape)}")
+        return dt, host, single, dev, N
+
+    def _dyn(self, fn_name, ins, out_tail, gravity=None, use_gravity=False, dtype=None, fext=None, use_fext=False, n_out=1):
+        """Shared front end of the fan-out kernels: every input (N,n) or (n,), one launch.  With n_out > 1 the kernel
+        writes that many outputs of the same shape, returned as a tuple."""
+        h = self._rne_handle()
+        n = self.n
+        dt, host, single, dev, N = self._dyn_inputs(ins, dtype)
         outs = [B.empty((N,) + out_tail, dt, like=dev[0]) for _ in range(n_out)]
         args = [h, B.code(dt)] + [B.ptr(t) for t in dev] + [N]
         if use_gravity:
@@ -593,6 +606,98 @@ class DHRobot:
         and ``dqdd_dtau = M^-1``.  All three come from one kernel launch."""
         return self._dyn("b2k_rne_accel_derivatives", [q, qd, torque], (self.n, self.n), gravity=gravity, use_gravity=True,
                          dtype=dtype, n_out=3)
+
+    # ---- parameter identification: the dynamics regressor (DESIGN f-16; no reference counterpart)
+    def dynamic_parameters(self) -> np.ndarray:
+        """The (14n,) float64 parameter vector pi of the current links, the one ``rne_regressor`` multiplies: 14 per link,
+        link-major, ``[m, m rx, m ry, m rz, Ixx, Iyy, Izz, Ixy, Iyz, Ixz, Jm, B, Tc+, Tc-]``.  r is the link's centre of
+        mass in its frame; the inertia entries are those of I_o = I + m (r.r E - r r^T), the link's inertia moved to the
+        link-frame origin, in the order of the 6-vector form of ``I``.  The symmetric part of ``I`` is used: the link
+        setter rejects an asymmetry above 1e-8, and ``rne_regressor(...) @ dynamic_parameters() == rne(...)`` holds up
+        to that asymmetry.  The gear ratio G is not a parameter."""
+        pi = np.zeros(14 * self.n)
+        for j, l in enumerate(self.links):
+            m, r = float(l.m), np.asarray(l.r, dtype=np.float64)
+            Io = 0.5 * (l.I + l.I.T) + m * (r @ r * np.eye(3) - np.outer(r, r))
+            pi[14 * j:14 * j + 14] = (m, *(m * r), Io[0, 0], Io[1, 1], Io[2, 2], Io[0, 1], Io[1, 2], Io[0, 2], l.Jm, l.B,
+                                      l.Tc[0], l.Tc[1])
+        return pi
+
+    def rne_regressor(self, q, qd, qdd, gravity=None, dtype=None):
+        """The dynamics regressor Y(q, qd, qdd): (n, 14n) for one state or (N, n, 14n), with
+        ``Y @ dynamic_parameters() == rne(q, qd, qdd, gravity)`` (no tip wrench) for every link table rne serves:
+        prismatic joints through d = q + offset, the modified-DH prismatic first joint as rne treats it, ``flip``
+        ignored.  Y depends on the kinematics and the gear ratios only, not on the masses, inertias or friction.
+
+        Column 14i + k of row j is the torque of joint j per unit of parameter k of link i: exact 0 for i < j.  The
+        friction columns of link j (Jm, B, Tc+, Tc-) are G_j^2 qdd_j, G_j^2 qd_j, |G_j| [qd_j > 0] and |G_j| [qd_j < 0]
+        in row j (0 at qd_j = 0, as rne) and 0 in every other row.  Input forms, dtype and device rules are those of
+        ``rne_derivatives``; one kernel launch."""
+        return self._dyn("b2k_rne_regressor", [q, qd, qdd], (self.n, 14 * self.n), gravity=gravity, use_gravity=True,
+                         dtype=dtype)
+
+    def regressor_gram(self, q, qd, qdd, tau, gravity=None, weights=None, dtype=None):
+        """The normal equations of identification, accumulated on the device without Y existing in full: numpy
+        ``(G, b, s)`` with G (14n, 14n) = sum Y^T W Y, b (14n,) = sum Y^T W tau and the float s = sum tau^T W tau over the
+        rows, W = diag(weights) (n joint weights >= 0, default 1), always in float64.  q, qd, qdd, tau (N, n) or (n,),
+        numpy or CUDA tensors; Y is computed in ``dtype`` (default: that of q) in chunks of 4096 rows.  G is exactly
+        symmetric and two equal calls give equal bits."""
+        import torch
+
+        h = self._rne_handle()
+        n, p = self.n, 14 * self.n
+        dt, _, _, dev, N = self._dyn_inputs([q, qd, qdd, tau], dtype)
+        w = None
+        if weights is not None:
+            w = np.ascontiguousarray(np.asarray(weights, dtype=np.float64))
+            if w.shape != (n,):
+                raise ValueError(f"weights must have shape ({n},); got {w.shape}")
+        G = torch.empty((p, p), dtype=torch.float64, device=dev[0].device)
+        b = torch.empty(p, dtype=torch.float64, device=dev[0].device)
+        s = torch.empty(1, dtype=torch.float64, device=dev[0].device)
+        _lib.check(_lib.lib().b2k_rne_regressor_gram(h, B.code(dt), *(B.ptr(t) for t in dev), N,
+                                                     _lib.dptr(self._kernel_gravity(gravity)), _lib.dptr(w), B.ptr(G),
+                                                     B.ptr(b), B.ptr(s), B.stream_ptr(dev[0])))
+        return G.cpu().numpy(), b.cpu().numpy(), float(s.item())
+
+    def identify(self, q, qd, qdd, tau, gravity=None, weights=None, friction=True, rcond=1e-10, dtype=None):
+        """Least-squares identification of the link parameters from logged (q, qd, qdd, tau): the named tuple
+        ``(pi, rank, rms)``.  pi (14n,) is the minimum-norm solution of tau = Y pi (the convention of
+        ``dynamic_parameters``) from the normal equations of ``regressor_gram``: G is scaled to unit diagonal, and
+        eigenvalues of the scaled G below ``rcond`` times the largest are dropped; rank is the number kept.  rcond must
+        exceed the rounding of the scaled G in the compute type: the default 1e-10 suits float64; float32 rounds Y to
+        about 1e-7, so an exact dependency between columns can leave an eigenvalue far above 1e-10 there (use about 1e-5).  Parameters
+        whose column of Y is zero (below 16 eps of the compute type times the largest column norm) get 0.  ``friction=False`` drops the four friction parameters of every link (they come
+        back as 0).  rms is the weighted residual sqrt((s - 2 pi.b + pi.G.pi) / (N n)); the three terms cancel, so an rms
+        below about sqrt(eps) times the rms of tau is not resolved (an exact fit reads as 0 up to that level).
+
+        Only combinations of parameters are identifiable in general, so pi is not a physical link table; base
+        parameters and writing pi back into the links are left to the caller."""
+        G, b, s = self.regressor_gram(q, qd, qdd, tau, gravity=gravity, weights=weights, dtype=dtype)
+        n = self.n
+        shape = tuple(q.shape) if hasattr(q, "shape") else np.shape(q)
+        N = 1 if len(shape) == 1 else int(shape[0])
+        keep = np.ones(14 * n, dtype=bool)
+        if not friction:
+            for j in range(n):
+                keep[14 * j + 10:14 * j + 14] = False
+        # A column at the rounding level of the compute type is a zero column: a structurally zero term that the link
+        # constants (cos(pi/2) = 6e-17) or cancelling products leave a few ulps off 0 would otherwise become a unit
+        # column after the scaling below.  The cut, 16 eps of the largest column norm (2e-6 in float32), sits well
+        # below real columns: on Puma560 inertial columns are 4e-5 of the armature columns (G^2 qdd).
+        eps = np.finfo(B.pick_dtype(q, dtype)).eps
+        keep &= np.diag(G) > (16 * eps) ** 2 * np.max(np.diag(G), initial=0.0)
+        pi = np.zeros(14 * n)
+        rank = 0
+        if keep.any():
+            Gk, bk = G[np.ix_(keep, keep)], b[keep]
+            d = 1.0 / np.sqrt(np.diag(Gk))
+            lam, V = np.linalg.eigh(d[:, None] * Gk * d[None, :])
+            use = lam > rcond * lam[-1]
+            rank = int(use.sum())
+            pi[keep] = d * (V[:, use] @ ((V[:, use].T @ (d * bk)) / lam[use]))
+        res = s - 2 * pi @ b + pi @ G @ pi
+        return IdentifyResult(pi, rank, float(np.sqrt(max(res, 0.0) / max(N * n, 1))))
 
     # ---- static forces (reference DynamicsMixin, Dynamics.py): _static.py, csrc/b2k_static.cu
     def _static_mass_table(self) -> np.ndarray:

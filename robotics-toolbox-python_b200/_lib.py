@@ -74,6 +74,8 @@ _PROTOS = {
     "b2k_rne_accel": (C.c_int, [vp, C.c_int, vp, vp, vp, i64, dp, vp, vp]),
     "b2k_rne_derivatives": (C.c_int, [vp, C.c_int, vp, vp, vp, i64, dp, dp, vp, vp, vp]),
     "b2k_rne_accel_derivatives": (C.c_int, [vp, C.c_int, vp, vp, vp, i64, dp, vp, vp, vp, vp]),
+    "b2k_rne_regressor": (C.c_int, [vp, C.c_int, vp, vp, vp, i64, dp, vp, vp]),
+    "b2k_rne_regressor_gram": (C.c_int, [vp, C.c_int, vp, vp, vp, vp, i64, dp, dp, vp, vp, vp, vp]),
     "b2k_gravjac": (C.c_int, [vp, C.c_int, vp, i64, i64, dp, dp, vp, vp, vp]),
     "b2k_pay": (C.c_int, [vp, C.c_int, vp, i64, i64, vp, i64, C.c_int, vp, vp]),
     "b2k_pay_jacobian": (C.c_int, [C.c_int, C.c_int, vp, vp, i64, i64, vp, vp]),

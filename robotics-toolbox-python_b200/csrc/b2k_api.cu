@@ -179,11 +179,12 @@ extern "C" int b2k_fkine_jacobe(b2k_chain_t c, int dtype, const void *q, int64_t
 // the generic kernels (b2k_rne.cuh), one translation unit per family of operations and dtype
 typedef int RneGenericFn(const b2k_rne_s *, int op, int dtype, const b2k_rne_args &, cudaStream_t);
 RneGenericFn b2k_rne_generic_rne, b2k_rne_generic_wrench, b2k_rne_generic_fan_f32, b2k_rne_generic_fan_f64,
-    b2k_rne_generic_deriv_f32, b2k_rne_generic_deriv_f64;
+    b2k_rne_generic_deriv_f32, b2k_rne_generic_deriv_f64, b2k_rne_generic_regressor_f32, b2k_rne_generic_regressor_f64;
 
 // Every argument is checked against the operation's row of B2K_RNE_OPS before any CUDA call; then the robot-specialised
 // kernel (b2k_rne_spec.cu) serves the full 32-row tiles of the operations it has, and the generic kernel the rest.
-static int rne_dispatch(const char *fn, int op, b2k_rne_t r, int dtype, b2k_rne_args a, void *stream)
+// The checks of an operation's handle, scalars and inputs (its row of B2K_RNE_OPS), in this order
+static int rne_check_inputs(const char *fn, int op, b2k_rne_t r, int dtype, const b2k_rne_args &a)
 {
     const b2k_rne_op_s &d = B2K_RNE_OPS[op];
     if (!r) { b2k_set_error("%s: rne handle is NULL", fn); return B2K_ERR_INVALID; }
@@ -195,6 +196,15 @@ static int rne_dispatch(const char *fn, int op, b2k_rne_t r, int dtype, b2k_rne_
     const int es = dtype == B2K_F64 ? 8 : 4;
     for (int i = 0; i < d.nin; i++)
         if ((rc = b2k_check_array(fn, d.in[i], a.in[i], a.nrows, es))) return rc;
+    return B2K_OK;
+}
+
+static int rne_dispatch(const char *fn, int op, b2k_rne_t r, int dtype, b2k_rne_args a, void *stream)
+{
+    const b2k_rne_op_s &d = B2K_RNE_OPS[op];
+    int rc;
+    if ((rc = rne_check_inputs(fn, op, r, dtype, a))) return rc;
+    const int es = dtype == B2K_F64 ? 8 : 4;
     // each output leaves through a per-warp stage of its rows, copied in b2k_stage_unit(row bytes) pieces (b2k_rne.cuh)
     for (int o = 0; o < d.nout; o++)
         if ((rc = b2k_check_array(fn, d.out[o], a.out[o], a.nrows, b2k_stage_unit(d.out_row(o, r->n) * es)))) return rc;
@@ -209,10 +219,12 @@ static int rne_dispatch(const char *fn, int op, b2k_rne_t r, int dtype, b2k_rne_
         for (int o = 0; o < d.nout; o++) a.out[o] = (char *)a.out[o] + (size_t)done * d.out_row(o, r->n) * es;
         a.nrows -= done;
     }
-    RneGenericFn *generic = op == B2K_GEN_RNE          ? b2k_rne_generic_rne
-                            : op == B2K_GEN_RNE_WRENCH ? b2k_rne_generic_wrench
-                            : op >= B2K_GEN_RNE_DERIV  ? (dtype == B2K_F64 ? b2k_rne_generic_deriv_f64 : b2k_rne_generic_deriv_f32)
-                                                       : (dtype == B2K_F64 ? b2k_rne_generic_fan_f64 : b2k_rne_generic_fan_f32);
+    const bool f64 = dtype == B2K_F64;
+    RneGenericFn *generic = op == B2K_GEN_RNE             ? b2k_rne_generic_rne
+                            : op == B2K_GEN_RNE_WRENCH    ? b2k_rne_generic_wrench
+                            : op == B2K_GEN_RNE_REGRESSOR ? (f64 ? b2k_rne_generic_regressor_f64 : b2k_rne_generic_regressor_f32)
+                            : op >= B2K_GEN_RNE_DERIV     ? (f64 ? b2k_rne_generic_deriv_f64 : b2k_rne_generic_deriv_f32)
+                                                          : (f64 ? b2k_rne_generic_fan_f64 : b2k_rne_generic_fan_f32);
     return generic(r, op, dtype, a, st);
 }
 
@@ -608,4 +620,47 @@ extern "C" int b2k_rne_accel_derivatives(b2k_rne_t r, int dtype, const void *q, 
 {
     return rne_dispatch("b2k_rne_accel_derivatives", B2K_GEN_ACCEL_DERIV, r, dtype,
                         {{q, qd, torque}, {dqdd_dq, dqdd_dqd, dqdd_dtau}, N, grav, nullptr}, stream);
+}
+
+// ------------------------------------------------------------------ the dynamics regressor and its normal equations (b2k_rne.cuh)
+extern "C" int b2k_rne_regressor(b2k_rne_t r, int dtype, const void *q, const void *qd, const void *qdd, int64_t N,
+                                 const double *grav, void *Y, void *stream)
+{
+    return rne_dispatch("b2k_rne_regressor", B2K_GEN_RNE_REGRESSOR, r, dtype, {{q, qd, qdd}, {Y}, N, grav, nullptr}, stream);
+}
+
+int b2k_rne_regressor_gram_f32(const b2k_rne_s *, const b2k_rne_args &, const void *, const double *, double *, double *,
+                               double *, cudaStream_t);
+int b2k_rne_regressor_gram_f64(const b2k_rne_s *, const b2k_rne_args &, const void *, const double *, double *, double *,
+                               double *, cudaStream_t);
+
+extern "C" int b2k_rne_regressor_gram(b2k_rne_t r, int dtype, const void *q, const void *qd, const void *qdd, const void *tau,
+                                      int64_t N, const double *grav, const double *weights, double *G, double *b, double *s,
+                                      void *stream)
+{
+    const char *fn = "b2k_rne_regressor_gram";
+    const b2k_rne_args a = {{q, qd, qdd}, {nullptr}, N, grav, nullptr};
+    int rc;
+    if ((rc = rne_check_inputs(fn, B2K_GEN_RNE_REGRESSOR, r, dtype, a))) return rc;
+    if ((rc = b2k_check_array(fn, "tau", tau, N, dtype == B2K_F64 ? 8 : 4))) return rc;
+    if (weights)
+        for (int j = 0; j < r->n; j++)
+            if (!isfinite(weights[j]) || weights[j] < 0) {
+                b2k_set_error("%s: weights[%d] = %g is not a finite value >= 0", fn, j, weights[j]);
+                return B2K_ERR_INVALID;
+            }
+    // the sums are written whatever N is (zeros for N = 0)
+    if ((rc = b2k_check_array(fn, "G", G, 1, 8)) || (rc = b2k_check_array(fn, "b", b, 1, 8)) || (rc = b2k_check_array(fn, "s", s, 1, 8)))
+        return rc;
+    B2K_ON_DEVICE_OF(G);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (N == 0) {
+        const size_t p = 14 * (size_t)r->n;
+        B2K_CUDA(cudaMemsetAsync(G, 0, p * p * sizeof(double), st));
+        B2K_CUDA(cudaMemsetAsync(b, 0, p * sizeof(double), st));
+        B2K_CUDA(cudaMemsetAsync(s, 0, sizeof(double), st));
+        return B2K_OK;
+    }
+    return dtype == B2K_F64 ? b2k_rne_regressor_gram_f64(r, a, tau, weights, G, b, s, st)
+                            : b2k_rne_regressor_gram_f32(r, a, tau, weights, G, b, s, st);
 }

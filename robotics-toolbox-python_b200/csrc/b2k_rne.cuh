@@ -914,6 +914,368 @@ k_rne_deriv(const __grid_constant__ RneP<real, N> P, const real *__restrict__ in
     }
 }
 
+// ------------------------------------------------------------------ the dynamics regressor (DESIGN f-16)
+// tau = Y(q, qd, qdd; g) pi without a tip wrench, pi = 14 parameters per link, link-major:
+//   [m, m rx, m ry, m rz, Ixx, Iyy, Izz, Ixy, Iyz, Ixz, Jm, B, Tc+, Tc-]
+// r the link's centre of mass in its frame, the inertia about the link-frame origin, I + m (r.r E - r r^T).
+// Row j of Y is built from the unit twist s = (sf, sn) of joint j carried out along the chain: joint j's torque from a
+// wrench (f, n) of link i >= j about O_i, in frame i, is sf . f + sn . n -- the transpose of the backward recursion of
+// rne_row_generic, which carries the wrench of link i in to joint j.  The wrench of link i is linear in its parameters:
+//   f = m a + wd x (m r) + w x (w x (m r)),   n = I_o wd + w x (I_o w) + (m r) x a
+// with w, wd, a the angular velocity, angular acceleration and frame-origin acceleration (gravity included) of link i in
+// its own frame, from the forward recursion below.
+
+// One step of the forward recursion: link j's w, wd and acc from link j-1's.  The forward half of rne_row_generic,
+// restated formula by formula with its quirks (ne.c:137-240 MDH, 245-347 DH; the MDH prismatic first joint, ne.c:187-204).
+template <typename real, int N, bool MDH, bool ALLREV>
+__device__ __forceinline__ void rne_forward_step(const RneP<real, N> &P, int j, const real *mq, const real *sth, const real *cth,
+                                                 const real *mqd, const real *mqdd, V3<real> gravity, V3<real> &w, V3<real> &wd,
+                                                 V3<real> &acc)
+{
+    typedef V3<real> V;
+    const bool pris = !ALLREV && (P.prismatic[j] != 0);
+    const real st = sth[j], ct = cth[j];
+    const real d = pris ? (mq[j] + P.offset[j]) : P.D[j];
+    const LinkRot<real, MDH> R(st, ct, P.sa[j], P.ca[j]);
+    const V pstar = MDH ? V{P.A[j], -d * P.sa[j], d * P.ca[j]} : V{P.A[j], d * P.sa[j], d * P.ca[j]};
+    const V qdv = {0, 0, mqd[j]}, qddv = {0, 0, mqdd[j]};
+    V wn, wdn, accn, t1, t2, t3;
+    if (MDH) {
+        if (!pris) {
+            if (j == 0) {
+                wn = qdv; wdn = qddv; t1 = gravity;
+            } else {
+                t1 = R.tmul(w);
+                wn = vadd(t1, qdv);
+                t3 = R.tmul(wd);
+                t2 = vcross(t1, qdv);
+                t1 = vadd(t2, t3);
+                wdn = vadd(t1, qddv);
+                t1 = vcross(w, pstar);
+                t2 = vcross(w, t1);
+                t1 = vcross(wd, pstar);
+                t1 = vadd(t1, t2);
+                t1 = vadd(t1, acc);
+            }
+            accn = R.tmul(t1);
+        } else {
+            if (j == 0) {
+                wn = qdv; wdn = qddv; accn = gravity; // sic, ne.c:187-204
+            } else {
+                wn = R.tmul(w);
+                wdn = R.tmul(wd);
+                t1 = vcross(wd, pstar);
+                t3 = vcross(w, pstar);
+                t2 = vcross(w, t3);
+                t1 = vadd(t1, t2);
+                t1 = vadd(t1, acc);
+                accn = R.tmul(t1);
+                t2 = R.tmul(w);
+                t1 = vcross(t2, qdv);
+                t1 = vscale(t1, (real)2);
+                accn = vadd(accn, t1);
+                accn = vadd(accn, qddv);
+            }
+        }
+    } else {
+        if (!pris) {
+            t1 = (j == 0) ? qdv : vadd(w, qdv);
+            wn = R.tmul(t1);
+            if (j == 0) t3 = qddv;
+            else {
+                t1 = vadd(wd, qddv);
+                t2 = vcross(w, qdv);
+                t3 = vadd(t1, t2);
+            }
+            wdn = R.tmul(t3);
+            t1 = vcross(wdn, pstar);
+            t2 = vcross(wn, pstar);
+            t3 = vcross(wn, t2);
+            accn = vadd(t1, t3);
+            t1 = R.tmul(j == 0 ? gravity : acc);
+            accn = vadd(accn, t1);
+        } else {
+            if (j == 0) {
+                wn = {0, 0, 0}; wdn = {0, 0, 0};
+                t1 = vadd(qddv, gravity);
+                accn = R.tmul(t1);
+            } else {
+                wn = R.tmul(w);
+                wdn = R.tmul(wd);
+                t1 = vadd(qddv, acc);
+                accn = R.tmul(t1);
+            }
+            t1 = vcross(wdn, pstar);
+            accn = vadd(accn, t1);
+            t1 = R.tmul(qdv);
+            t2 = vcross(wn, t1);
+            t2 = vscale(t2, (real)2);
+            accn = vadd(accn, t2);
+            t2 = vcross(wn, pstar);
+            t3 = vcross(wn, t2);
+            accn = vadd(accn, t3);
+        }
+    }
+    w = wn; wd = wdn; acc = accn;
+}
+
+// The per-warp slab of one joint row, and how it leaves so that every 32-byte sector of Y is written whole by one warp
+// instruction.  A row of the batch is 14 N^2 reals, joint row j of it 14 N: these pieces start on a sector boundary only
+// for some N and dtypes, so a sector can hold the end of joint row j and the start of j + 1, or the end of a row's last
+// joint row and the start of the next row's first.  Slab row l (the tile's row l) is laid out from the sector boundary at
+// or below the start of its joint row: [tail of joint row j - 1 | joint row j | start of the next row's joint row 0 (last
+// j only)].  Joint row j leaves from its first sector boundary up to its last one; the partial sector at its end goes out
+// with joint row j + 1 (the tail is carried to the front of the slab row), and the partial sector at the start of a row's
+// joint row 0 waits in STASH until the previous row's last joint row, which completes the sector.  The warp drains one
+// tile row at a time, consecutive lanes on consecutive reals from a sector boundary.  Where every joint row starts on a
+// sector boundary the carry and the stash are empty and the tile drains as one sequence, all lanes busy.
+template <typename real, int N>
+struct RegSlab {
+    static constexpr int ROW = 14 * N;
+    static constexpr int SE = 32 / (int)sizeof(real); // reals per sector
+    static constexpr int LD = (ROW + 2 * SE) | 1;     // slab row stride in reals
+    static constexpr int STASH = 32 * LD;             // offset of the per-row stash of SE reals
+    static constexpr int BYTES = ((32 * LD + 32 * SE) * (int)sizeof(real) + 15) & ~15;
+};
+
+template <typename real, int N, bool MDH, bool ALLREV>
+__global__ void __launch_bounds__(B2K_THREADS, 1)
+k_rne_regressor(const __grid_constant__ RneP<real, N> P, const real *__restrict__ in0, const real *__restrict__ in1,
+                const real *__restrict__ in2, long long nrows, real *__restrict__ out, int warp_smem_bytes, int in_bytes,
+                int qmode)
+{
+    typedef RegSlab<real, N> SL;
+    typedef V3<real> V;
+    constexpr int ROWN = 14 * N * N; // reals per row of the batch
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    const int lane = threadIdx.x & 31;
+    const int warp = threadIdx.x >> 5;
+    unsigned char *wbase = smem_raw + (size_t)warp * warp_smem_bytes;
+    real *s0 = reinterpret_cast<real *>(wbase);
+    real *s1 = reinterpret_cast<real *>(wbase + in_bytes);
+    real *s2 = reinterpret_cast<real *>(wbase + 2 * in_bytes);
+    real *slab = reinterpret_cast<real *>(wbase + 3 * in_bytes);
+    const int lds = qmode ? N : (N | 1);
+    const long long ntiles = (nrows + 31) >> 5;
+    const float inv_n = 1.0f / (float)N;
+    const long long tile = (long long)blockIdx.x * B2K_WARPS_PER_BLOCK + warp; // one tile per warp, one-shot grid
+    if (tile >= ntiles) return;
+    const long long row0 = tile << 5;
+    const int rows_here = (int)((nrows - row0) < 32 ? (nrows - row0) : 32);
+    load_q_tile<real>(s0, in0 + row0 * N, rows_here, N, inv_n, qmode, lane);
+    load_q_tile<real>(s1, in1 + row0 * N, rows_here, N, inv_n, qmode, lane);
+    load_q_tile<real>(s2, in2 + row0 * N, rows_here, N, inv_n, qmode, lane);
+    cp_async_wait_all();
+    __syncwarp();
+    const int myrow = (lane < rows_here ? lane : 0) * lds;
+    const real *mq = s0 + myrow, *mqd = s1 + myrow, *mqdd = s2 + myrow;
+
+    real sth[N], cth[N];
+    rne_sincos<real, N, ALLREV>(P, mq, sth, cth);
+    const V grav = {P.grav[0], P.grav[1], P.grav[2]};
+    real *my = slab + lane * SL::LD;
+    real *gtile = out + row0 * ROWN;
+    constexpr int SE = SL::SE;
+    // reals between joint row jr of tile row r and the sector boundary at or below it
+    auto mis_of = [&](int r, int jr) { return (int)((reinterpret_cast<uintptr_t>(gtile + (long long)r * ROWN + jr * SL::ROW) & 31) / sizeof(real)); };
+    int mis_prev = 0;
+    // every joint row of every row starts on a sector boundary (fp64 with even N, fp32 with N divisible by 4, and Y
+    // 32-byte aligned): no carry or stash is needed, and the tile drains as one sequence
+    const bool whole = (SL::ROW * (int)sizeof(real)) % 32 == 0 && mis_of(0, 0) == 0;
+
+#pragma unroll 1
+    for (int jr = 0; jr < N; jr++) { // joint row jr of every row of the tile
+        const int mis = mis_of(lane, jr);
+        if (jr > 0) // the tail of joint row jr - 1 that did not fill its last sector
+            for (int t = 0; t < mis; t++) my[t] = my[mis_prev + SL::ROW - mis + t];
+        mis_prev = mis;
+        V w = {0, 0, 0}, wd = {0, 0, 0}, acc = {0, 0, 0};
+        V sf = {0, 0, 0}, sn = {0, 0, 0};
+#pragma unroll
+        for (int i = 0; i < N; i++) {
+            rne_forward_step<real, N, MDH, ALLREV>(P, i, mq, sth, cth, mqd, mqdd, grav, w, wd, acc);
+            real *y = my + mis + 14 * i;
+            if (i < jr) {
+#pragma unroll
+                for (int k = 0; k < 14; k++) y[k] = 0;
+                continue;
+            }
+            const bool pris = !ALLREV && (P.prismatic[i] != 0);
+            const real d = pris ? (mq[i] + P.offset[i]) : P.D[i];
+            const V ps = MDH ? V{P.A[i], -d * P.sa[i], d * P.ca[i]} : V{P.A[i], d * P.sa[i], d * P.ca[i]};
+            if (i == jr) { // joint jr's own unit twist, as rne_row_generic projects its wrench
+                const V z = MDH ? V{0, 0, 1} : V{0, P.sa[i], P.ca[i]}; // MDH: z of frame i; DH: R_i^T z0 (axis on frame i-1)
+                if (pris) { sf = z; sn = {0, 0, 0}; }
+                else { sn = z; sf = MDH ? V{0, 0, 0} : vcross(z, ps); } // DH: the moment is taken about O_{i-1} = O_i - p*
+            } else { // carried out through joint i: the transpose of the backward step
+                const LinkRot<real, MDH> R(sth[i], cth[i], P.sa[i], P.ca[i]);
+                if (MDH) {
+                    sf = R.tmul(vadd(sf, vcross(sn, ps)));
+                    sn = R.tmul(sn);
+                } else {
+                    sn = R.tmul(sn);
+                    sf = vadd(R.tmul(sf), vcross(sn, ps));
+                }
+            }
+            // the 10 inertial columns: the coefficients of m, m r and I_o in sf . f + sn . n
+            y[0] = vdot(sf, acc);
+            const V h = vadd(vadd(vcross(sf, wd), vscale(w, vdot(sf, w))), vadd(vscale(sf, -vdot(w, w)), vcross(acc, sn)));
+            y[1] = h.x; y[2] = h.y; y[3] = h.z;
+            const V u = vcross(sn, w); // sn . (w x I w) = u . I w
+            y[4] = sn.x * wd.x + u.x * w.x;
+            y[5] = sn.y * wd.y + u.y * w.y;
+            y[6] = sn.z * wd.z + u.z * w.z;
+            y[7] = sn.x * wd.y + sn.y * wd.x + u.x * w.y + u.y * w.x;
+            y[8] = sn.y * wd.z + sn.z * wd.y + u.y * w.z + u.z * w.y;
+            y[9] = sn.x * wd.z + sn.z * wd.x + u.x * w.z + u.z * w.x;
+            // joint friction acts in joint i only; P holds the constants of a unit table: G^2, G^2, |G|, |G|
+            const real qdi = mqd[i];
+            const bool own = i == jr;
+            y[10] = own ? P.c_jm[i] * mqdd[i] : (real)0;
+            y[11] = own ? P.c_b[i] * qdi : (real)0;
+            y[12] = own && qdi > 0 ? P.c_tcp[i] : (real)0;
+            y[13] = own && qdi < 0 ? P.c_tcm[i] : (real)0;
+        }
+        if (jr == 0) // the start of joint row 0 up to its first sector boundary: written with the previous row's end
+            for (int t = 0; t < (SE - mis) % SE; t++) slab[SL::STASH + lane * SE + t] = my[mis + t];
+        const int end = mis + SL::ROW; // slab position of the end of joint row jr
+        if (jr == N - 1) {
+            __syncwarp();
+            if (lane < rows_here - 1) // complete the last sector with the next row's stashed start
+                for (int t = 0; t < (SE - end % SE) % SE; t++) my[end + t] = slab[SL::STASH + (lane + 1) * SE + t];
+        }
+        __syncwarp();
+        if (whole) { // every piece starts on a sector boundary: the tile's pieces back to back, all lanes busy
+            const int cnt = rows_here * SL::ROW;
+            real *g = gtile + jr * SL::ROW;
+            for (int e = lane; e < cnt; e += 32) {
+                const int r = e / SL::ROW, c = e - r * SL::ROW;
+                g[(long long)r * ROWN + c] = slab[r * SL::LD + c];
+            }
+        } else { // one tile row at a time from its first sector boundary, consecutive lanes on consecutive reals
+            for (int r = 0; r < rows_here; r++) {
+                const int m = mis_of(r, jr);
+                const int e = m + SL::ROW;
+                const int lo = jr > 0 ? 0 : (r > 0 ? m + (SE - m) % SE : m);
+                const int hi = jr < N - 1 ? e - e % SE : (r < rows_here - 1 ? e + (SE - e % SE) % SE : e);
+                real *g = gtile + (long long)r * ROWN + jr * SL::ROW - m; // the sector boundary at or below joint row jr
+                for (int u = lo + lane; u < hi; u += 32) g[u] = slab[r * SL::LD + u];
+            }
+        }
+        __syncwarp();
+    }
+}
+
+// ------------------------------------------------------------------ normal equations of the regressor (DESIGN f-16)
+// G = sum Y^T W Y, b = sum Y^T W tau, s = sum tau^T W tau over a batch, in fp64, without Y ever existing in full: the
+// regressor kernel writes a chunk of REG_CHUNK rows into a stream-ordered scratch buffer, k_regressor_syrk folds it into
+// per-(tile pair, slice) partials, k_regressor_gram_reduce sums the partials.  The three are one Gram matrix of the
+// augmented rows [Y[row, j, :] | tau[row, j]] weighted by w_j.  Every sum runs in a fixed order: no atomics, two equal
+// calls give equal bits.
+constexpr long long REG_CHUNK = 4096; // rows per chunk: Puma560 fp64 is 16.5 MB of Y, well inside H100's 50 MB L2
+constexpr int REG_TILE = 32;          // the Gram matrix in 32 x 32 tiles, upper triangle only
+constexpr int REG_KB = 16;            // augmented rows per k-step
+
+struct RegWeights {
+    double w[B2K_MAX_JOINTS];
+};
+
+// tile pair t (row-major over the upper triangle of an nt x nt tiling) -> (ti, tj), ti <= tj
+__device__ __forceinline__ void reg_tile_pair(int t, int nt, int &ti, int &tj)
+{
+    ti = 0;
+    while (t >= nt - ti) { t -= nt - ti; ti++; }
+    tj = ti + t;
+}
+
+// Block (tile pair, slice): 4 groups of 64 threads, each thread a 4 x 4 register tile of the 32 x 32 tile; group g takes
+// every 4th k-step of the slice, and the groups are summed in order at the end.
+template <typename real>
+__global__ void __launch_bounds__(256)
+k_regressor_syrk(const real *__restrict__ Y, const real *__restrict__ tau, long long K, int n, int p, int nt,
+                 const __grid_constant__ RegWeights W,
+                 double *__restrict__ part, int accumulate)
+{
+    __shared__ __align__(16) double sm[4][2][REG_KB][REG_TILE]; // per group: the A and B k-step tiles; then the group sums
+    const int tid = threadIdx.x, g = tid >> 6, t = tid & 63, tx = t & 7, ty = t >> 3;
+    int ti, tj;
+    reg_tile_pair(blockIdx.x, nt, ti, tj);
+    const long long nkb = (K + REG_KB - 1) / REG_KB;
+    const long long b0 = nkb * blockIdx.y / gridDim.y, b1 = nkb * (blockIdx.y + 1) / gridDim.y;
+    const long long rounds = (b1 - b0 + 3) / 4;
+    double acc[4][4];
+#pragma unroll
+    for (int u = 0; u < 4; u++)
+#pragma unroll
+        for (int v = 0; v < 4; v++) acc[u][v] = 0;
+    // K <= REG_CHUNK * n: 32-bit row arithmetic
+    const int ca = ti * REG_TILE, cb = tj * REG_TILE;
+    auto elem = [&](int k, int col) -> double {
+        if (col > p) return 0.0;
+        return col < p ? (double)Y[(size_t)k * p + col] : (double)tau[k];
+    };
+    for (long long rd = 0; rd < rounds; rd++) {
+        const int kb = (int)(b0 + 4 * rd + g);
+#pragma unroll
+        for (int m = 0; m < REG_KB * REG_TILE / 64; m++) {
+            const int e = t + 64 * m, kk = e / REG_TILE, cc = e % REG_TILE;
+            const int k = kb * REG_KB + kk;
+            const bool live = kb < b1 && k < K;
+            sm[g][0][kk][cc] = live ? W.w[k % n] * elem(k, ca + cc) : 0.0;
+            sm[g][1][kk][cc] = live ? elem(k, cb + cc) : 0.0;
+        }
+        __syncthreads();
+#pragma unroll
+        for (int kk = 0; kk < REG_KB; kk++) {
+            const double2 a01 = *reinterpret_cast<const double2 *>(&sm[g][0][kk][ty * 4]);
+            const double2 a23 = *reinterpret_cast<const double2 *>(&sm[g][0][kk][ty * 4 + 2]);
+            const double2 c01 = *reinterpret_cast<const double2 *>(&sm[g][1][kk][tx * 4]);
+            const double2 c23 = *reinterpret_cast<const double2 *>(&sm[g][1][kk][tx * 4 + 2]);
+            const double a[4] = {a01.x, a01.y, a23.x, a23.y}, c[4] = {c01.x, c01.y, c23.x, c23.y};
+#pragma unroll
+            for (int u = 0; u < 4; u++)
+#pragma unroll
+                for (int v = 0; v < 4; v++) acc[u][v] = fma(a[u], c[v], acc[u][v]);
+        }
+        __syncthreads();
+    }
+    double *red = &sm[0][0][0][0]; // 4 groups x 1024 sums
+#pragma unroll
+    for (int u = 0; u < 4; u++)
+#pragma unroll
+        for (int v = 0; v < 4; v++) red[g * 1024 + (ty * 4 + u) * REG_TILE + tx * 4 + v] = acc[u][v];
+    __syncthreads();
+    double *dst = part + ((size_t)blockIdx.y * gridDim.x + blockIdx.x) * (REG_TILE * REG_TILE);
+#pragma unroll
+    for (int m = 0; m < 4; m++) {
+        const int e = tid + 256 * m;
+        const double sum = ((red[e] + red[1024 + e]) + red[2048 + e]) + red[3072 + e];
+        dst[e] = accumulate ? dst[e] + sum : sum;
+    }
+}
+
+// entry (a, c) of the augmented (p + 1) x (p + 1) Gram matrix: the slices summed in order; (a, c) and (c, a) read the same
+// partials in the same order, so G comes out exactly symmetric
+template <int TILE>
+__global__ void __launch_bounds__(256)
+k_regressor_gram_reduce(const double *__restrict__ part, int slices, int npairs, int nt, int p, double *__restrict__ G,
+                        double *__restrict__ b, double *__restrict__ s)
+{
+    const int P = p + 1;
+    const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= P * P) return;
+    const int a = idx / P, c = idx - a * P;
+    const int lo = a < c ? a : c, hi = a < c ? c : a;
+    const int ti = lo / TILE, tj = hi / TILE;
+    const int t = ti * nt - ti * (ti - 1) / 2 + (tj - ti);
+    const int e = (lo % TILE) * TILE + hi % TILE;
+    double sum = 0;
+    for (int sl = 0; sl < slices; sl++) sum += part[((size_t)sl * npairs + t) * (TILE * TILE) + e];
+    if (a < p && c < p) G[(size_t)a * p + c] = sum;
+    else if (a < p) b[a] = sum;
+    else if (c == p) *s = sum;
+}
+
 // ------------------------------------------------------------------ the generic launch path of every operation
 // The generic kernel of operation OP (B2K_GEN_*) for one link-table shape
 template <typename real, int N, bool MDH, bool ALLREV, int OP>
@@ -923,6 +1285,7 @@ constexpr auto rne_generic_kernel()
     else if constexpr (OP == B2K_GEN_RNE_WRENCH) return k_rne_wrench<real, N, MDH, ALLREV>;
     else if constexpr (OP == B2K_GEN_RNE_DERIV) return k_rne_deriv<real, N, MDH, ALLREV, DERIV_INVERSE>;
     else if constexpr (OP == B2K_GEN_ACCEL_DERIV) return k_rne_deriv<real, N, MDH, ALLREV, DERIV_FORWARD>;
+    else if constexpr (OP == B2K_GEN_RNE_REGRESSOR) return k_rne_regressor<real, N, MDH, ALLREV>;
     else return k_rne_fan<real, N, MDH, ALLREV, OP - B2K_GEN_INERTIA>;
 }
 
@@ -933,14 +1296,22 @@ int rne_generic_launch_op(const b2k_rne_s *r, const b2k_rne_args &a, cudaStream_
 {
     constexpr b2k_rne_op_s op = B2K_RNE_OPS[OP];
     RneP<real, N> P;
-    rne_fill_params<real, N>(r, op.grav ? a.grav : nullptr, op.fext ? a.fext : nullptr, P);
+    if constexpr (OP == B2K_GEN_RNE_REGRESSOR) { // the friction constants of a unit table: G^2, G^2, |G|, |G|
+        b2k_rne_s unit = *r;
+        for (int j = 0; j < N; j++) unit.L[j][19] = unit.L[j][21] = unit.L[j][22] = unit.L[j][23] = 1.0;
+        rne_fill_params<real, N>(&unit, a.grav, nullptr, P);
+    } else {
+        rne_fill_params<real, N>(r, op.grav ? a.grav : nullptr, op.fext ? a.fext : nullptr, P);
+    }
     if (OP == B2K_GEN_CORIOLIS) { // the reference works on robot.nofriction(True, True) (Dynamics.py:818)
         for (int j = 0; j < N; j++) { P.c_b[j] = 0; P.c_tcp[j] = 0; P.c_tcm[j] = 0; }
     }
     // per warp: the input tiles, then the output stage (the base wrench has its own behind tau's; the derivative
-    // outputs take turns in one)
+    // outputs take turns in one; the regressor's is the slab of one joint row)
     const size_t inb = fkj_q_bytes<real>(N);
-    const size_t stage = (size_t)TileStage<real, op.out_row(0, N)>::BYTES + (op.wrench ? (size_t)TileStage<real, 6>::BYTES : 0);
+    size_t stage;
+    if constexpr (OP == B2K_GEN_RNE_REGRESSOR) stage = RegSlab<real, N>::BYTES;
+    else stage = (size_t)TileStage<real, op.out_row(0, N)>::BYTES + (op.wrench ? (size_t)TileStage<real, 6>::BYTES : 0);
     const size_t wsm = (op.nin * inb + stage + 15) & ~(size_t)15;
     const size_t smem = wsm * B2K_WARPS_PER_BLOCK;
     const real *in[3] = {(const real *)a.in[0], (const real *)a.in[1], (const real *)a.in[2]};
@@ -949,7 +1320,10 @@ int rne_generic_launch_op(const b2k_rne_s *r, const b2k_rne_args &a, cudaStream_
     for (int i = 0; i < op.nin; i++) qmode = qmode && fkj_qmode<real>(in[i], N);
     const long long ntiles = (a.nrows + 31) / 32;
     const unsigned grid = (unsigned)((ntiles + B2K_WARPS_PER_BLOCK - 1) / B2K_WARPS_PER_BLOCK);
-    const char *what = OP == B2K_GEN_RNE || OP == B2K_GEN_RNE_WRENCH ? "rne" : (OP >= B2K_GEN_RNE_DERIV ? "rne derivative" : "rne fan-out");
+    const char *what = OP == B2K_GEN_RNE || OP == B2K_GEN_RNE_WRENCH ? "rne"
+                       : OP == B2K_GEN_RNE_REGRESSOR                 ? "rne regressor"
+                       : OP >= B2K_GEN_RNE_DERIV                     ? "rne derivative"
+                                                                     : "rne fan-out";
     auto launch = [&](auto kern) -> int {
         const int per_sm = b2k_blocks_per_sm((const void *)kern, B2K_THREADS, smem);
         if (per_sm < 1) return per_sm < 0 ? per_sm : (b2k_set_error("%s kernel does not fit on an SM", what), B2K_ERR_INVALID);
@@ -982,4 +1356,53 @@ int rne_generic_launch(const b2k_rne_s *r, int op, const b2k_rne_args &a, cudaSt
         return B2K_ERR_INVALID;
     }
 #undef B2K_CASE
+}
+
+// The normal equations of the regressor over a.nrows rows (a.in = q, qd, qdd; grav in a.grav), tau (N, n) of the compute
+// type, w the n joint weights; G (p, p), b (p), s (1) fp64 device arrays, p = 14 n.  b2k_api.cu has checked every
+// argument and handles N = 0.
+template <typename real>
+int rne_regressor_gram(const b2k_rne_s *r, const b2k_rne_args &a, const void *tau, const double *w, double *G, double *b,
+                       double *s, cudaStream_t st)
+{
+    const int n = r->n, p = 14 * n, nt = (p + 1 + REG_TILE - 1) / REG_TILE, npairs = nt * (nt + 1) / 2;
+    const long long chunk = a.nrows < REG_CHUNK ? a.nrows : REG_CHUNK;
+    // slices: about two blocks of 256 threads per SM, each slice at least 4 k-steps of a full chunk
+    const long long kmax = (chunk * n + REG_KB - 1) / REG_KB;
+    int slices = (2 * b2k_num_sms() + npairs - 1) / npairs;
+    if (slices > kmax / 4) slices = (int)(kmax / 4 > 0 ? kmax / 4 : 1);
+    RegWeights W;
+    for (int j = 0; j < B2K_MAX_JOINTS; j++) W.w[j] = j < n ? (w ? w[j] : 1.0) : 0.0;
+    const size_t ybytes = ((size_t)chunk * n * p * sizeof(real) + 255) & ~(size_t)255;
+    const size_t pbytes = (size_t)slices * npairs * REG_TILE * REG_TILE * sizeof(double);
+    b2k_keep_mempool();
+    void *scratch = nullptr;
+    B2K_CUDA(cudaMallocAsync(&scratch, ybytes + pbytes, st));
+    real *Y = (real *)scratch;
+    double *part = (double *)((char *)scratch + ybytes);
+    int rc = B2K_OK;
+    for (long long c0 = 0; c0 < a.nrows && rc == B2K_OK; c0 += chunk) {
+        const long long rows = a.nrows - c0 < chunk ? a.nrows - c0 : chunk;
+        b2k_rne_args ca = a;
+        for (int i = 0; i < 3; i++) ca.in[i] = (const real *)a.in[i] + c0 * n;
+        ca.out[0] = Y;
+        ca.nrows = rows;
+        rc = rne_generic_launch<real, B2K_GEN_RNE_REGRESSOR>(r, B2K_GEN_RNE_REGRESSOR, ca, st);
+        if (rc) break;
+        k_regressor_syrk<real><<<dim3(npairs, slices), 256, 0, st>>>(Y, (const real *)tau + c0 * n, rows * n, n, p, nt, W, part,
+                                                                      c0 > 0);
+        b2k_count_launch();
+        const cudaError_t e = cudaGetLastError();
+        if (e != cudaSuccess) rc = b2k_cuda_fail(e, "k_regressor_syrk launch");
+    }
+    if (rc == B2K_OK) {
+        const int P = p + 1;
+        k_regressor_gram_reduce<REG_TILE><<<(P * P + 255) / 256, 256, 0, st>>>(part, slices, npairs, nt, p, G, b, s);
+        b2k_count_launch();
+        const cudaError_t e = cudaGetLastError();
+        if (e != cudaSuccess) rc = b2k_cuda_fail(e, "k_regressor_gram_reduce launch");
+    }
+    const cudaError_t e = cudaFreeAsync(scratch, st);
+    if (rc == B2K_OK && e != cudaSuccess) rc = b2k_cuda_fail(e, "cudaFreeAsync");
+    return rc;
 }

@@ -790,3 +790,79 @@ if any(want(c) for c in DERIV_CASES):
             report(c_acc, ms, N, (3 * n + 3 * n * n) * es, dict(card, **fd, bound="compute (expected, not measured)",
                                                                  speedup_vs_fd_route=round(fd["fd_route_ms"] / ms, 2)))
         del q0, qd0, x0, o
+
+# The dynamics regressor (DHRobot.rne_regressor, b2k_rne_regressor) and its normal equations (b2k_rne_regressor_gram),
+# Puma560 (DH) and PandaMDH, N device rows.  Algorithmic bytes per row of the regressor: (3n + 14n^2) es, against
+# 3.35 TB/s.  The gram is compute work: n p^2 / 2 FMAs per row (p = 14n, the upper triangle of p x p per joint row),
+# reported in FP64 FLOP/s against the data sheet's 34 TFLOP/s (non-tensor).  unit_route is what a user has without the
+# regressor, timed in the same call on the same rows: 14n b2k_rne launches, one per unit link table (tests/regressor_ref.py;
+# the m r columns need one more subtraction each, not counted), with both routes alternated.  The card's name and power limit are read in the same run.
+REG_CASES = [f"regressor_{r}_{t}" for r in ("puma", "pandamdh") for t in ("f64", "f32")] + \
+            [f"regressor_gram_{r}_{t}" for r in ("puma", "pandamdh") for t in ("f64", "f32")]
+if any(want(c) for c in REG_CASES):
+    import subprocess
+
+    try:
+        plim = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True,
+                              text=True, timeout=30).stdout.strip()
+    except Exception as e:  # the figure is context, the timing does not depend on it
+        plim = f"unavailable ({type(e).__name__})"
+    card = {"gpu": torch.cuda.get_device_name(0), "power_limit": plim}
+    Lr = rtb._lib.lib()
+    str_ = torch.cuda.current_stream().cuda_stream
+    rngr = np.random.default_rng(16)
+    for rname, rob in (("puma", rtb.models.Puma560()), ("pandamdh", rtb.models.PandaMDH())):
+        n, p = rob.n, 14 * rob.n
+        hr = rob._rne_handle()
+        gr = rob._kernel_gravity(None)
+        for dt in (np.float64, np.float32):
+            tag = "f64" if dt == np.float64 else "f32"
+            c_reg, c_gram = f"regressor_{rname}_{tag}", f"regressor_gram_{rname}_{tag}"
+            if not (want(c_reg) or want(c_gram)):
+                continue
+            es = np.dtype(dt).itemsize
+            code = rtb._lib.F64 if dt == np.float64 else rtb._lib.F32
+            tt = torch.float64 if dt == np.float64 else torch.float32
+            q0, qd0, qdd0, tau0 = (torch.from_numpy(rngr.uniform(-2, 2, (N, n)).astype(dt)).to(dev) for _ in range(4))
+            if want(c_reg):
+                Y = torch.empty((N, n, p), dtype=tt, device=dev)
+                units = []
+                for i in range(p):  # one rne handle per column; which parameter is 1 does not change an rne launch's time
+                    import ctypes
+                    T = rob._pack_rne().reshape(-1, 24).copy()
+                    T[:, 6:20] = 0.0
+                    T[:, 21:24] = 0.0
+                    T[i // 14, 6] = 1.0
+                    hu = rtb._lib.vp()
+                    rtb._lib.check(Lr.b2k_rne_create(n, rob.mdh, rtb._lib.dptr(np.ascontiguousarray(T.ravel())), ctypes.byref(hu)))
+                    units.append(hu)
+                outs = [torch.empty((N, n), dtype=tt, device=dev) for _ in range(p)]
+
+                def unit_route(i):
+                    for hu, t in zip(units, outs):
+                        rtb._lib.check(Lr.b2k_rne(hu, code, q0.data_ptr(), qd0.data_ptr(), qdd0.data_ptr(), N, rtb._lib.dptr(gr), None,
+                                                  t.data_ptr(), str_))
+
+                ms_u, ms = [], []
+                for _ in range(2):  # alternate the two routes, so that both see the same clocks
+                    ms_u.append(timeit(unit_route, 1))
+                    ms.append(timeit(lambda i: rtb._lib.check(Lr.b2k_rne_regressor(hr, code, q0.data_ptr(), qd0.data_ptr(), qdd0.data_ptr(), N,
+                                                                                   rtb._lib.dptr(gr), Y.data_ptr(), str_)), 1))
+                ms_u, ms = min(ms_u), min(ms)
+                bpr = (3 * n + 14 * n * n) * es
+                report(c_reg, ms, N, bpr, dict(card, frac_of_3p35TBps=round(bpr * N / (ms * 1e-3) / 3.35e12, 4), unit_route_ms=round(ms_u, 4),
+                                               unit_route_launches=p, speedup_vs_unit_route=round(ms_u / ms, 2),
+                                               kernel=rob.rne_kernel_info("rne_regressor", dt)))
+                for hu in units:
+                    Lr.b2k_rne_destroy(hu)
+                del Y, outs
+            if want(c_gram):
+                G = torch.empty((p, p), dtype=torch.float64, device=dev)
+                b = torch.empty(p, dtype=torch.float64, device=dev)
+                s = torch.empty(1, dtype=torch.float64, device=dev)
+                ms = timeit(lambda i: rtb._lib.check(Lr.b2k_rne_regressor_gram(hr, code, q0.data_ptr(), qd0.data_ptr(), qdd0.data_ptr(), tau0.data_ptr(),
+                                                                               N, rtb._lib.dptr(gr), None, G.data_ptr(), b.data_ptr(), s.data_ptr(), str_)), 1)
+                flops = 2 * (n * p * p / 2) * N
+                report(c_gram, ms, N, 4 * n * es, dict(card, fp64_tflops=round(flops / (ms * 1e-3) / 1e12, 2),
+                                                      frac_of_34TFLOPs=round(flops / (ms * 1e-3) / 34e12, 4)))
+            del q0, qd0, qdd0, tau0
