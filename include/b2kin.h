@@ -487,6 +487,20 @@ int b2k_ikine_6s(int dtype, const double *dh, const double *base, const double *
  *        nearer the first axis than |d2 + d3 + d4| or when the elbow cosine exceeds 1 by more than 64 eps of dtype. */
 int b2k_ikine_ur(int dtype, const double *dh, const double *base, const double *tool, const void *T, int64_t N, int nconf,
                  const int32_t *conf, void *q, int32_t *ok, void *stream);
+/* b2k_ikine_panda is the same for Panda-type 7R arms at a given q7 (DHRobot.ikine_panda; the reference has no
+ * counterpart): the analytic joint solution of a modified-DH 7R arm with joint 7's coordinate fixed per row, no iteration.
+ *   dh   host (7,4) rows of (d, a, alpha, offset), link k = Rx(alpha_k) Tx(a_k) Rz(q_k + offset_k) Tz(d_k).  The pattern,
+ *        each condition to 1e-9: alpha2 .. alpha6 = (-pi/2, +pi/2, +pi/2, -pi/2, +pi/2), a2 = a3 = a6 = 0,
+ *        d2 = d4 = d6 = 0, hypot(a4, d3) != 0, hypot(a5, d5) != 0 (PandaMDH).  Anything else is B2K_ERR_INVALID.
+ *   q7   (N,) device array of dtype, aligned to its element size, non-NULL when N > 0: q[.., 6] of every solution of
+ *        the row, as given.  A non-finite q7 gives a NaN row with ok = 0.
+ *   conf bit 0 set = shoulder right ("r": sin(theta2) >= 0), bit 1 set = elbow down ("d"; "u" = ((O2 - O4) x
+ *        (O6 - O4)) . z4 >= 0), bit 2 set = wrist flipped ("f"; "n" = (O2 - O6) . x5 >= 0)
+ *   q    (N,nconf,7) joints 1..6 wrapped into [-pi, pi) and q7; NaN where out of reach
+ *   base, tool, T, ok, the validation and the N = 0 rule as for b2k_ikine_6s.  A row is out of reach when the elbow
+ *        cosine exceeds 1 by more than 64 eps of dtype, or when the wrist needs |p| > h + 64 eps |O6 - O2| (DESIGN f-17). */
+int b2k_ikine_panda(int dtype, const double *dh, const double *base, const double *tool, const void *T, const void *q7,
+                    int64_t N, int nconf, const int32_t *conf, void *q, int32_t *ok, void *stream);
 
 /* ---------------------------------------------------------------- pure functions of the Jacobian
  * The six functions below take a batch of Jacobians J (N,6,n), n = 1..B2K_MAX_JOINTS.  J, qd and the output must be

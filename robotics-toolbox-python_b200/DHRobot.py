@@ -5,7 +5,7 @@ Mirrors the hot-path part of the reference's ``DHRobot`` (reference
 src/roboticstoolbox/robot/DHRobot.py): ``ets()`` 878-918, ``fkine`` 920-979, ``jacobe`` 1066-1140,
 ``jacob0`` 1142-1198, ``rne`` 1373-1456 with its parameter packing ``_init_rne`` 1340-1361 and
 dirty tracking (DHLink.py:24-51), ``ikine_LM`` 2454-2474, and the closed-form ``ikine_6s`` as ``ikine_a``; ``ikine_ur``
-is the closed form of UR-type arms, which the reference lacks.
+and ``ikine_panda`` are the closed forms of UR-type arms and of Panda-type arms at a given q7, which the reference lacks.
 """
 from __future__ import annotations
 
@@ -192,7 +192,7 @@ class DHRobot:
         q1, q2 = self.ikine_LM(T1, **kwargs), self.ikine_LM(T2, **kwargs)
         return _jtraj(q1.q, q2.q, t, device=device)
 
-    # ---- closed-form inverse kinematics (reference DHRobot.ikine_6s, which Puma560.ikine_a calls; and UR-type arms):
+    # ---- closed-form inverse kinematics (reference DHRobot.ikine_6s, which Puma560.ikine_a calls; UR- and Panda-type arms):
     # csrc/b2k_ik6s.cu
     _IKINE_A_LETTERS = ("lr", "ud", "nf")
 
@@ -215,13 +215,14 @@ class DHRobot:
             out += given.pop() if given else pair[0]
         return out
 
-    def _ikine_a_table(self, method="ikine_a") -> np.ndarray:
-        """(6,4) rows of (d, a, alpha, offset) for b2k_ikine_6s / b2k_ikine_ur, after the checks their tables cannot
-        express; ``method`` names the caller in the messages"""
-        if self.n != 6:
-            raise ValueError(f"{method}: the closed form serves 6-joint arms; this robot has {self.n} joints")
-        if self.mdh:
-            raise ValueError(f"{method}: the closed form serves standard DH; this robot uses modified DH")
+    def _ikine_a_table(self, method="ikine_a", n=6, mdh=False) -> np.ndarray:
+        """(n,4) rows of (d, a, alpha, offset) for b2k_ikine_6s / b2k_ikine_ur (n = 6, standard DH) or b2k_ikine_panda
+        (n = 7, modified DH), after the checks their tables cannot express; ``method`` names the caller in the messages"""
+        if self.n != n:
+            raise ValueError(f"{method}: the closed form serves {n}-joint arms; this robot has {self.n} joints")
+        if bool(self.mdh) != mdh:
+            have, want = ("modified DH", "standard DH") if self.mdh else ("standard DH", "modified DH")
+            raise ValueError(f"{method}: the closed form serves {want}; this robot uses {have}")
         for j, l in enumerate(self.links):
             if not l.isrevolute:
                 raise ValueError(f"{method}: joint {j + 1} is prismatic; the closed form needs revolute joints")
@@ -256,8 +257,28 @@ class DHRobot:
         placement and the reason strings are those of :meth:`ikine_a`.  Joint limits are not applied."""
         return self._ikine_closed(T, config, dtype, "b2k_ikine_ur", "ikine_ur")
 
-    def _ikine_closed(self, T, config, dtype, entry, method) -> IKSolution:
-        """The body of ikine_a and ikine_ur: ``entry`` is the C entry point, ``method`` names the caller in messages"""
+    def ikine_panda(self, T, q7, config="lun", dtype=None) -> IKSolution:
+        """Analytic inverse kinematics of a Panda-type 7R arm (Franka Emika Panda, :class:`models.PandaMDH`, and any arm of
+        its link pattern) at a given last joint coordinate q7: the exact joint solution for a shoulder (l / r), elbow
+        (u / d) and wrist (n / f) configuration, up to eight per pose, with no iteration.  Fixing q7 makes the 7R arm's
+        one-parameter family of solutions finite; sweeping q7 over a batch explores its redundancy.
+
+        The robot must be a modified-DH, all-revolute, unflipped 7-joint arm with alpha2 .. alpha6 = (-pi/2, pi/2, pi/2,
+        -pi/2, pi/2), a2 = a3 = a6 = 0, d2 = d4 = d6 = 0, hypot(a4, d3) != 0 and hypot(a5, d5) != 0; any other robot
+        raises ValueError naming what breaks the pattern.  a1, alpha1, d1, d3, a4, a5, d5, a7, alpha7, d7, the offsets,
+        the base and the tool are free.  ``q7`` is a scalar or one value per pose, (N,) numpy or a CUDA tensor; it is
+        q[6] of every returned solution as given, and a non-finite q7 gives a NaN row.  The letters are predicates of
+        the solution, with O_k and x_k, z_k the origin and axes of link frame k: ``r`` iff sin(theta2) >= 0 (at
+        sin(theta2) = 0 both shoulder codes return theta2 = atan2(R13, R33) within rounding of 0, so both read as ``r``),
+        ``u`` iff ((O2 - O4) x (O6 - O4)) . z4 >= 0, ``n`` iff (O2 - O6) . x5 >= 0.  q has 7 columns: (7,), (N,7),
+        (k,7) or (N,k,7); otherwise inputs, outputs, shapes, dtypes, placement and the reason strings are those of
+        :meth:`ikine_a`.  Joint limits are not applied."""
+        return self._ikine_closed(T, config, dtype, "b2k_ikine_panda", "ikine_panda", q7=q7)
+
+    def _ikine_closed(self, T, config, dtype, entry, method, q7=None) -> IKSolution:
+        """The body of ikine_a, ikine_ur and ikine_panda: ``entry`` is the C entry point, ``method`` names the caller in
+        messages, ``q7`` is given for the 7R entry point only"""
+        seven = entry == "b2k_ikine_panda"
         configs = [config] if isinstance(config, str) else list(config)
         if not 1 <= len(configs) <= 8:
             raise ValueError(f"{method}: give 1 to 8 configurations, got {len(configs)}")
@@ -266,13 +287,15 @@ class DHRobot:
             v = self.config_validate(c, self._IKINE_A_LETTERS)
             codes.append(int(v[0] == "r") | int(v[1] == "d") << 1 | int(v[2] == "f") << 2)
         conf = np.array(codes, dtype=np.int32)
-        dh = self._ikine_a_table(method)
+        dh = self._ikine_a_table(method, 7, True) if seven else self._ikine_a_table(method)
         base = None if np.array_equal(self._base, np.eye(4)) else np.ascontiguousarray(self._base)
         tool = None if np.array_equal(self._tool, np.eye(4)) else np.ascontiguousarray(self._tool)
         solve = getattr(_lib.lib(), entry)
         cp = conf.ctypes.data_as(_lib.ip)
+        no_q7 = (None,) if seven else ()
         # the link pattern is checked by the C entry point; N = 0 validates without touching a device
-        _lib.check(solve(_lib.F64, _lib.dptr(dh), _lib.dptr(base), _lib.dptr(tool), None, 0, len(conf), cp, None, None, None))
+        _lib.check(solve(_lib.F64, _lib.dptr(dh), _lib.dptr(base), _lib.dptr(tool), None, *no_q7, 0, len(conf), cp, None, None,
+                         None))
         T = getattr(T, "A", T)
         B.check_numeric(T, "T")
         if not B.is_tensor(T):
@@ -283,10 +306,11 @@ class DHRobot:
         dt = B.pick_dtype(T, dtype)
         Td = B.to_device(T, dt).reshape(-1, 4, 4).contiguous()
         N, k = Td.shape[0], len(conf)
-        q = B.empty((N, k, 6), dt, like=Td)
+        q7d = (self._ikine_q7(q7, N, dt, Td, method),) if seven else ()
+        q = B.empty((N, k, dh.shape[0]), dt, like=Td)
         ok = B.empty_i32((N, k), like=Td)
-        _lib.check(solve(B.code(dt), _lib.dptr(dh), _lib.dptr(base), _lib.dptr(tool), B.ptr(Td), N, k, cp, B.ptr(q), B.ptr(ok),
-                         B.stream_ptr(Td)))
+        _lib.check(solve(B.code(dt), _lib.dptr(dh), _lib.dptr(base), _lib.dptr(tool), B.ptr(Td), *map(B.ptr, q7d), N, k, cp,
+                         B.ptr(q), B.ptr(ok), B.stream_ptr(Td)))
         reached = B.to_host(ok).astype(bool)
         if not B.is_tensor(T):
             q = B.to_host(q)
@@ -303,6 +327,25 @@ class DHRobot:
             what = "rows" if isinstance(config, str) else "solutions"
             reason = f"Out of reach: {missed} of {reached.size} {what}"
         return IKSolution(q=q, success=missed == 0, reason=reason)
+
+    @staticmethod
+    def _ikine_q7(q7, N, dt, Td, method):
+        """q7 as a contiguous (N,) tensor of dtype dt on the device of Td: a scalar is repeated, an array must be (N,)"""
+        B.check_numeric(q7, "q7")
+        if B.is_tensor(q7):
+            if q7.is_cuda and q7.device != Td.device:
+                raise ValueError(f"{method}: q7 is on {q7.device}, T on {Td.device}")
+            if q7.ndim == 0:
+                q7 = float(q7)
+        else:
+            q7 = np.asarray(q7)
+            if q7.ndim == 0:
+                q7 = float(q7)
+        if isinstance(q7, float):
+            return B.torch().full((N,), q7, dtype=B.tdtype(dt), device=Td.device)
+        if tuple(q7.shape) != (N,):
+            raise ValueError(f"{method}: q7 must be a scalar or have shape ({N},), one value per pose; got {tuple(q7.shape)}")
+        return B.to_device(q7, dt, device=Td.device)
 
     def ik_NR(self, Tep, **kwargs):
         return self.ets().ik_NR(Tep, **kwargs)

@@ -94,6 +94,7 @@ _PROTOS = {
     "b2k_opspace_xdd": (C.c_int, [C.c_int, C.c_int, vp, vp, vp, vp, i64, vp, vp]),
     "b2k_ikine_6s": (C.c_int, [C.c_int, dp, dp, dp, vp, i64, C.c_int, ip, vp, vp, vp]),
     "b2k_ikine_ur": (C.c_int, [C.c_int, dp, dp, dp, vp, i64, C.c_int, ip, vp, vp, vp]),
+    "b2k_ikine_panda": (C.c_int, [C.c_int, dp, dp, dp, vp, vp, i64, C.c_int, ip, vp, vp, vp]),
     "b2k_p_servo_rpy": (C.c_int, [C.c_int, vp, vp, i64, i64, dp, C.c_double, vp, vp, vp]),
     "b2k_ctraj": (C.c_int, [C.c_int, dp, dp, vp, i64, vp, vp]),
     "b2k_mstraj": (C.c_int, [C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int64), C.POINTER(C.c_int64), ip, dp, dp, dp, dp, i64, vp, vp]),

@@ -538,6 +538,67 @@ if want("ikine_ur_"):
             del qi, oki
     del Tq, T64
 
+# Closed-form IK of Panda-type arms at a given q7 (b2k_ikine_panda) of PandaMDH on device-resident poses and q7, with the
+# card context of the blocks above, so that `--only ikine_` times all three kernels in one run.  Bytes per row = T and q7
+# in, q and the ok flags out: (16 + 1 + 7k) reals + 4k for k configurations.  For context per solved pose, ik_LM (the
+# public call, joint limits on) and ikine_panda with all eight configurations are timed on the same --ik-rows reachable
+# targets, ikine_panda at each target's own q7.
+if want("ikine_panda_"):
+    import subprocess
+
+    try:
+        plim = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True,
+                              text=True, timeout=30).stdout.strip()
+    except Exception as e:  # the figure is context, the timing does not depend on it
+        plim = f"unavailable ({type(e).__name__})"
+    card = {"gpu": torch.cuda.get_device_name(0), "power_limit": plim}
+    pmdh = rtb.models.PandaMDH()
+    NI = args.rows
+    Qp = torch.from_numpy(rng.uniform(-np.pi, np.pi, (NI, 7))).to(dev)
+    T64, q764 = pmdh.ets().eval(Qp), Qp[:, 6].contiguous()
+    Li = rtb._lib.lib()
+    sti = torch.cuda.current_stream().cuda_stream
+    dhi = np.ascontiguousarray([[l.d, l.a, l.alpha, l.offset] for l in pmdh.links], dtype=np.float64)
+    tl = np.ascontiguousarray(pmdh._tool)
+    for dt, tag in ((np.float64, "f64"), (np.float32, "f32")):
+        Ti, q7i = (T64, q764) if dt == np.float64 else (T64.float(), q764.float())
+        sz = np.dtype(dt).itemsize
+        for nc in (1, 8):
+            case = f"ikine_panda_pandamdh_{nc}conf_{tag}"
+            if not want(case):
+                continue
+            bpr = (16 + 1 + 7 * nc) * sz + 4 * nc
+            conf = np.arange(nc, dtype=np.int32)
+            qi = torch.empty((NI, nc, 7), dtype=Ti.dtype, device=dev)
+            oki = torch.empty((NI, nc), dtype=torch.int32, device=dev)
+            code = rtb._lib.F64 if dt == np.float64 else rtb._lib.F32
+            ms = timeit(lambda i: rtb._lib.check(Li.b2k_ikine_panda(code, rtb._lib.dptr(dhi), None, rtb._lib.dptr(tl), Ti.data_ptr(),
+                                                                    q7i.data_ptr(), NI, nc, conf.ctypes.data_as(rtb._lib.ip),
+                                                                    qi.data_ptr(), oki.data_ptr(), sti)), 1)
+            report(case, ms, NI, bpr, dict(card, api="C ABI, poses and q7 on the device", frac_of_3350=round(bpr * NI / (ms * 1e-3) / 3.35e12, 4),
+                                           solved=float(oki.float().mean())))
+            del qi, oki
+    del Qp, T64, q764
+    case = "ikine_panda_vs_ik_lm_pandamdh_f64"
+    if want(case):
+        M = args.ik_rows
+        ql = pmdh.qlim
+        Qm = torch.from_numpy(np.random.default_rng(2).uniform(ql[0], ql[1], (M, 7))).to(dev)
+        Tm = pmdh.ets().eval(Qm)
+        q7m = Qm[:, 6].contiguous()
+        eight = ["lun", "run", "ldn", "rdn", "luf", "ruf", "ldf", "rdf"]
+        lm_ms = timeit(lambda i: pmdh.ik_LM(Tm), 1)
+        okv = pmdh.ik_LM(Tm)[1]
+        lm_ok = float((okv.cpu().numpy() if hasattr(okv, "cpu") else np.asarray(okv)).mean())
+        cf_ms = timeit(lambda i: pmdh.ikine_panda(Tm, q7m, config=eight), 1)
+        cf = pmdh.ikine_panda(Tm, q7m, config=eight)
+        cf_ok = float((~torch.isnan(cf.q[:, :, 0])).any(1).float().mean())
+        report(case, cf_ms, M, (16 + 1 + 56) * 8 + 32,
+               dict(card, api="public Python calls on device-resident targets", ik_lm_ms=round(lm_ms, 4), ik_lm_solved=lm_ok,
+                    ik_lm_us_per_solved_pose=round(lm_ms * 1e3 / max(lm_ok * M, 1), 5), ikine_panda_solved=cf_ok,
+                    ikine_panda_us_per_solved_pose=round(cf_ms * 1e3 / max(cf_ok * M, 1), 5)))
+        del Qm, Tm, q7m, cf
+
 # IK (config 4): reachable targets, chan
 if want("ik_"):
     panda = rtb.models.Panda().ets()
