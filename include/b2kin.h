@@ -331,6 +331,28 @@ int b2k_tree_dyn(b2k_tree_t tree, int op, int dtype, const void *in0, const void
 #define B2K_DYN_ACCEL_DERIV 8
 int b2k_tree_derivatives(b2k_tree_t tree, int op, int dtype, const void *q, const void *qd, const void *x, int64_t N,
                          const double *grav, void *out0, void *out1, void *out2, void *stream);
+/* The dynamics regressor of a tree, for identifying its inertial parameters from logged (q, qd, qdd, tau):
+ * tau = Y(q, qd, qdd; g) pi exactly, for any rigid-body group inertia.  pi has p = 10 n entries, 10 per joint group in
+ * group order (the order of b2k_tree_rne's tau):  pi[10j .. 10j+9] = [m, hx, hy, hz, Ixx, Iyy, Izz, Ixy, Iyz, Ixz]
+ * with I6[j] = [[m E, -[h]x], [[h]x, Ib]], Ib = [[Ixx, Ixy, Ixz], [Ixy, Iyy, Iyz], [Ixz, Iyz, Izz]] (for point masses
+ * h = sum m r, Ib = sum m (r.r E - r r^T)).  Y[i, 10k .. 10k+9] is exact 0 unless group k is group i or hangs below it.
+ * Y does not depend on I6.  There are no friction or motor columns: b2k_tree_rne has no such terms.
+ *   b2k_tree_regressor       Y (N, n, 10n) row-major, one launch of a kernel generated for the tree (NVRTC, op code
+ *                            B2K_DYN_REGRESSOR); grav = MINUS the robot's gravity, as for b2k_tree_rne.  q, qd, qdd, Y
+ *                            device, 16-byte aligned.
+ *   b2k_tree_regressor_gram  the normal equations, always in fp64, without Y existing in full: G (p, p) = sum Y^T W Y,
+ *                            b (p) = sum Y^T W tau, s (1) = sum tau^T W tau, W = diag(weights) (host, n values in group
+ *                            order, finite and >= 0; NULL = all 1).  tau (N, n) has the compute type and group order.
+ *                            G is exactly symmetric and equal calls give equal bits.  G, b, s are device arrays, 8-byte
+ *                            aligned, written also for N = 0 (zeros, no kernel).
+ * b2k_tree_dyn and b2k_tree_derivatives reject B2K_DYN_REGRESSOR; b2k_tree_codegen / b2k_tree_info take it (the generated
+ * function, rne_regressor_row(..., i, y), writes joint row i of Y).  Every argument is checked before any CUDA call. */
+#define B2K_DYN_REGRESSOR 10
+int b2k_tree_regressor(b2k_tree_t tree, int dtype, const void *q, const void *qd, const void *qdd, int64_t N,
+                       const double *grav, void *Y, void *stream);
+int b2k_tree_regressor_gram(b2k_tree_t tree, int dtype, const void *q, const void *qd, const void *qdd, const void *tau,
+                            int64_t N, const double *grav, const double *weights, double *G, double *b, double *s,
+                            void *stream);
 int b2k_tree_codegen(b2k_tree_t tree, int op, int grav_mask, char *src, int64_t src_cap, double *consts, int32_t consts_cap,
                      int32_t *n_consts, int32_t *counts);
 int b2k_tree_info(b2k_tree_t tree, int op, int dtype, const double *grav, char *buf, int64_t cap);

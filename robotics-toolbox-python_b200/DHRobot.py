@@ -10,12 +10,12 @@ and ``ikine_panda`` are the closed forms of UR-type arms and of Panda-type arms 
 from __future__ import annotations
 
 import ctypes as C
-from collections import namedtuple
 from typing import List, Optional
 
 import numpy as np
 
 from . import _buffers as B
+from . import _identify
 from . import _lib
 from . import _opspace
 from . import _static
@@ -24,9 +24,7 @@ from .DHLink import DHLink
 from .ET import ET
 from .ETS import ETS, _mat44
 from .IK import IKSolution
-
-
-IdentifyResult = namedtuple("IdentifyResult", "pi rank rms")
+from ._identify import IdentifyResult  # noqa: F401  (the result type of identify)
 
 
 class DHRobot:
@@ -724,23 +722,7 @@ class DHRobot:
         if not friction:
             for j in range(n):
                 keep[14 * j + 10:14 * j + 14] = False
-        # A column at the rounding level of the compute type is a zero column: a structurally zero term that the link
-        # constants (cos(pi/2) = 6e-17) or cancelling products leave a few ulps off 0 would otherwise become a unit
-        # column after the scaling below.  The cut, 16 eps of the largest column norm (2e-6 in float32), sits well
-        # below real columns: on Puma560 inertial columns are 4e-5 of the armature columns (G^2 qdd).
-        eps = np.finfo(B.pick_dtype(q, dtype)).eps
-        keep &= np.diag(G) > (16 * eps) ** 2 * np.max(np.diag(G), initial=0.0)
-        pi = np.zeros(14 * n)
-        rank = 0
-        if keep.any():
-            Gk, bk = G[np.ix_(keep, keep)], b[keep]
-            d = 1.0 / np.sqrt(np.diag(Gk))
-            lam, V = np.linalg.eigh(d[:, None] * Gk * d[None, :])
-            use = lam > rcond * lam[-1]
-            rank = int(use.sum())
-            pi[keep] = d * (V[:, use] @ ((V[:, use].T @ (d * bk)) / lam[use]))
-        res = s - 2 * pi @ b + pi @ G @ pi
-        return IdentifyResult(pi, rank, float(np.sqrt(max(res, 0.0) / max(N * n, 1))))
+        return _identify.solve(G, b, s, keep, np.finfo(B.pick_dtype(q, dtype)).eps, rcond, N, n)
 
     # ---- static forces (reference DynamicsMixin, Dynamics.py): _static.py, csrc/b2k_static.cu
     def _static_mass_table(self) -> np.ndarray:

@@ -11,6 +11,7 @@ from typing import List, Optional, Union
 import numpy as np
 
 from . import _buffers as B
+from . import _identify
 from . import _lib
 from . import _opspace
 from . import _static
@@ -496,7 +497,7 @@ class Robot:
         return tau[0] if single else tau
 
     _DYN_OPS = {"rne": 0, "inertia": 1, "gravload": 2, "itorque": 3, "coriolis": 4, "accel": 5, "rne_derivatives": 7,
-                "accel_derivatives": 8}
+                "accel_derivatives": 8, "rne_regressor": 10}
 
     def rne_kernel_info(self, dtype=np.float64, gravity=None, op="rne") -> str:
         g = self._gravity if gravity is None else np.asarray(gravity, dtype=np.float64).reshape(3)
@@ -507,9 +508,8 @@ class Robot:
 
     # ---- dynamics built on the recursion (reference DynamicsMixin, Dynamics.py, which BaseRobot inherits: each method
     #      there is a Python loop of self.rne calls; here one generated kernel per operation, b2k_tree_dyn)
-    def _tree_dyn(self, op, ins, names, out_tail, gravity=None, dtype=None, nout=1):
-        """One generated kernel over rows of `ins`; returns one array of shape (N,) + out_tail, or a tuple of `nout` of
-        them (the derivative operations, b2k_tree_derivatives)."""
+    def _tree_inputs(self, ins, names, dtype):
+        """The rows of `ins` as contiguous (N, n) device tensors of one compute type: (dt, host, single, dev, N)."""
         for x, nm in zip(ins, names):
             B.check_numeric(x, nm)
         n = self.n
@@ -526,11 +526,23 @@ class Robot:
         N = dev[0].shape[0]
         if any(t.shape[0] != N for t in dev):
             raise ValueError(", ".join(names) + " must have the same number of rows")
+        return dt, host, single, dev, N
+
+    def _kernel_gravity(self, gravity):
         g = self._gravity if gravity is None else np.asarray(gravity, dtype=np.float64).reshape(3)
-        ag = np.ascontiguousarray(-g)
+        return np.ascontiguousarray(-g)  # a_grav = -gravity (Robot.py:1785-1788)
+
+    def _tree_dyn(self, op, ins, names, out_tail, gravity=None, dtype=None, nout=1):
+        """One generated kernel over rows of `ins`; returns one array of shape (N,) + out_tail, or a tuple of `nout` of
+        them (the derivative operations, b2k_tree_derivatives)."""
+        dt, host, single, dev, N = self._tree_inputs(ins, names, dtype)
+        ag = self._kernel_gravity(gravity)
         outs = [B.empty((N,) + tuple(out_tail), dt, like=dev[0]) for _ in range(nout)]
         ptrs = [B.ptr(t) for t in dev] + [None] * (3 - len(dev))
-        if op in ("rne_derivatives", "accel_derivatives"):
+        if op == "rne_regressor":
+            _lib.check(_lib.lib().b2k_tree_regressor(self._tree_handle(), B.code(dt), ptrs[0], ptrs[1], ptrs[2], N, _lib.dptr(ag),
+                                                     B.ptr(outs[0]), B.stream_ptr(dev[0])))
+        elif op in ("rne_derivatives", "accel_derivatives"):
             optrs = [B.ptr(o) for o in outs] + [None] * (3 - nout)
             _lib.check(_lib.lib().b2k_tree_derivatives(self._tree_handle(), self._DYN_OPS[op], B.code(dt), ptrs[0], ptrs[1],
                                                        ptrs[2], N, _lib.dptr(ag), *optrs, B.stream_ptr(dev[0])))
@@ -581,6 +593,66 @@ class Robot:
         singular M (a point mass on its own joint axis) gives non-finite rows, as ``accel`` does."""
         return self._tree_dyn("accel_derivatives", (q, qd, torque), ("q", "qd", "torque"), (self.n, self.n), gravity=gravity,
                               dtype=dtype, nout=3)
+
+    # ---- parameter identification: the dynamics regressor of the tree (DESIGN f-18; no reference counterpart)
+    def dynamic_parameters(self) -> np.ndarray:
+        """The (10n,) float64 parameter vector pi that ``rne_regressor`` multiplies: 10 per joint group, in the group order
+        of ``rne``'s torques, ``[m, hx, hy, hz, Ixx, Iyy, Izz, Ixy, Iyz, Ixz]``, read from the group's spatial inertia
+        ``tree_description()["I6"] = [[m E, -[h]x], [[h]x, Ib]]`` in the joint link's frame.  As ``rne`` builds I6 from the
+        links' masses and centres of mass only, h = sum m r and Ib = sum m (r.r E - r r^T) over the group's links."""
+        pi = []
+        for I6 in self.tree_description()["I6"]:
+            pi += [I6[0, 0], I6[5, 1], I6[3, 2], I6[4, 0], I6[3, 3], I6[4, 4], I6[5, 5], I6[3, 4], I6[4, 5], I6[3, 5]]
+        return np.array(pi, dtype=np.float64)
+
+    def rne_regressor(self, q, qd, qdd, gravity=None, dtype=None):
+        """The dynamics regressor Y(q, qd, qdd): (n, 10n) for one state or (N, n, 10n), with
+        ``Y @ dynamic_parameters() == rne(q, qd, qdd, gravity=gravity)``.  Row i is joint group i's torque as ``rne``
+        orders it; column 10k + c is that torque per unit of parameter c of group k, exact 0 unless group k is group i or
+        hangs below it.  The identity holds for any rigid-body group inertia, not only the point masses ``rne`` builds.
+        Y depends on the kinematics alone, not on the masses.  Input forms, dtype and device rules are those of
+        ``rne_derivatives``; one launch of a kernel generated for this robot."""
+        return self._tree_dyn("rne_regressor", (q, qd, qdd), ("q", "qd", "qdd"), (self.n, 10 * self.n), gravity=gravity,
+                              dtype=dtype)
+
+    def regressor_gram(self, q, qd, qdd, tau, gravity=None, weights=None, dtype=None):
+        """The normal equations of identification, accumulated on the device without Y existing in full: numpy
+        ``(G, b, s)`` with G (10n, 10n) = sum Y^T W Y, b (10n,) = sum Y^T W tau and the float s = sum tau^T W tau over the
+        rows, W = diag(weights) (n weights >= 0 in group order, default 1), always in float64.  q, qd, qdd, tau (N, n) or
+        (n,), numpy or CUDA tensors, tau in the group order of ``rne``; Y is computed in ``dtype`` (default: that of q) in
+        chunks of 4096 rows.  G is exactly symmetric and two equal calls give equal bits."""
+        import torch
+
+        n, p = self.n, 10 * self.n
+        dt, _, _, dev, N = self._tree_inputs((q, qd, qdd, tau), ("q", "qd", "qdd", "tau"), dtype)
+        w = None
+        if weights is not None:
+            w = np.ascontiguousarray(np.asarray(weights, dtype=np.float64))
+            if w.shape != (n,):
+                raise ValueError(f"weights must have shape ({n},); got {w.shape}")
+        G = torch.empty((p, p), dtype=torch.float64, device=dev[0].device)
+        b = torch.empty(p, dtype=torch.float64, device=dev[0].device)
+        s = torch.empty(1, dtype=torch.float64, device=dev[0].device)
+        _lib.check(_lib.lib().b2k_tree_regressor_gram(self._tree_handle(), B.code(dt), *(B.ptr(t) for t in dev), N,
+                                                      _lib.dptr(self._kernel_gravity(gravity)), _lib.dptr(w), B.ptr(G),
+                                                      B.ptr(b), B.ptr(s), B.stream_ptr(dev[0])))
+        return G.cpu().numpy(), b.cpu().numpy(), float(s.item())
+
+    def identify(self, q, qd, qdd, tau, gravity=None, weights=None, rcond=1e-10, dtype=None):
+        """Least-squares identification of the groups' inertial parameters from logged (q, qd, qdd, tau): the named tuple
+        ``(pi, rank, rms)``, solved as ``DHRobot.identify`` solves it.  pi (10n,) is the minimum-norm solution of
+        tau = Y pi in the convention of ``dynamic_parameters``, from the normal equations of ``regressor_gram``: G is
+        scaled to unit diagonal, and eigenvalues below ``rcond`` times the largest are dropped; rank is the number kept.
+        The default rcond suits float64; float32 needs about 1e-5.  Parameters whose column of Y is zero (below 16 eps
+        of the compute type times the largest column norm) get 0.  rms is the weighted residual
+        sqrt((s - 2 pi.b + pi.G.pi) / (N n)), not resolved below about sqrt(eps) times the rms of tau.  Only
+        combinations of parameters are identifiable in general; base parameters and writing pi back into the links are
+        left to the caller (a point-mass link cannot hold Ib)."""
+        G, b, s = self.regressor_gram(q, qd, qdd, tau, gravity=gravity, weights=weights, dtype=dtype)
+        shape = tuple(q.shape) if hasattr(q, "shape") else np.shape(q)
+        N = 1 if len(shape) == 1 else int(shape[0])
+        return _identify.solve(G, b, s, np.ones(10 * self.n, dtype=bool), np.finfo(B.pick_dtype(q, dtype)).eps, rcond, N,
+                               self.n)
 
     # ---- operational-space dynamics (reference DynamicsMixin, Dynamics.py between gravload and itorque): _opspace.py
     def _opspace_robot(self):

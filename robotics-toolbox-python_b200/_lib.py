@@ -65,6 +65,8 @@ _PROTOS = {
     "b2k_tree_rne": (C.c_int, [vp, C.c_int, vp, vp, vp, i64, dp, vp, vp]),
     "b2k_tree_dyn": (C.c_int, [vp, C.c_int, C.c_int, vp, vp, vp, i64, dp, vp, vp]),
     "b2k_tree_derivatives": (C.c_int, [vp, C.c_int, C.c_int, vp, vp, vp, i64, dp, vp, vp, vp, vp]),
+    "b2k_tree_regressor": (C.c_int, [vp, C.c_int, vp, vp, vp, i64, dp, vp, vp]),
+    "b2k_tree_regressor_gram": (C.c_int, [vp, C.c_int, vp, vp, vp, vp, i64, dp, dp, vp, vp, vp, vp]),
     "b2k_tree_codegen": (C.c_int, [vp, C.c_int, C.c_int, C.c_char_p, i64, dp, C.c_int32, ip, ip]),
     "b2k_tree_info": (C.c_int, [vp, C.c_int, C.c_int, dp, C.c_char_p, i64]),
     "b2k_rne_inertia": (C.c_int, [vp, C.c_int, vp, i64, vp, vp]),

@@ -136,25 +136,30 @@ struct b2k_rne_s {
 // Operations on an rne handle.  B2K_GEN_RNE..B2K_GEN_RNE_WRENCH are served by the robot-specialised kernels
 // (b2k_rne_gen.cpp, b2k_rne_spec.cu) on the full 32-row tiles and by the generic ones (b2k_rne.cuh) on the rest; the
 // derivatives of DH arms only by the generic ones, those of trees by the generated kernels.  RNE..ACCEL, RNE_DERIV and
-// ACCEL_DERIV are also the public B2K_DYN_* codes of the tree entry points.  RNE_REGRESSOR (DH arms only, generic kernel
-// only) is no tree operation: the tree entry points reject its code.
+// ACCEL_DERIV are also the public B2K_DYN_* codes of the tree entry points.  The regressors are one operation per robot
+// kind: RNE_REGRESSOR (DH arms, 14 parameters per link, generic kernel only) is no tree operation, and TREE_REGRESSOR
+// (B2K_DYN_REGRESSOR: trees, 10 parameters per joint group, generated kernel only) is no DH operation; each robot kind's
+// entry points reject the other's code.
 enum { B2K_GEN_RNE = 0, B2K_GEN_INERTIA = 1, B2K_GEN_GRAVLOAD = 2, B2K_GEN_ITORQUE = 3, B2K_GEN_CORIOLIS = 4, B2K_GEN_ACCEL = 5,
-       B2K_GEN_RNE_WRENCH = 6, B2K_GEN_RNE_DERIV = 7, B2K_GEN_ACCEL_DERIV = 8, B2K_GEN_RNE_REGRESSOR = 9, B2K_GEN_NOPS = 10 };
+       B2K_GEN_RNE_WRENCH = 6, B2K_GEN_RNE_DERIV = 7, B2K_GEN_ACCEL_DERIV = 8, B2K_GEN_RNE_REGRESSOR = 9,
+       B2K_GEN_TREE_REGRESSOR = 10, B2K_GEN_NOPS = 11 };
 static_assert(B2K_GEN_RNE == B2K_DYN_RNE && B2K_GEN_INERTIA == B2K_DYN_INERTIA && B2K_GEN_GRAVLOAD == B2K_DYN_GRAVLOAD &&
                   B2K_GEN_ITORQUE == B2K_DYN_ITORQUE && B2K_GEN_CORIOLIS == B2K_DYN_CORIOLIS && B2K_GEN_ACCEL == B2K_DYN_ACCEL &&
-                  B2K_GEN_RNE_DERIV == B2K_DYN_RNE_DERIV && B2K_GEN_ACCEL_DERIV == B2K_DYN_ACCEL_DERIV,
+                  B2K_GEN_RNE_DERIV == B2K_DYN_RNE_DERIV && B2K_GEN_ACCEL_DERIV == B2K_DYN_ACCEL_DERIV &&
+                  B2K_GEN_TREE_REGRESSOR == B2K_DYN_REGRESSOR,
               "B2K_DYN_* (b2kin.h) are the B2K_GEN_* codes of the tree operations");
 
 // What an operation reads and writes.  Every input is an (N, n) array; every output has rows of n or n * n reals, except
-// the base wrench, the (N, 6) second output of B2K_GEN_RNE_WRENCH, and the regressor, (N, n, 14 n).
+// the base wrench, the (N, 6) second output of B2K_GEN_RNE_WRENCH, and the regressors, (N, n, k n) with k parameters per
+// link (14 DH, 10 tree).
 struct b2k_rne_op_s {
     int nin, nout;          // input / output arrays
     bool square;            // output rows of n * n reals
     bool wrench;            // the second output is the base wrench
     bool grav, fext;        // reads the gravity vector / the tip wrench
     const char *in[3], *out[3]; // argument names, as the error messages print them
-    bool regressor = false;     // output rows of n * 14 n reals
-    constexpr int out_row(int o, int n) const { return regressor ? 14 * n * n : (wrench && o == 1 ? 6 : (square ? n * n : n)); }
+    int regressor = 0;          // a regressor: parameters per link, output rows of n * regressor * n reals
+    constexpr int out_row(int o, int n) const { return regressor ? regressor * n * n : (wrench && o == 1 ? 6 : (square ? n * n : n)); }
 };
 inline constexpr b2k_rne_op_s B2K_RNE_OPS[B2K_GEN_NOPS] = {
     {3, 1, false, false, true, true, {"q", "qd", "qdd"}, {"tau"}},                                     // RNE
@@ -166,7 +171,8 @@ inline constexpr b2k_rne_op_s B2K_RNE_OPS[B2K_GEN_NOPS] = {
     {3, 2, false, true, true, true, {"q", "qd", "qdd"}, {"tau", "wbase"}},                            // RNE_WRENCH
     {3, 2, true, false, true, true, {"q", "qd", "qdd"}, {"dtau_dq", "dtau_dqd"}},                     // RNE_DERIV
     {3, 3, true, false, true, false, {"q", "qd", "torque"}, {"dqdd_dq", "dqdd_dqd", "dqdd_dtau"}},    // ACCEL_DERIV
-    {3, 1, false, false, true, false, {"q", "qd", "qdd"}, {"Y"}, true},                               // RNE_REGRESSOR
+    {3, 1, false, false, true, false, {"q", "qd", "qdd"}, {"Y"}, 14},                                 // RNE_REGRESSOR
+    {3, 1, false, false, true, false, {"q", "qd", "qdd"}, {"Y"}, 10},                                 // TREE_REGRESSOR
 };
 
 // The arrays of one launch of an operation, device pointers: unused entries are NULL
@@ -183,6 +189,9 @@ void b2k_rne_spec_detach(b2k_rne_s *r);
 // or a negative b2k_status.  out2: the base wrench (nrows, 6) of B2K_GEN_RNE_WRENCH, NULL for every other mode.
 long long b2k_rne_spec_launch(const b2k_rne_s *r, int mode, int dtype, const void *in0, const void *in1, const void *in2,
                               long long nrows, const double *grav, const double *fext, void *out, void *out2, cudaStream_t st);
+// Y (a.out[0]) of a tree's regressor over a.nrows rows of a.in = q, qd, qdd (b2k_rne_spec.cu): the chunks of
+// b2k_tree_regressor_gram, whose arguments are already checked
+int b2k_tree_regressor_rows(b2k_tree_t t, int dtype, const b2k_rne_args &a, cudaStream_t st);
 
 // ---- error plumbing and argument checks (b2k_api.cu)
 void b2k_set_error(const char *fmt, ...);

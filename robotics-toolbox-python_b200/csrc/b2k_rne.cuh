@@ -1176,8 +1176,10 @@ constexpr long long REG_CHUNK = 4096; // rows per chunk: Puma560 fp64 is 16.5 MB
 constexpr int REG_TILE = 32;          // the Gram matrix in 32 x 32 tiles, upper triangle only
 constexpr int REG_KB = 16;            // augmented rows per k-step
 
+constexpr int REG_MAX_ROWS = 16; // joints (DH, up to B2K_MAX_JOINTS) or joint groups (trees, up to 16) per row of the batch
+
 struct RegWeights {
-    double w[B2K_MAX_JOINTS];
+    double w[REG_MAX_ROWS]; // W.w[k % n]: one weight per joint row
 };
 
 // tile pair t (row-major over the upper triangle of an nt x nt tiling) -> (ti, tj), ti <= tj
@@ -1358,21 +1360,24 @@ int rne_generic_launch(const b2k_rne_s *r, int op, const b2k_rne_args &a, cudaSt
 #undef B2K_CASE
 }
 
-// The normal equations of the regressor over a.nrows rows (a.in = q, qd, qdd; grav in a.grav), tau (N, n) of the compute
-// type, w the n joint weights; G (p, p), b (p), s (1) fp64 device arrays, p = 14 n.  b2k_api.cu has checked every
+// The normal equations of a regressor over a.nrows rows (a.in = q, qd, qdd; grav in a.grav), tau (N, n) of the compute
+// type, w the n joint weights; G (p, p), b (p), s (1) fp64 device arrays, p = k n with k parameters per link.  make_y(ca)
+// writes the rows of one chunk (ca.in, ca.nrows) into ca.out[0] = Y (ca.nrows, n, p) and returns a b2k_status: the DH
+// and the tree regressors share the chunks, the slices and the two reduction kernels.  The caller has checked every
 // argument and handles N = 0.
-template <typename real>
-int rne_regressor_gram(const b2k_rne_s *r, const b2k_rne_args &a, const void *tau, const double *w, double *G, double *b,
-                       double *s, cudaStream_t st)
+template <typename real, typename MakeY>
+int regressor_gram(int n, int p, const b2k_rne_args &a, const void *tau, const double *w, double *G, double *b, double *s,
+                   cudaStream_t st, MakeY &&make_y)
 {
-    const int n = r->n, p = 14 * n, nt = (p + 1 + REG_TILE - 1) / REG_TILE, npairs = nt * (nt + 1) / 2;
+    if (n > REG_MAX_ROWS) { b2k_set_error("regressor_gram: %d joint rows exceed %d", n, REG_MAX_ROWS); return B2K_ERR_INVALID; }
+    const int nt = (p + 1 + REG_TILE - 1) / REG_TILE, npairs = nt * (nt + 1) / 2;
     const long long chunk = a.nrows < REG_CHUNK ? a.nrows : REG_CHUNK;
     // slices: about two blocks of 256 threads per SM, each slice at least 4 k-steps of a full chunk
     const long long kmax = (chunk * n + REG_KB - 1) / REG_KB;
     int slices = (2 * b2k_num_sms() + npairs - 1) / npairs;
     if (slices > kmax / 4) slices = (int)(kmax / 4 > 0 ? kmax / 4 : 1);
     RegWeights W;
-    for (int j = 0; j < B2K_MAX_JOINTS; j++) W.w[j] = j < n ? (w ? w[j] : 1.0) : 0.0;
+    for (int j = 0; j < REG_MAX_ROWS; j++) W.w[j] = j < n ? (w ? w[j] : 1.0) : 0.0;
     const size_t ybytes = ((size_t)chunk * n * p * sizeof(real) + 255) & ~(size_t)255;
     const size_t pbytes = (size_t)slices * npairs * REG_TILE * REG_TILE * sizeof(double);
     b2k_keep_mempool();
@@ -1387,7 +1392,7 @@ int rne_regressor_gram(const b2k_rne_s *r, const b2k_rne_args &a, const void *ta
         for (int i = 0; i < 3; i++) ca.in[i] = (const real *)a.in[i] + c0 * n;
         ca.out[0] = Y;
         ca.nrows = rows;
-        rc = rne_generic_launch<real, B2K_GEN_RNE_REGRESSOR>(r, B2K_GEN_RNE_REGRESSOR, ca, st);
+        rc = make_y(ca);
         if (rc) break;
         k_regressor_syrk<real><<<dim3(npairs, slices), 256, 0, st>>>(Y, (const real *)tau + c0 * n, rows * n, n, p, nt, W, part,
                                                                       c0 > 0);
@@ -1405,4 +1410,14 @@ int rne_regressor_gram(const b2k_rne_s *r, const b2k_rne_args &a, const void *ta
     const cudaError_t e = cudaFreeAsync(scratch, st);
     if (rc == B2K_OK && e != cudaSuccess) rc = b2k_cuda_fail(e, "cudaFreeAsync");
     return rc;
+}
+
+// The normal equations of the DH regressor, p = 14 n; b2k_api.cu has checked every argument and handles N = 0.
+template <typename real>
+int rne_regressor_gram(const b2k_rne_s *r, const b2k_rne_args &a, const void *tau, const double *w, double *G, double *b,
+                       double *s, cudaStream_t st)
+{
+    return regressor_gram<real>(r->n, 14 * r->n, a, tau, w, G, b, s, st, [&](const b2k_rne_args &ca) {
+        return rne_generic_launch<real, B2K_GEN_RNE_REGRESSOR>(r, B2K_GEN_RNE_REGRESSOR, ca, st);
+    });
 }

@@ -618,6 +618,7 @@ int b2k_rne_generate(const b2k_rne_s *r, const b2k_gen_opts &o, b2k_gen_out &out
         out.error = "the derivatives of DH arms are served by the generic kernel";
         return -1;
     }
+    if (o.mode == B2K_GEN_TREE_REGRESSOR) { out.error = "the tree regressor is no operation of DH arms"; return -1; }
     const int N = r->n;
     Gen g;
     std::vector<Link> L(N);
@@ -735,39 +736,47 @@ int b2k_tree_generate(const b2k_tree_s *t, const b2k_gen_opts &o, b2k_gen_out &o
         (axis % 3 == 0 ? u.x : (axis % 3 == 1 ? u.y : u.z)) = x;
         return u;
     };
-    // one evaluation of the recursion: in.qd / in.qdd are indexed like q (jindex), the torques come out in group order
-    // (Robot.py:1890-1899); in.grav is a_grav = MINUS the gravity vector (the caller negates), linear part only
-    auto rec = [&](const Inputs &in) {
+    // the motion of group j in its own frame from its parent's: angular / linear velocity w, vl and acceleration aw, av
+    // (spatial, Featherstone's), and p, the origin of the joint frame in the parent's.  in.qd / in.qdd are indexed like q
+    // (jindex); in.grav is a_grav = MINUS the gravity vector (the caller negates), linear part only
+    struct Kin { std::vector<V3> w, vl, aw, av, p; };
+    auto kin = [&](int j, const Inputs &in, Kin &K) {
         const V3 &agrav = in.grav;
-        std::vector<V3> w(N), vl(N), fl(N), fa(N), p(N);
-        std::vector<V3> aw(N), av(N);
+        std::vector<V3> &w = K.w, &vl = K.vl, &aw = K.aw, &av = K.av, &p = K.p;
+        const double *C = t->C[j];
+        const int ax = t->axis[j];
+        const bool rev = ax < 3;
+        const Sym &qdj = in.qd[t->jindex[j]], &qddj = in.qdd[t->jindex[j]];
+        auto RT = [&](const V3 &u) { return T.jointR(ax, st[j], ct[j], T.constR(C, u, true), true); };
+        // p = pc + Rc (e_axis * eta) for a prismatic joint
+        const double pc[3] = {C[3], C[7], C[11]};
+        p[j] = v.cst(pc);
+        if (!rev) p[j] = v.fix(v.add(p[j], T.constR(C, unit(ax, qq[j]), false)));
+        const V3 vJw = rev ? unit(ax, qdj) : v.zero(), vJv = rev ? v.zero() : unit(ax, qdj);
+        const V3 aJw = rev ? unit(ax, qddj) : v.zero(), aJv = rev ? v.zero() : unit(ax, qddj);
+        const int pa = t->parent[j];
+        if (pa < 0) {
+            w[j] = vJw; vl[j] = vJv;
+            aw[j] = aJw;
+            av[j] = v.fix(v.add(RT(agrav), aJv));
+        } else {
+            w[j] = v.fix(v.add(RT(w[pa]), vJw));
+            vl[j] = v.fix(v.add(RT(v.cross_acc(w[pa], p[j], &vl[pa])), vJv));
+            const V3 wxJw = v.cross_acc(w[j], vJw);
+            aw[j] = v.fix(v.add(v.add(RT(aw[pa]), aJw), wxJw));
+            const V3 t1 = RT(v.cross_acc(aw[pa], p[j], &av[pa]));
+            const V3 t2 = v.cross_acc(w[j], vJv, &aJv);
+            const V3 t3 = v.cross_acc(vl[j], vJw, &t2);
+            av[j] = v.fix(v.add(t1, t3));
+        }
+    };
+    // one evaluation of the recursion; the torques come out in group order (Robot.py:1890-1899)
+    auto rec = [&](const Inputs &in) {
+        Kin K{std::vector<V3>(N), std::vector<V3>(N), std::vector<V3>(N), std::vector<V3>(N), std::vector<V3>(N)};
+        std::vector<V3> &w = K.w, &vl = K.vl, &aw = K.aw, &av = K.av, &p = K.p;
+        std::vector<V3> fl(N), fa(N);
         for (int j = 0; j < N; j++) {
-            const double *C = t->C[j];
-            const int ax = t->axis[j];
-            const bool rev = ax < 3;
-            const Sym &qdj = in.qd[t->jindex[j]], &qddj = in.qdd[t->jindex[j]];
-            auto RT = [&](const V3 &u) { return T.jointR(ax, st[j], ct[j], T.constR(C, u, true), true); };
-            // p = pc + Rc (e_axis * eta) for a prismatic joint
-            const double pc[3] = {C[3], C[7], C[11]};
-            p[j] = v.cst(pc);
-            if (!rev) p[j] = v.fix(v.add(p[j], T.constR(C, unit(ax, qq[j]), false)));
-            const V3 vJw = rev ? unit(ax, qdj) : v.zero(), vJv = rev ? v.zero() : unit(ax, qdj);
-            const V3 aJw = rev ? unit(ax, qddj) : v.zero(), aJv = rev ? v.zero() : unit(ax, qddj);
-            const int pa = t->parent[j];
-            if (pa < 0) {
-                w[j] = vJw; vl[j] = vJv;
-                aw[j] = aJw;
-                av[j] = v.fix(v.add(RT(agrav), aJv));
-            } else {
-                w[j] = v.fix(v.add(RT(w[pa]), vJw));
-                vl[j] = v.fix(v.add(RT(v.cross_acc(w[pa], p[j], &vl[pa])), vJv));
-                const V3 wxJw = v.cross_acc(w[j], vJw);
-                aw[j] = v.fix(v.add(v.add(RT(aw[pa]), aJw), wxJw));
-                const V3 t1 = RT(v.cross_acc(aw[pa], p[j], &av[pa]));
-                const V3 t2 = v.cross_acc(w[j], vJv, &aJv);
-                const V3 t3 = v.cross_acc(vl[j], vJw, &t2);
-                av[j] = v.fix(v.add(t1, t3));
-            }
+            kin(j, in, K);
             const double *I6 = t->I6[j];
             const V3 hl = v.fix(v.add(T.mat3(I6, 0, 0, vl[j]), T.mat3(I6, 0, 3, w[j])));
             const V3 ha = v.fix(v.add(T.mat3(I6, 3, 0, vl[j]), T.mat3(I6, 3, 3, w[j])));
@@ -795,11 +804,84 @@ int b2k_tree_generate(const b2k_tree_s *t, const b2k_gen_opts &o, b2k_gen_out &o
         }
         return tau;
     };
+    std::string src;
+    if (o.mode == B2K_GEN_TREE_REGRESSOR) {
+        // The regressor: tau_i = s_i . f_i, and f_i sums the wrenches of group i and of every group below it, carried in by
+        // the backward pass.  So Y[i, 10k + c] is joint i's unit twist s carried OUT to group k (the transpose of the
+        // backward step: s_l' = R^T (s_l + s_a x p), s_a' = R^T s_a) dotted with group k's wrench f = I a + v x* (I v) for
+        // the basis inertia of parameter c.  Written out with A = av + w x vl (the classical acceleration of the origin):
+        //   m: s_l . A      h: s_l x aw + w (s_l . w) - s_l (w . w) + A x s_a      Ib: s_a^T Ib aw + (s_a x w)^T Ib w
+        // One case per joint row i, each with the forward pass of the groups it needs (the ancestors of i, i and its
+        // subtree): the kernel stages and drains Y one joint row at a time, and a forward pass kept live across the rows
+        // would not fit the registers.  Rows of other groups are exact zeros.
+        Inputs in;
+        std::vector<Sym> qdv(N), qddv(N);
+        for (int k = 0; k < N; k++) { qdv[k] = g.var("qd[" + std::to_string(k) + "]"); qddv[k] = g.var("qdd[" + std::to_string(k) + "]"); }
+        in.qd = qdv; in.qdd = qddv;
+        in.grav = {(o.grav_mask & 1) ? g.var("grav[0]") : Gen::zero(), (o.grav_mask & 2) ? g.var("grav[1]") : Gen::zero(),
+                   (o.grav_mask & 4) ? g.var("grav[2]") : Gen::zero()};
+        auto dot = [&](const V3 &a, const V3 &b) { return g.sum({g.mul(a.x, b.x), g.mul(a.y, b.y), g.mul(a.z, b.z)}); };
+        g.code.push_back("    switch (i) {");
+        for (int i = 0; i < N; i++) {
+            std::vector<bool> below(N, false), need(N, false); // group k is i or hangs below it / its motion is needed
+            for (int k = 0; k < N; k++) below[k] = k == i || (t->parent[k] >= 0 && below[t->parent[k]]);
+            for (int k = N - 1; k >= 0; k--)
+                if (below[k] || need[k]) { need[k] = true; if (t->parent[k] >= 0) need[t->parent[k]] = true; }
+            g.code.push_back("    case " + std::to_string(i) + ": {");
+            Kin K{std::vector<V3>(N), std::vector<V3>(N), std::vector<V3>(N), std::vector<V3>(N), std::vector<V3>(N)};
+            std::vector<V3> sl(N), sa(N);
+            for (int k = 0; k < N; k++) {
+                if (!below[k]) {
+                    if (need[k]) kin(k, in, K);
+                    for (int c = 0; c < 10; c++) g.code.push_back("        y[" + std::to_string(10 * k + c) + "] = (real)0;");
+                    continue;
+                }
+                kin(k, in, K);
+                const int ax = t->axis[k];
+                if (k == i) { // the motion subspace of joint i (ignoring its flip, as rne does)
+                    sl[k] = ax < 3 ? v.zero() : unit(ax, Gen::cst(1.0));
+                    sa[k] = ax < 3 ? unit(ax, Gen::cst(1.0)) : v.zero();
+                } else {
+                    const int pa = t->parent[k];
+                    const double *C = t->C[k];
+                    auto RT = [&](const V3 &u) { return T.jointR(ax, st[k], ct[k], T.constR(C, u, true), true); };
+                    sl[k] = v.fix(RT(v.cross_acc(sa[pa], K.p[k], &sl[pa])));
+                    sa[k] = v.fix(RT(sa[pa]));
+                }
+                const V3 &w = K.w[k], &aw = K.aw[k], &s_l = sl[k], &s_a = sa[k];
+                const V3 A = v.fix(v.cross_acc(w, K.vl[k], &K.av[k]));
+                const Sym slw = g.fix(dot(s_l, w)), ww = g.fix(dot(w, w));
+                const V3 hw = v.scale(slw, w), hs = v.scale(g.neg(ww), s_l);
+                const V3 t1 = v.cross_acc(A, s_a, &hw, &hs);
+                const V3 hcoef = v.cross_acc(s_l, aw, &t1);
+                const V3 u = v.fix(v.cross_acc(s_a, w));
+                const V3 sa_ = v.fix(s_a), aw_ = v.fix(aw), w_ = v.fix(w);
+                auto sum2 = [&](const Sym &a1, const Sym &b1, const Sym &a2, const Sym &b2) { return g.sum({g.mul(a1, b1), g.mul(a2, b2)}); };
+                const Sym coef[10] = {dot(s_l, A), hcoef.x, hcoef.y, hcoef.z,
+                                      sum2(sa_.x, aw_.x, u.x, w_.x), sum2(sa_.y, aw_.y, u.y, w_.y), sum2(sa_.z, aw_.z, u.z, w_.z),
+                                      g.sum({g.mul(sa_.x, aw_.y), g.mul(sa_.y, aw_.x), g.mul(u.x, w_.y), g.mul(u.y, w_.x)}),
+                                      g.sum({g.mul(sa_.y, aw_.z), g.mul(sa_.z, aw_.y), g.mul(u.y, w_.z), g.mul(u.z, w_.y)}),
+                                      g.sum({g.mul(sa_.x, aw_.z), g.mul(sa_.z, aw_.x), g.mul(u.x, w_.z), g.mul(u.z, w_.x)})};
+                for (int c = 0; c < 10; c++) g.code.push_back("    " + assign(g, "y[" + std::to_string(10 * k + c) + "]", coef[c]));
+            }
+            g.code.push_back("    } break;");
+        }
+        g.code.push_back("    }");
+        src = "__device__ __forceinline__ void rne_regressor_row(const real *C, const real *grav, const real *fext, const real *st, "
+              "const real *ct, const real *qq, const real *qd, const real *qdd, int i, real *y)\n{\n";
+        for (const std::string &s : g.code) src += s + "\n";
+        src += "}\n";
+        out.source = src;
+        out.consts = g.consts;
+        if (out.consts.empty()) out.consts.push_back(0.0);
+        out.n_mul = g.n_mul; out.n_fma = g.n_fma; out.n_add = g.n_add;
+        out.error.clear();
+        return 0;
+    }
     std::vector<std::string> tail;
     const char *sig = nullptr;
     b2k_gen_opts oo = o;
     oo.has_fext = 0; // Robot.rne has no tip wrench
-    std::string src;
     if (o.mode == B2K_GEN_ACCEL_DERIV) {
         // two functions over one constant bank: rne_row, the ACCEL row (M and torque - rne(q, qd, 0)), and rne_deriv_row,
         // the RNE_DERIV row that the kernel evaluates at the solved qdd* with the same gravity

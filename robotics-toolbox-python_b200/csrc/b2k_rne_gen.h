@@ -38,5 +38,7 @@ int b2k_tree_generate(const b2k_tree_s *t, const b2k_gen_opts &o, b2k_gen_out &o
 // [f; m] the base exerts on link 1, in frame 0, moment about its origin).  Trees (b2k_tree_generate) reject RNE_WRENCH.
 // Trees only: RNE_DERIV generates `rne_deriv_row(C, grav, fext, st, ct, qq, qd, qdd, dq, dqd)`, dq / dqd the n x n blocks
 // d tau_i / d q_k and d tau_i / d qd_k (i group order, k q order); ACCEL_DERIV generates the ACCEL `rne_row` followed by
-// that `rne_deriv_row` over one constant bank.
+// that `rne_deriv_row` over one constant bank.  TREE_REGRESSOR (trees only) generates
+// `rne_regressor_row(C, grav, fext, st, ct, qq, qd, qdd, i, y)`: joint row i of the regressor, y[10k + c] = d tau_i / d pi_c
+// of group k (10 n reals, group order, exact 0 unless group k is i or hangs below it).
 int b2k_rne_generate(const b2k_rne_s *r, const b2k_gen_opts &o, b2k_gen_out &out);

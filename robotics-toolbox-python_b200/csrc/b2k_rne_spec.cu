@@ -392,6 +392,63 @@ k_rne_deriv_spec(const __grid_constant__ SpecP P, const real *__restrict__ in0, 
 }
 )B2KSRC";
 
+// ------------------------------------------------------------------ the dynamics regressor of a tree (MODE 10)
+// A row of Y is NJ joint rows of 10 NJ reals (20 KB at n = 16 in fp64), too large to stage 32 whole rows per warp.  The
+// generated rne_regressor_row(..., i, y) writes joint row i of one row; the warp stages joint row i of its 32 rows in a
+// slab (odd row stride: the one-row-per-lane writes are free of bank conflicts) and drains it before the next joint row,
+// consecutive lanes on consecutive reals of Y.  WPB warps per block as fit the shared memory, up to 4.
+const char *kReg = R"B2KSRC(
+#define ROWY (10 * NJ)                                  /* reals of one joint row of Y */
+#define LDY (ROWY | 1)                                  /* slab row stride, in reals */
+#define SLAB_BYTES ((32 * LDY * (int)sizeof(real) + 15) & ~15)
+#define WARP_BYTES (NIN * IN_BYTES + SLAB_BYTES)
+
+extern "C" __global__ void __launch_bounds__(32 * WPB, MINB)
+k_rne_regressor_spec(const __grid_constant__ SpecP P, const real *__restrict__ in0, const real *__restrict__ in1,
+                     const real *__restrict__ in2, real *__restrict__ out, long long ntiles)
+{
+    extern __shared__ __align__(16) unsigned char smem[];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const long long tile = (long long)blockIdx.x * WPB + warp;
+    if (tile >= ntiles) return;
+    unsigned char *wb = smem + (size_t)warp * WARP_BYTES;
+    real *slab = reinterpret_cast<real *>(wb + NIN * IN_BYTES);
+    const size_t row0 = (size_t)tile * 32;
+    load_tile(reinterpret_cast<real *>(wb), in0 + row0 * NJ, lane);
+    load_tile(reinterpret_cast<real *>(wb + IN_BYTES), in1 + row0 * NJ, lane);
+    load_tile(reinterpret_cast<real *>(wb + 2 * IN_BYTES), in2 + row0 * NJ, lane);
+#if !PADIN
+    asm volatile("cp.async.commit_group;\n" ::: "memory");
+    asm volatile("cp.async.wait_group 0;\n" ::: "memory");
+#endif
+    __syncwarp();
+    const real *s0 = reinterpret_cast<const real *>(wb);
+    const real *s1 = reinterpret_cast<const real *>(wb + IN_BYTES);
+    const real *s2 = reinterpret_cast<const real *>(wb + 2 * IN_BYTES);
+    real th[NJ], st[NJ], ct[NJ], a1[NJ], a2[NJ];
+#pragma unroll
+    for (int j = 0; j < NJ; j++) {
+        th[j] = s0[lane * LDI + j] + P.offset[j];
+        a1[j] = s1[lane * LDI + j];
+        a2[j] = s2[lane * LDI + j];
+    }
+    sincos_batch(th, P.trig, st, ct);
+    real *gt = out + row0 * (size_t)(NJ * ROWY);
+#pragma unroll 1
+    for (int i = 0; i < NJ; i++) {
+        rne_regressor_row(P.C, P.grav, P.fext, st, ct, th, a1, a2, i, slab + lane * LDY);
+        __syncwarp();
+        real *g = gt + i * ROWY; // joint row i of the tile's first row; the tile's rows are NJ * ROWY apart
+#pragma unroll 4
+        for (int e = lane; e < 32 * ROWY; e += 32) {
+            const int r = e / ROWY, c = e - r * ROWY;
+            g[(size_t)r * (NJ * ROWY) + c] = slab[r * LDY + c];
+        }
+        __syncwarp();
+    }
+}
+)B2KSRC";
+
 // ------------------------------------------------------------------ forward-dynamics integrator (DynamicsMixin.fdyn)
 // The reference integrates ONE state with scipy's RK45, calling accel() -- n + 1 Python rne loops and a numpy solve --
 // for every stage (Dynamics.py:185-422).  Here one lane integrates one trajectory of an ensemble entirely on the device:
@@ -686,7 +743,7 @@ std::string build_source(const GenFn &gen, int n, int mode, int dtype, Program &
     p.n_mul = g.n_mul; p.n_fma = g.n_fma; p.n_add = g.n_add;
     const b2k_rne_op_s &op = B2K_RNE_OPS[mode];
     p.nin = op.nin;
-    const bool deriv = mode == B2K_GEN_RNE_DERIV || mode == B2K_GEN_ACCEL_DERIV;
+    const bool deriv = mode == B2K_GEN_RNE_DERIV || mode == B2K_GEN_ACCEL_DERIV, reg = mode == B2K_GEN_TREE_REGRESSOR;
     p.nout = op.out_row(0, n);
     p.nout2 = op.nout > 1 ? op.out_row(1, n) : 0; // tau (N, n) and the base wrench (N, 6)
     p.nres = mode == B2K_GEN_ACCEL ? n * n + n : p.nout + p.nout2;
@@ -715,10 +772,15 @@ std::string build_source(const GenFn &gen, int n, int mode, int dtype, Program &
         p.wpb = (int)std::min<size_t>(4, (220 * 1024) / warp_bytes);
         p.smem = (size_t)std::max(p.wpb, 1) * warp_bytes;
     }
+    if (reg) { // per warp the input tiles and the slab of one joint row (32 x 10 n reals, odd stride); up to 4 warps
+        const size_t warp_bytes = p.nin * in_bytes + (((size_t)32 * ((10 * n) | 1) * es + 15) & ~(size_t)15);
+        p.wpb = (int)std::min<size_t>(4, (220 * 1024) / warp_bytes);
+        p.smem = (size_t)std::max(p.wpb, 1) * warp_bytes;
+    }
     if (p.smem > 220 * 1024) { p.why = "a tile of this operation does not fit the shared memory of an SM (" + std::to_string(p.smem) + " B)"; return std::string(); }
     int minb = (int)((200 * 1024) / (p.smem + 1024));
     // resident blocks to aim for (swept: fp64 96 registers / 5 blocks, fp32 64 registers / 8 blocks)
-    const int want = deriv ? 1 : light ? (es == 8 ? 5 : 8) : (es == 8 ? 2 : 3);
+    const int want = deriv || reg ? 1 : light ? (es == 8 ? 5 : 8) : (es == 8 ? 2 : 3);
     if (minb > want) minb = want;
     if (minb < 1) minb = 1;
     auto D = [&](const char *k, long long v) { defs.push_back(std::string("-D") + k + "=" + std::to_string(v)); };
@@ -726,9 +788,9 @@ std::string build_source(const GenFn &gen, int n, int mode, int dtype, Program &
     D("REAL_IS_F64", es == 8);
     D("NJ", n); D("NC", p.nc); D("MODE", mode); D("NIN", p.nin); D("NOUT", p.nout); D("NRES", p.nres); D("PADIN", padin); D("MINB", minb); D("TPW", tpw);
     if (p.nout2) D("NOUT2", p.nout2);
-    if (deriv) D("WPB", p.wpb);
+    if (deriv || reg) D("WPB", p.wpb);
     // in1 / in2 of the generated function are the second / third input rows; the RNE proper names them qd / qdd
-    return std::string(kPrologue) + g.source + (kernel_text ? kernel_text : std::string(kTileIn) + (deriv ? kDeriv : kKernel));
+    return std::string(kPrologue) + g.source + (kernel_text ? kernel_text : std::string(kTileIn) + (deriv ? kDeriv : reg ? kReg : kKernel));
 }
 
 void compile(const GenFn &gen, int n, const Key &key, Program &p)
@@ -740,6 +802,7 @@ void compile(const GenFn &gen, int n, const Key &key, Program &p)
     const bool fdyn = std::get<0>(key) / 100 == 2;
     if (fdyn) p.entry = "k_fdyn";
     else if (mode == B2K_GEN_RNE_DERIV || mode == B2K_GEN_ACCEL_DERIV) p.entry = "k_rne_deriv_spec";
+    else if (mode == B2K_GEN_TREE_REGRESSOR) p.entry = "k_rne_regressor_spec";
     const std::string src = build_source(gen, n, mode, dtype, p, defs, fdyn ? kFdyn : nullptr);
     if (src.empty()) return;
     std::vector<std::string> opts = {"--gpu-architecture=sm_90a", "--std=c++17"};
@@ -1040,14 +1103,19 @@ static Program *tree_program(b2k_tree_t t, int mode, int dtype, int gmask)
     }, t->n, key);
 }
 
-// Robot.rne (mode 0), the operations DynamicsMixin builds on it (modes 1-5: inertia, gravload, itorque, coriolis, accel) and
-// their derivatives (modes 7, 8; `derivs`: the b2k_tree_derivatives entry point) for a rigid-body tree: the generated kernel
-// on the full tiles, one padded tile for the ragged tail.  out[0..nout) are the operation's output arrays.
-static int tree_run(const char *fn, b2k_tree_t t, int mode, bool derivs, int dtype, const void *in0, const void *in1, const void *in2,
-                    int64_t N, const double *grav, void *const out[3], void *stream)
+// Robot.rne (mode 0), the operations DynamicsMixin builds on it (modes 1-5: inertia, gravload, itorque, coriolis, accel),
+// their derivatives (modes 7, 8; TREE_DERIVS: the b2k_tree_derivatives entry point) and the regressor (mode 10,
+// TREE_REGRESSOR) for a rigid-body tree: the generated kernel on the full tiles, one padded tile for the ragged tail.
+// out[0..nout) are the operation's output arrays.
+enum TreeEntry { TREE_DYN, TREE_DERIVS, TREE_REGRESSOR };
+static int tree_run(const char *fn, b2k_tree_t t, int mode, TreeEntry entry, int dtype, const void *in0, const void *in1,
+                    const void *in2, int64_t N, const double *grav, void *const out[3], void *stream)
 {
     if (!t) { b2k_set_error("%s: tree handle is NULL", fn); return B2K_ERR_INVALID; }
-    if (derivs ? (mode != B2K_GEN_RNE_DERIV && mode != B2K_GEN_ACCEL_DERIV) : (mode < B2K_GEN_RNE || mode > B2K_GEN_ACCEL)) {
+    const bool derivs = entry == TREE_DERIVS;
+    if (entry == TREE_REGRESSOR ? mode != B2K_GEN_TREE_REGRESSOR
+        : derivs                ? (mode != B2K_GEN_RNE_DERIV && mode != B2K_GEN_ACCEL_DERIV)
+                                : (mode < B2K_GEN_RNE || mode > B2K_GEN_ACCEL)) {
         if (derivs) b2k_set_error("%s: operation %d is not B2K_DYN_RNE_DERIV or B2K_DYN_ACCEL_DERIV", fn, mode);
         else b2k_set_error("%s: operation %d is not one of B2K_DYN_*", fn, mode);
         return B2K_ERR_INVALID;
@@ -1109,21 +1177,88 @@ extern "C" int b2k_tree_rne(b2k_tree_t t, int dtype, const void *q, const void *
                             void *tau, void *stream)
 {
     void *const out[3] = {tau, nullptr, nullptr};
-    return tree_run("b2k_tree_rne", t, B2K_GEN_RNE, false, dtype, q, qd, qdd, N, grav, out, stream);
+    return tree_run("b2k_tree_rne", t, B2K_GEN_RNE, TREE_DYN, dtype, q, qd, qdd, N, grav, out, stream);
 }
 
 extern "C" int b2k_tree_dyn(b2k_tree_t t, int op, int dtype, const void *in0, const void *in1, const void *in2, int64_t N,
                             const double *grav, void *out, void *stream)
 {
     void *const outs[3] = {out, nullptr, nullptr};
-    return tree_run("b2k_tree_dyn", t, op, false, dtype, in0, in1, in2, N, grav, outs, stream);
+    return tree_run("b2k_tree_dyn", t, op, TREE_DYN, dtype, in0, in1, in2, N, grav, outs, stream);
 }
 
 extern "C" int b2k_tree_derivatives(b2k_tree_t t, int op, int dtype, const void *q, const void *qd, const void *x, int64_t N,
                                     const double *grav, void *out0, void *out1, void *out2, void *stream)
 {
     void *const outs[3] = {out0, out1, out2};
-    return tree_run("b2k_tree_derivatives", t, op, true, dtype, q, qd, x, N, grav, outs, stream);
+    return tree_run("b2k_tree_derivatives", t, op, TREE_DERIVS, dtype, q, qd, x, N, grav, outs, stream);
+}
+
+extern "C" int b2k_tree_regressor(b2k_tree_t t, int dtype, const void *q, const void *qd, const void *qdd, int64_t N,
+                                  const double *grav, void *Y, void *stream)
+{
+    void *const outs[3] = {Y, nullptr, nullptr};
+    return tree_run("b2k_tree_regressor", t, B2K_GEN_TREE_REGRESSOR, TREE_REGRESSOR, dtype, q, qd, qdd, N, grav, outs, stream);
+}
+
+int b2k_tree_regressor_rows(b2k_tree_t t, int dtype, const b2k_rne_args &a, cudaStream_t st)
+{
+    void *const outs[3] = {a.out[0], nullptr, nullptr};
+    return tree_run("b2k_tree_regressor_gram", t, B2K_GEN_TREE_REGRESSOR, TREE_REGRESSOR, dtype, a.in[0], a.in[1], a.in[2],
+                    a.nrows, a.grav, outs, st);
+}
+
+int b2k_tree_regressor_gram_f32(b2k_tree_t, int, const b2k_rne_args &, const void *, const double *, double *, double *, double *,
+                                cudaStream_t);
+int b2k_tree_regressor_gram_f64(b2k_tree_t, int, const b2k_rne_args &, const void *, const double *, double *, double *, double *,
+                                cudaStream_t);
+
+// The normal equations of the tree regressor (b2k_rne.cuh: regressor_gram, shared with the DH arms).  Every argument is
+// checked, and the kernel built, before any CUDA call.
+extern "C" int b2k_tree_regressor_gram(b2k_tree_t t, int dtype, const void *q, const void *qd, const void *qdd, const void *tau,
+                                       int64_t N, const double *grav, const double *weights, double *G, double *b, double *s,
+                                       void *stream)
+{
+    const char *fn = "b2k_tree_regressor_gram";
+    if (!t) { b2k_set_error("%s: tree handle is NULL", fn); return B2K_ERR_INVALID; }
+    if (dtype != B2K_F32 && dtype != B2K_F64) { b2k_set_error("%s: dtype must be B2K_F32 or B2K_F64", fn); return B2K_ERR_INVALID; }
+    if (N < 0) { b2k_set_error("%s: N is negative", fn); return B2K_ERR_INVALID; }
+    if (!grav) { b2k_set_error("%s: grav is NULL (pass MINUS the robot's gravity: a_grav of Robot.rne)", fn); return B2K_ERR_INVALID; }
+    const int es = dtype == B2K_F64 ? 8 : 4, n = t->n;
+    int rc;
+    const char *names[3] = {"q", "qd", "qdd"};
+    const void *ins[3] = {q, qd, qdd};
+    for (int i = 0; i < 3; i++)
+        if ((rc = b2k_check_array(fn, names[i], ins[i], N, 16))) return rc;
+    if ((rc = b2k_check_array(fn, "tau", tau, N, es))) return rc;
+    if (weights)
+        for (int j = 0; j < n; j++)
+            if (!isfinite(weights[j]) || weights[j] < 0) {
+                b2k_set_error("%s: weights[%d] = %g is not a finite value >= 0", fn, j, weights[j]);
+                return B2K_ERR_INVALID;
+            }
+    // the sums are written whatever N is (zeros for N = 0)
+    if ((rc = b2k_check_array(fn, "G", G, 1, 8)) || (rc = b2k_check_array(fn, "b", b, 1, 8)) || (rc = b2k_check_array(fn, "s", s, 1, 8)))
+        return rc;
+    const b2k_rne_args a = {{q, qd, qdd}, {nullptr}, N, grav, nullptr};
+    if (N > 0) { // the generated kernel is built before any CUDA call, so that a tree it cannot serve leaves no work queued
+        Program *p = tree_program(t, B2K_GEN_TREE_REGRESSOR, dtype, grav_mask_of(grav));
+        if (!p || !p->ok) {
+            b2k_set_error("%s: the kernel for this robot could not be built (%s)", fn, p ? p->why.c_str() : "no cache");
+            return B2K_ERR_INVALID;
+        }
+    }
+    B2K_ON_DEVICE_OF(G);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (N == 0) {
+        const size_t p = 10 * (size_t)n;
+        B2K_CUDA(cudaMemsetAsync(G, 0, p * p * sizeof(double), st));
+        B2K_CUDA(cudaMemsetAsync(b, 0, p * sizeof(double), st));
+        B2K_CUDA(cudaMemsetAsync(s, 0, sizeof(double), st));
+        return B2K_OK;
+    }
+    return dtype == B2K_F64 ? b2k_tree_regressor_gram_f64(t, n, a, tau, weights, G, b, s, st)
+                            : b2k_tree_regressor_gram_f32(t, n, a, tau, weights, G, b, s, st);
 }
 
 extern "C" int b2k_tree_codegen(b2k_tree_t t, int op, int grav_mask, char *src, int64_t src_cap, double *consts, int32_t consts_cap,
@@ -1150,7 +1285,7 @@ extern "C" int b2k_tree_codegen(b2k_tree_t t, int op, int grav_mask, char *src, 
 extern "C" int b2k_tree_info(b2k_tree_t t, int op, int dtype, const double *grav, char *buf, int64_t cap)
 {
     if (!t || !buf || cap < 1) { b2k_set_error("b2k_tree_info: bad arguments"); return B2K_ERR_INVALID; }
-    if (op < B2K_GEN_RNE || op > B2K_GEN_ACCEL_DERIV || op == B2K_GEN_RNE_WRENCH) {
+    if (op < B2K_GEN_RNE || (op > B2K_GEN_ACCEL_DERIV && op != B2K_GEN_TREE_REGRESSOR) || op == B2K_GEN_RNE_WRENCH) {
         b2k_set_error("b2k_tree_info: operation %d is not one of B2K_DYN_*", op);
         return B2K_ERR_INVALID;
     }
@@ -1159,7 +1294,7 @@ extern "C" int b2k_tree_info(b2k_tree_t t, int op, int dtype, const double *grav
     else if (op == B2K_GEN_RNE)
         snprintf(buf, (size_t)cap, "k_rne_spec<%s,tree n=%d>: %d mul + %d fma + %d add per row, %d constants, %d regs, %zu B smem/block",
                  dtype == B2K_F64 ? "double" : "float", t->n, p->n_mul, p->n_fma, p->n_add, p->nc, p->regs, p->smem);
-    else if (p->nblk)
+    else if (p->nblk || op == B2K_GEN_TREE_REGRESSOR)
         snprintf(buf, (size_t)cap, "%s<%s,tree n=%d,mode=%d>: %d mul + %d fma + %d add per row, %d constants, %d regs, %zu B smem/block, "
                  "%d warps/block",
                  p->entry, dtype == B2K_F64 ? "double" : "float", t->n, op, p->n_mul, p->n_fma, p->n_add, p->nc, p->regs, p->smem, p->wpb);

@@ -927,3 +927,87 @@ if any(want(c) for c in REG_CASES):
                 report(c_gram, ms, N, 4 * n * es, dict(card, fp64_tflops=round(flops / (ms * 1e-3) / 1e12, 2),
                                                       frac_of_34TFLOPs=round(flops / (ms * 1e-3) / 34e12, 4)))
             del q0, qd0, qdd0, tau0
+
+# The dynamics regressor of a rigid-body tree (Robot.rne_regressor, b2k_tree_regressor) and its normal equations
+# (b2k_tree_regressor_gram): the Puma560 assembled as an ETS robot and a branched 16-joint tree, N device rows.
+# Algorithmic bytes per row of the regressor: (3n + 10n^2) es, against 3.35 TB/s.  The gram is reported in FP64 FLOP/s
+# (n p^2 / 2 FMAs per row, p = 10n).  unit_route is what a user has without the regressor, timed in the same call on the
+# same rows with both routes alternated: 10n b2k_tree_rne launches, one per handle whose only nonzero inertia is one unit
+# parameter of one group (tests/tree_regressor_ref.py).  The card's name and power limit are read in the same run.
+TREG_CASES = [f"tree_regressor_{r}_{t}" for r in ("puma", "tree16") for t in ("f64", "f32")] + \
+             [f"tree_regressor_gram_{r}_{t}" for r in ("puma", "tree16") for t in ("f64", "f32")]
+if any(want(c) for c in TREG_CASES):
+    import ctypes
+    import subprocess
+
+    try:
+        plim = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True,
+                              text=True, timeout=30).stdout.strip()
+    except Exception as e:  # the figure is context, the timing does not depend on it
+        plim = f"unavailable ({type(e).__name__})"
+    card = {"gpu": torch.cuda.get_device_name(0), "power_limit": plim}
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import tree_regressor_ref as TRR  # noqa: E402
+    from test_gpu_tree import random_robot  # noqa: E402
+    from test_gpu_tree_derivs import puma_ets  # noqa: E402
+
+    Lt = rtb._lib.lib()
+    stt = torch.cuda.current_stream().cuda_stream
+    rngq = np.random.default_rng(18)
+    for rname, rob in (("puma", puma_ets(0.0)[0]), ("tree16", random_robot(np.random.default_rng(61), 16, True))):
+        n, p = rob.n, 10 * rob.n
+        ht = rob._tree_handle()
+        ag = rob._kernel_gravity(None)
+        desc = rob.tree_description()
+        for dt in (np.float64, np.float32):
+            tag = "f64" if dt == np.float64 else "f32"
+            c_reg, c_gram = f"tree_regressor_{rname}_{tag}", f"tree_regressor_gram_{rname}_{tag}"
+            if not (want(c_reg) or want(c_gram)):
+                continue
+            es = np.dtype(dt).itemsize
+            code = rtb._lib.F64 if dt == np.float64 else rtb._lib.F32
+            tt = torch.float64 if dt == np.float64 else torch.float32
+            q0, qd0, qdd0, tau0 = (torch.from_numpy(rngq.uniform(-2, 2, (N, n)).astype(dt)).to(dev) for _ in range(4))
+            if want(c_reg):
+                Y = torch.empty((N, n, p), dtype=tt, device=dev)
+                units = []
+                for k in range(p):
+                    I6 = np.zeros((n, 6, 6))
+                    I6[k // 10] = TRR.basis(k % 10)
+                    i32 = [np.ascontiguousarray(desc[key], dtype=np.int32) for key in ("parent", "axis", "flip", "jindex")]
+                    Cm = np.ascontiguousarray(np.asarray(desc["C"], dtype=np.float64)[:, :3, :].reshape(n, 12))
+                    hu = rtb._lib.vp()
+                    rtb._lib.check(Lt.b2k_tree_create(n, *(a.ctypes.data_as(rtb._lib.ip) for a in i32), rtb._lib.dptr(Cm),
+                                                      rtb._lib.dptr(np.ascontiguousarray(I6.reshape(n, 36))), ctypes.byref(hu)))
+                    units.append(hu)
+                outs = [torch.empty((N, n), dtype=tt, device=dev) for _ in range(p)]
+
+                def unit_route(i):
+                    for hu, t in zip(units, outs):
+                        rtb._lib.check(Lt.b2k_tree_rne(hu, code, q0.data_ptr(), qd0.data_ptr(), qdd0.data_ptr(), N, rtb._lib.dptr(ag),
+                                                       t.data_ptr(), stt))
+
+                ms_u, ms = [], []
+                for _ in range(2):  # alternate the two routes, so that both see the same clocks
+                    ms_u.append(timeit(unit_route, 1))
+                    ms.append(timeit(lambda i: rtb._lib.check(Lt.b2k_tree_regressor(ht, code, q0.data_ptr(), qd0.data_ptr(), qdd0.data_ptr(),
+                                                                                    N, rtb._lib.dptr(ag), Y.data_ptr(), stt)), 1))
+                ms_u, ms = min(ms_u), min(ms)
+                bpr = (3 * n + 10 * n * n) * es
+                report(c_reg, ms, N, bpr, dict(card, frac_of_3p35TBps=round(bpr * N / (ms * 1e-3) / 3.35e12, 4), unit_route_ms=round(ms_u, 4),
+                                               unit_route_launches=p, speedup_vs_unit_route=round(ms_u / ms, 2),
+                                               kernel=rob.rne_kernel_info(dt, op="rne_regressor")))
+                for hu in units:
+                    Lt.b2k_tree_destroy(hu)
+                del Y, outs
+            if want(c_gram):
+                G = torch.empty((p, p), dtype=torch.float64, device=dev)
+                b = torch.empty(p, dtype=torch.float64, device=dev)
+                s = torch.empty(1, dtype=torch.float64, device=dev)
+                ms = timeit(lambda i: rtb._lib.check(Lt.b2k_tree_regressor_gram(ht, code, q0.data_ptr(), qd0.data_ptr(), qdd0.data_ptr(),
+                                                                                tau0.data_ptr(), N, rtb._lib.dptr(ag), None, G.data_ptr(),
+                                                                                b.data_ptr(), s.data_ptr(), stt)), 1)
+                flops = 2 * (n * p * p / 2) * N
+                report(c_gram, ms, N, 4 * n * es, dict(card, fp64_tflops=round(flops / (ms * 1e-3) / 1e12, 2),
+                                                      frac_of_34TFLOPs=round(flops / (ms * 1e-3) / 34e12, 4)))
+            del q0, qd0, qdd0, tau0
