@@ -455,6 +455,26 @@ int b2k_tree_fdyn(b2k_tree_t tree, int dtype, const void *q0, const void *qd0, i
                  double rtol, double atol, double max_step, double first_step, double dt, int grid, int M, void *out_t,
                  void *out_q, void *out_qd, int32_t *out_count, int32_t *out_status, void *stream);
 
+/* Fixed-step rollouts with discrete-time sensitivities, for sampling MPC and shooting methods (iLQR / DDP): one lane per
+ * trajectory, K classical RK4 steps of x = [q; qd] under a torque held over each step,
+ *   f(x, tau) = [qd; accel(q, qd, tau)]     k1 = f(x_k), k2 = f(x_k + dt/2 k1), k3 = f(x_k + dt/2 k2), k4 = f(x_k + dt k3)
+ *   x_{k+1} = x_k + dt/6 (k1 + 2 k2 + 2 k3 + k4)
+ * with accel exactly that of the robot (b2k_rne_accel: friction and armature kept; b2k_tree_dyn B2K_DYN_ACCEL).  A (N,K,2n,2n)
+ * and B (N,K,2n,n) are the exact derivatives of that map, A_k = d x_{k+1} / d x_k and B_k = d x_{k+1} / d tau_k, [i, j] =
+ * d out_i / d in_j, chained through the four stages from the derivatives of accel at each stage state (Coulomb friction
+ * contributes 0).  A singular M gives non-finite values from that step on; no error is raised.
+ *   q0, qd0 (N,n) device (qd0 may be NULL = at rest); tau (K,n) device with tau_stride 0 (one sequence for every trajectory)
+ *   or (N,K,n) with tau_stride K n; q, qd (N,K+1,n) device, index 0 the initial state.  A and B both NULL: states only;
+ *   both non-NULL: with sensitivities (the states are bit-identical either way); one NULL is rejected.  Every array needs
+ *   the alignment of its element type.  dt finite and > 0, K >= 1, grav as the family's accel takes it (MINUS the robot's
+ *   gravity).  DH arms must be all-revolute.  Every argument is checked, and the kernel built (NVRTC), before any CUDA
+ *   call; N = 0 launches nothing.  b2k_rne_spec_info / b2k_tree_info describe the kernels with mode / op 305 (states only)
+ *   and 308 (with sensitivities). */
+int b2k_rne_rollout(b2k_rne_t rne, int dtype, const void *q0, const void *qd0, int64_t N, int32_t K, double dt,
+                    const double *grav, const void *tau, int64_t tau_stride, void *q, void *qd, void *A, void *B, void *stream);
+int b2k_tree_rollout(b2k_tree_t tree, int dtype, const void *q0, const void *qd0, int64_t N, int32_t K, double dt,
+                     const double *grav, const void *tau, int64_t tau_stride, void *q, void *qd, void *A, void *B, void *stream);
+
 /* ---------------------------------------------------------------- operational-space dynamics
  * The arithmetic of DynamicsMixin.inertia_x, coriolis_x, gravload_x and accel_x (robot/Dynamics.py, between gravload and
  * itorque: per row np.linalg.inv / pinv of the analytical Jacobian and numpy triple products, in a Python loop), as an

@@ -500,11 +500,15 @@ class Robot:
                 "accel_derivatives": 8, "rne_regressor": 10}
 
     def rne_kernel_info(self, dtype=np.float64, gravity=None, op="rne") -> str:
+        """The generated kernel that serves `op`; ``op="rollout"`` gives two lines, states only and with sensitivities."""
         g = self._gravity if gravity is None else np.asarray(gravity, dtype=np.float64).reshape(3)
         ag = np.ascontiguousarray(-g)
         buf = C.create_string_buffer(2048)
-        _lib.check(_lib.lib().b2k_tree_info(self._tree_handle(), self._DYN_OPS[op], B.code(np.dtype(dtype)), _lib.dptr(ag), buf, 2048))
-        return buf.value.decode()
+        lines = []
+        for code in ((305, 308) if op == "rollout" else (self._DYN_OPS[op],)):
+            _lib.check(_lib.lib().b2k_tree_info(self._tree_handle(), code, B.code(np.dtype(dtype)), _lib.dptr(ag), buf, 2048))
+            lines.append(buf.value.decode())
+        return "\n".join(lines)
 
     # ---- dynamics built on the recursion (reference DynamicsMixin, Dynamics.py, which BaseRobot inherits: each method
     #      there is a Python loop of self.rne calls; here one generated kernel per operation, b2k_tree_dyn)
@@ -699,6 +703,20 @@ class Robot:
         return _fdyn(self, None if callable_q else _lib.lib().b2k_tree_fdyn, None if callable_q else self._tree_handle(), kernel_gravity,
                      T, q0, Q=Q, Q_args=Q_args, qd0=qd0, solver=solver, solver_args=solver_args, dt=dt, gravity=gravity,
                      max_steps=max_steps, dtype=dtype)
+
+    def rollout(self, q0, tau, dt, qd0=None, sensitivities=False, gravity=None, dtype=None):
+        """Fixed-step RK4 rollouts under a torque sequence with their exact linearisation A_k = d x_{k+1} / d x_k,
+        B_k = d x_{k+1} / d tau_k: the named tuple ``(t, q, qd, A, B)``.  Arguments, semantics and return values as
+        ``DHRobot.rollout``, with this robot's ``accel`` (tau and its columns in the order ``accel`` takes them) and
+        ``accel_derivatives``; one launch of a kernel generated for this robot (n <= 16).  The first call compiles the
+        kernel (NVRTC; the sensitivities program of a 16-joint tree takes about 30-40 s on a CPU core), and the
+        sensitivities kernel's per-thread working set of 15 n^2 reals (30 KB at n = 16 in fp64) lives in local memory,
+        which the driver reserves for every thread the device can hold (about 1 GB per 5 KB of stack on an H100) and keeps
+        for the life of the process."""
+        from ._rollout import rollout as _rollout
+
+        return _rollout(self, _lib.lib().b2k_tree_rollout, self._tree_handle(), self._kernel_gravity, q0, tau, dt, qd0=qd0,
+                        sensitivities=sensitivities, gravity=gravity, dtype=dtype)
 
     # ---- model ingestion
     @classmethod

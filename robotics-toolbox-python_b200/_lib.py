@@ -60,6 +60,8 @@ _PROTOS = {
                                C.c_double, C.c_double, C.c_double, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp]),
     "b2k_tree_fdyn": (C.c_int, [vp, C.c_int, vp, vp, i64, C.c_double, dp, C.c_int, dp, vp, dp, dp, dp, C.c_double, C.c_double,
                                C.c_double, C.c_double, C.c_double, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp]),
+    "b2k_rne_rollout": (C.c_int, [vp, C.c_int, vp, vp, i64, C.c_int32, C.c_double, dp, vp, i64, vp, vp, vp, vp, vp]),
+    "b2k_tree_rollout": (C.c_int, [vp, C.c_int, vp, vp, i64, C.c_int32, C.c_double, dp, vp, i64, vp, vp, vp, vp, vp]),
     "b2k_tree_create": (C.c_int, [C.c_int, ip, ip, ip, ip, dp, dp, C.POINTER(vp)]),
     "b2k_tree_destroy": (C.c_int, [vp]),
     "b2k_tree_rne": (C.c_int, [vp, C.c_int, vp, vp, vp, i64, dp, vp, vp]),

@@ -222,7 +222,7 @@ struct Gen {
             return o.neg ? neg(T[o.id]) : T[o.id];
         };
         for (int id = 0; id < upto; id++) {
-            const Def &d = defs[id];
+            const Def d = defs[id]; // a copy: the rules below emit, and emit() grows defs
             switch (d.op) {
             case Def::LEAF: break;
             case Def::MUL: T[id] = sum({mul(dtf(d.a), val(d.b)), mul(val(d.a), dtf(d.b))}); break;
@@ -439,10 +439,16 @@ std::vector<Sym> recursion(Gen &g, const std::vector<Link> &L, bool mdh, const I
                 tq = g.fix(g.add(tq, Gen::cst(c)));
             } else { // tq + Tc+ [qd > 0] + Tc- [qd < 0]: two FMAs against 0 / 1 masks, no branch
                 const std::string q = g.spell(qdo);
-                std::string e = g.spell(g.operand(tq));
+                // the Coulomb term is piecewise constant: tangent() reads the result as tq + 0 (tq itself may be a
+                // structural zero: a link with no mass, inertia or other actuator term on its axis)
+                Def d;
+                d.op = Def::ADD; d.b.isc = true;
+                if (tq.k == Sym::Z) d.a.isc = true;
+                else d.a = g.operand(tq);
+                std::string e = tq.k == Sym::Z ? "(real)0" : g.spell(d.a);
                 if (l.c_tcm != 0.0) { Opd m; m.isc = true; m.c = l.c_tcm; e = "fma(" + g.spell(m) + ", step_neg(" + q + "), " + e + ")"; g.n_fma++; }
                 if (l.c_tcp != 0.0) { Opd p; p.isc = true; p.c = l.c_tcp; e = "fma(" + g.spell(p) + ", step_pos(" + q + "), " + e + ")"; g.n_fma++; }
-                tq = g.emit(e);
+                tq = g.emit(e, d);
             }
         }
         tau[j] = tq;
@@ -614,48 +620,64 @@ int assemble(Gen &g, int N, const b2k_gen_opts &o, const RecFn &rec, std::vector
 
 int b2k_rne_generate(const b2k_rne_s *r, const b2k_gen_opts &o, b2k_gen_out &out)
 {
-    if (o.mode == B2K_GEN_RNE_DERIV || o.mode == B2K_GEN_ACCEL_DERIV) {
-        out.error = "the derivatives of DH arms are served by the generic kernel";
-        return -1;
-    }
     if (o.mode == B2K_GEN_TREE_REGRESSOR) { out.error = "the tree regressor is no operation of DH arms"; return -1; }
     const int N = r->n;
     Gen g;
     std::vector<Link> L(N);
-    for (int j = 0; j < N; j++) {
-        const double *l = r->L[j];
-        const double alpha = l[0], A = l[1], theta = l[2], D = l[3], G = l[20];
-        const double sa = snap(sin(alpha)), ca = snap(cos(alpha));
-        L[j].pris = ((int)l[4] != 0);
-        L[j].sa = Gen::cst(sa);
-        L[j].ca = Gen::cst(ca);
-        Sym d;
-        if (L[j].pris) { // the joint variable is the link offset d = q + offset (qq = q + offset in the kernel), theta is fixed
-            L[j].st = Gen::cst(snap(sin(theta)));
-            L[j].ct = Gen::cst(snap(cos(theta)));
-            d = g.var("qq[" + std::to_string(j) + "]");
-        } else {
-            L[j].st = g.var("st[" + std::to_string(j) + "]");
-            L[j].ct = g.var("ct[" + std::to_string(j) + "]");
-            d = Gen::cst(D);
+    auto links = [&]() { // the link table, with this function's joint inputs (st, ct, qq) as fresh leaves
+        for (int j = 0; j < N; j++) {
+            const double *l = r->L[j];
+            const double alpha = l[0], A = l[1], theta = l[2], D = l[3], G = l[20];
+            const double sa = snap(sin(alpha)), ca = snap(cos(alpha));
+            L[j].pris = ((int)l[4] != 0);
+            L[j].sa = Gen::cst(sa);
+            L[j].ca = Gen::cst(ca);
+            Sym d;
+            if (L[j].pris) { // the joint variable is the link offset d = q + offset (qq = q + offset in the kernel), theta is fixed
+                L[j].st = Gen::cst(snap(sin(theta)));
+                L[j].ct = Gen::cst(snap(cos(theta)));
+                d = g.var("qq[" + std::to_string(j) + "]");
+            } else {
+                L[j].st = g.var("st[" + std::to_string(j) + "]");
+                L[j].ct = g.var("ct[" + std::to_string(j) + "]");
+                d = Gen::cst(D);
+            }
+            L[j].ps = {Gen::cst(A), g.fix(g.mul(d, Gen::cst(r->mdh ? -sa : sa))), g.fix(g.mul(d, Gen::cst(ca)))};
+            L[j].m = l[6];
+            for (int k = 0; k < 3; k++) L[j].r[k] = l[7 + k];
+            for (int k = 0; k < 9; k++) L[j].I[k] = l[10 + k];
+            L[j].c_jm = G * G * l[19];
+            L[j].c_b = G * G * l[21];
+            L[j].c_tcp = fabs(G) * l[22];
+            L[j].c_tcm = fabs(G) * l[23];
         }
-        L[j].ps = {Gen::cst(A), g.fix(g.mul(d, Gen::cst(r->mdh ? -sa : sa))), g.fix(g.mul(d, Gen::cst(ca)))};
-        L[j].m = l[6];
-        for (int k = 0; k < 3; k++) L[j].r[k] = l[7 + k];
-        for (int k = 0; k < 9; k++) L[j].I[k] = l[10 + k];
-        L[j].c_jm = G * G * l[19];
-        L[j].c_b = G * G * l[21];
-        L[j].c_tcp = fabs(G) * l[22];
-        L[j].c_tcm = fabs(G) * l[23];
-    }
+    };
+    links();
+    const RecFn rec = [&](const Inputs &in) { return recursion(g, L, r->mdh != 0, in); };
+    auto function = [](const Gen &gg, const char *sig, const std::vector<std::string> &tail) {
+        std::string f = std::string("__device__ __forceinline__ void ") + sig + "\n{\n";
+        for (const std::string &s : gg.code) f += s + "\n";
+        for (const std::string &s : tail) f += s + "\n";
+        return f + "}\n";
+    };
     std::vector<std::string> tail;
     const char *sig = nullptr;
-    if (assemble(g, N, o, [&](const Inputs &in) { return recursion(g, L, r->mdh != 0, in); }, tail, sig, out.error)) return -1;
-    std::string src = std::string("__device__ __forceinline__ void ") + sig + "\n{\n";
-    for (const std::string &s : g.code) src += s + "\n";
-    for (const std::string &s : tail) src += s + "\n";
-    src += "}\n";
-    out.source = src;
+    std::string src;
+    b2k_gen_opts oo = o;
+    if (o.mode == B2K_GEN_RNE_DERIV || o.mode == B2K_GEN_ACCEL_DERIV) oo.has_fext = 0; // no tip wrench
+    if (o.mode == B2K_GEN_ACCEL_DERIV) {
+        // two functions over one constant bank, as for trees: rne_row, the ACCEL row, and rne_deriv_row, the RNE_DERIV row
+        // that the kernel evaluates at the solved qdd* with the same gravity
+        oo.mode = B2K_GEN_ACCEL;
+        if (assemble(g, N, oo, rec, tail, sig, out.error)) return -1;
+        src = function(g, sig, tail);
+        g.code.clear();
+        tail.clear();
+        links();
+        oo.mode = B2K_GEN_RNE_DERIV;
+    }
+    if (assemble(g, N, oo, rec, tail, sig, out.error)) return -1;
+    out.source = src + function(g, sig, tail);
     out.consts = g.consts;
     if (out.consts.empty()) out.consts.push_back(0.0);
     out.n_mul = g.n_mul; out.n_fma = g.n_fma; out.n_add = g.n_add;

@@ -17,6 +17,8 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <cmath>
+
 #include <algorithm>
 #include <functional>
 #include <map>
@@ -623,6 +625,167 @@ k_fdyn(const __grid_constant__ SpecP P, const __grid_constant__ FdynP F, const r
 }
 )B2KSRC";
 
+// ------------------------------------------------------------------ fixed-step RK4 rollouts (DHRobot.rollout, Robot.rollout)
+// One lane integrates one trajectory, as k_fdyn does.  Each stage is one ACCEL row (rne_row) and its LDL^T solve; with
+// SENS (the ACCEL_DERIV program) also M^-1 from the same factors, the derivative row at qdd* mapped by -M^-1, and the
+// stage's column of the chain rule dk_i = J_f (e + c dt dk_{i-1}) (+ [0; M^-1] for the torque columns), J_f = [[0, I],
+// [dqdd_dq, dqdd_dqd]], whose upper half is a copy.  The per-lane working set (dk_{i-1} and the sums of the stages, 6 n^2
+// reals each, and three n x n blocks) lives in local memory.  The 6 n^2 reals of A_k | B_k leave through a per-warp slab of
+// 32 lanes x CH reals: the warp writes one lane's CH consecutive reals per store instruction, so every store is coalesced
+// at every n, where a stage of whole blocks (32 x 6 n^2 reals) would not fit the shared memory from n = 13 (fp64) on.
+// Both programs run the same value path (compiled without FMA contraction), so their states are bit-identical.
+const char *kRollout = R"B2KSRC(
+#define NS (2 * NJ)
+#define NSQ (NJ * NJ)
+#define NSENS (6 * NSQ)  /* reals of A_k (2n x 2n) followed by B_k (2n x n) */
+#define CH 32            /* reals per lane of one drain of the slab */
+
+struct RollP { real h2, h, h6; int K; long long tau_stride; };
+
+extern "C" __global__ void __launch_bounds__(64)
+k_rollout(const __grid_constant__ SpecP P, const __grid_constant__ RollP R, const real *__restrict__ q0, const real *__restrict__ qd0,
+          const real *__restrict__ tau, real *__restrict__ oq, real *__restrict__ oqd, real *__restrict__ oA, real *__restrict__ oB,
+          long long ntraj)
+{
+    const long long tr = (long long)blockIdx.x * 64 + threadIdx.x;
+    if (tr - (threadIdx.x & 31) >= ntraj) return; // a warp with no trajectory (the drains synchronise within a warp only)
+    const bool live = tr < ntraj; // dead lanes integrate the zero state and store nothing: the drains need the whole warp
+    const long long trc = live ? tr : 0;
+    real x[NS];
+#pragma unroll
+    for (int j = 0; j < NJ; j++) {
+        x[j] = live ? q0[trc * NJ + j] : (real)0;
+        x[NJ + j] = live && qd0 ? qd0[trc * NJ + j] : (real)0;
+    }
+    auto store = [&](int k) {
+        if (!live) return;
+        const size_t o = ((size_t)tr * (R.K + 1) + k) * NJ;
+#pragma unroll
+        for (int j = 0; j < NJ; j++) { oq[o + j] = x[j]; oqd[o + j] = x[NJ + j]; }
+    };
+    store(0);
+#if SENS
+    __shared__ real slab[2][32 * (CH + 1)];
+    const int lane = threadIdx.x & 31;
+    real *sl = slab[threadIdx.x >> 5];
+    const long long tw = tr - lane; // the warp's first trajectory
+    // dk_{i-1} and the weighted sum of the stages, both laid out as A_k | B_k: column c < 2n of x at [i * 2n + c], column
+    // c of tau at [4 n^2 + i * n + c]
+    real Pk[NSENS], acc[NSENS], Dq[NSQ], Dqd[NSQ], Mi[NSQ];
+#endif
+    const real *tbase = tau + trc * R.tau_stride;
+#pragma unroll 1
+    for (int k = 0; k < R.K; k++) {
+        real tq[NJ], ks[NS], kp[NS];
+#pragma unroll
+        for (int j = 0; j < NJ; j++) tq[j] = tbase[(size_t)k * NJ + j];
+#pragma unroll 1
+        for (int s = 0; s < 4; s++) {
+            const real c = s == 0 ? (real)0 : s == 3 ? R.h : R.h2;
+            real xs[NS];
+#pragma unroll
+            for (int i = 0; i < NS; i++) xs[i] = s == 0 ? x[i] : fma(c, kp[i], x[i]);
+            real th[NJ], st[NJ], ct[NJ], res[NSQ + NJ], d[NJ];
+#pragma unroll
+            for (int j = 0; j < NJ; j++) th[j] = xs[j] + P.offset[j];
+            sincos_batch(th, P.trig, st, ct);
+            rne_row(P.C, P.grav, P.fext, st, ct, th, xs + NJ, tq, res);
+            ldlt_factor(res, d);
+            ldlt_solve(res, d, res + NSQ);
+            real kn[NS];
+#pragma unroll
+            for (int j = 0; j < NJ; j++) { kn[j] = xs[NJ + j]; kn[NJ + j] = res[NSQ + j]; }
+#if SENS
+#pragma unroll 1
+            for (int cc = 0; cc < NJ; cc++) { // M^-1, column by column, before the derivative row: the factors die here
+                real y[NJ];
+#pragma unroll
+                for (int i = 0; i < NJ; i++) y[i] = (real)(i == cc);
+                ldlt_solve(res, d, y);
+#pragma unroll
+                for (int i = 0; i < NJ; i++) Mi[i * NJ + cc] = y[i];
+            }
+            rne_deriv_row(P.C, P.grav, P.fext, st, ct, th, xs + NJ, kn + NJ, Dq, Dqd);
+#pragma unroll 1
+            for (int cc = 0; cc < NS; cc++) { // dqdd_dx = -M^-1 dtau_dx, in place
+                real *blk = cc < NJ ? Dq : Dqd;
+                const int cj = cc < NJ ? cc : cc - NJ;
+                real v[NJ];
+#pragma unroll
+                for (int i = 0; i < NJ; i++) v[i] = blk[i * NJ + cj];
+#pragma unroll
+                for (int i = 0; i < NJ; i++) {
+                    real y = (real)0;
+#pragma unroll
+                    for (int j = 0; j < NJ; j++) y = fma(-Mi[i * NJ + j], v[j], y);
+                    blk[i * NJ + cj] = y;
+                }
+            }
+            const real w = s == 0 || s == 3 ? (real)1 : (real)2;
+#pragma unroll 1
+            for (int col = 0; col < NS + NJ; col++) {
+                const bool xcol = col < NS;
+                const int base = xcol ? col : 4 * NSQ + col - NS, ld = xcol ? NS : NJ;
+                real sv[NS]; // the stage state's derivative along this column: e_col (x only) + c dt dk_{i-1}
+#pragma unroll
+                for (int i = 0; i < NS; i++) {
+                    const real e = (real)(xcol && i == col);
+                    sv[i] = s == 0 ? e : fma(c, Pk[base + i * ld], e);
+                }
+                real nv[NS];
+#pragma unroll
+                for (int r = 0; r < NJ; r++) {
+                    nv[r] = sv[NJ + r];
+                    real y = xcol ? (real)0 : Mi[r * NJ + col - NS];
+#pragma unroll
+                    for (int m = 0; m < NJ; m++) y = fma(Dq[r * NJ + m], sv[m], y);
+#pragma unroll
+                    for (int m = 0; m < NJ; m++) y = fma(Dqd[r * NJ + m], sv[NJ + m], y);
+                    nv[NJ + r] = y;
+                }
+#pragma unroll
+                for (int i = 0; i < NS; i++) {
+                    Pk[base + i * ld] = nv[i];
+                    acc[base + i * ld] = s == 0 ? nv[i] : fma(w, nv[i], acc[base + i * ld]);
+                }
+            }
+#endif
+#pragma unroll
+            for (int i = 0; i < NS; i++) {
+                ks[i] = s == 0 ? kn[i] : fma(s == 3 ? (real)1 : (real)2, kn[i], ks[i]);
+                kp[i] = kn[i];
+            }
+        }
+#pragma unroll
+        for (int i = 0; i < NS; i++) x[i] = fma(R.h6, ks[i], x[i]);
+        store(k + 1);
+#if SENS
+        // A_k = I + dt/6 (dk1 + 2 dk2 + 2 dk3 + dk4), B_k = dt/6 (...), drained CH reals per lane at a time
+#pragma unroll 1
+        for (int c0 = 0; c0 < NSENS; c0 += CH) {
+#pragma unroll 4
+            for (int e = 0; e < CH; e++) {
+                const int i = c0 + e;
+                if (i < NSENS) sl[lane * (CH + 1) + e] = fma(R.h6, acc[i], (real)(i < 4 * NSQ && i % (NS + 1) == 0));
+            }
+            __syncwarp();
+#pragma unroll 4
+            for (int r = 0; r < 32; r++) {
+                const int i = c0 + lane;
+                if (i < NSENS && tw + r < ntraj) {
+                    const size_t blk = (size_t)(tw + r) * R.K + k;
+                    const real v = sl[r * (CH + 1) + lane];
+                    if (i < 4 * NSQ) oA[blk * (4 * NSQ) + i] = v;
+                    else oB[blk * (2 * NSQ) + i - 4 * NSQ] = v;
+                }
+            }
+            __syncwarp();
+        }
+#endif
+    }
+}
+)B2KSRC";
+
 // ------------------------------------------------------------------ dynamic loading of NVRTC and the driver API
 struct Nvrtc {
     void *h = nullptr;
@@ -743,7 +906,9 @@ std::string build_source(const GenFn &gen, int n, int mode, int dtype, Program &
     p.n_mul = g.n_mul; p.n_fma = g.n_fma; p.n_add = g.n_add;
     const b2k_rne_op_s &op = B2K_RNE_OPS[mode];
     p.nin = op.nin;
-    const bool deriv = mode == B2K_GEN_RNE_DERIV || mode == B2K_GEN_ACCEL_DERIV, reg = mode == B2K_GEN_TREE_REGRESSOR;
+    // the rollout kernel (kRollout) runs the ACCEL / ACCEL_DERIV rows in its own 64-lane blocks: none of the tile sizing below
+    const bool roll = kernel_text == kRollout;
+    const bool deriv = !roll && (mode == B2K_GEN_RNE_DERIV || mode == B2K_GEN_ACCEL_DERIV), reg = mode == B2K_GEN_TREE_REGRESSOR;
     p.nout = op.out_row(0, n);
     p.nout2 = op.nout > 1 ? op.out_row(1, n) : 0; // tau (N, n) and the base wrench (N, 6)
     p.nres = mode == B2K_GEN_ACCEL ? n * n + n : p.nout + p.nout2;
@@ -777,6 +942,10 @@ std::string build_source(const GenFn &gen, int n, int mode, int dtype, Program &
         p.wpb = (int)std::min<size_t>(4, (220 * 1024) / warp_bytes);
         p.smem = (size_t)std::max(p.wpb, 1) * warp_bytes;
     }
+    if (roll) { // static shared memory only (the slab of the sensitivities); SENS selects the program
+        p.smem = 0; p.wpb = 2;
+        defs.push_back(std::string("-DSENS=") + (mode == B2K_GEN_ACCEL_DERIV ? "1" : "0"));
+    }
     if (p.smem > 220 * 1024) { p.why = "a tile of this operation does not fit the shared memory of an SM (" + std::to_string(p.smem) + " B)"; return std::string(); }
     int minb = (int)((200 * 1024) / (p.smem + 1024));
     // resident blocks to aim for (swept: fp64 96 registers / 5 blocks, fp32 64 registers / 8 blocks)
@@ -799,13 +968,15 @@ void compile(const GenFn &gen, int n, const Key &key, Program &p)
     Nvrtc *N = nvrtc();
     if (!N->h) { p.why = N->why; return; }
     std::vector<std::string> defs;
-    const bool fdyn = std::get<0>(key) / 100 == 2;
+    const bool fdyn = std::get<0>(key) / 100 == 2, roll = std::get<0>(key) / 100 == 3;
     if (fdyn) p.entry = "k_fdyn";
+    else if (roll) p.entry = "k_rollout";
     else if (mode == B2K_GEN_RNE_DERIV || mode == B2K_GEN_ACCEL_DERIV) p.entry = "k_rne_deriv_spec";
     else if (mode == B2K_GEN_TREE_REGRESSOR) p.entry = "k_rne_regressor_spec";
-    const std::string src = build_source(gen, n, mode, dtype, p, defs, fdyn ? kFdyn : nullptr);
+    const std::string src = build_source(gen, n, mode, dtype, p, defs, fdyn ? kFdyn : roll ? kRollout : nullptr);
     if (src.empty()) return;
     std::vector<std::string> opts = {"--gpu-architecture=sm_90a", "--std=c++17"};
+    if (roll) opts.push_back("--fmad=false"); // no contraction: both rollout programs round the states alike
     if (getenv("B2K_RNE_SPEC_LINEINFO")) opts.push_back("-lineinfo");
     for (auto &d : defs) opts.push_back(d);
     std::vector<const char *> copts;
@@ -1039,8 +1210,11 @@ extern "C" int b2k_rne_spec_info(b2k_rne_t r, int mode, int dtype, const double 
             const bool ug = gm >= 0 && gm < B2K_GEN_NOPS && B2K_RNE_OPS[gm].grav;
             const Key key(mode, dtype, ug ? grav_mask_of(grav) : 0, has_fext);
             const Key gkey(gm, dtype, ug ? grav_mask_of(grav) : 0, has_fext);
-            Program *p = get_program(static_cast<SpecCache *>(r->spec), dh_gen(r, gkey), r->n, key);
-            if (!p || !p->ok) s = std::string("generic (") + (p ? p->why : "no cache") + ")";
+            // b2k_rne_derivatives / b2k_rne_accel_derivatives run the generic kernel; their generated rows serve rollouts only
+            const bool generic = mode == B2K_GEN_RNE_DERIV || mode == B2K_GEN_ACCEL_DERIV;
+            Program *p = generic ? nullptr : get_program(static_cast<SpecCache *>(r->spec), dh_gen(r, gkey), r->n, key);
+            if (generic) s = "generic (the derivatives of DH arms are served by the generic kernel)";
+            else if (!p || !p->ok) s = std::string("generic (") + (p ? p->why : "no cache") + ")";
             else {
                 char t[256];
                 snprintf(t, sizeof(t), "%s<%s,n=%d,mode=%d>: %d mul + %d fma + %d add per row, %d constants, %d regs, %zu B smem/block, %d tiles/warp",
@@ -1093,14 +1267,18 @@ extern "C" int b2k_tree_destroy(b2k_tree_t t)
     return B2K_OK;
 }
 
-static Program *tree_program(b2k_tree_t t, int mode, int dtype, int gmask)
+static GenFn tree_gen(b2k_tree_t t, int mode, int gmask)
 {
-    const Key key(100 + mode, dtype, gmask, 0);
-    return get_program(static_cast<SpecCache *>(t->spec), [t, mode, gmask](b2k_gen_out &g) {
+    return [t, mode, gmask](b2k_gen_out &g) {
         b2k_gen_opts o;
         o.mode = mode; o.grav_mask = gmask; o.has_fext = 0;
         return b2k_tree_generate(t, o, g);
-    }, t->n, key);
+    };
+}
+
+static Program *tree_program(b2k_tree_t t, int mode, int dtype, int gmask)
+{
+    return get_program(static_cast<SpecCache *>(t->spec), tree_gen(t, mode, gmask), t->n, Key(100 + mode, dtype, gmask, 0));
 }
 
 // Robot.rne (mode 0), the operations DynamicsMixin builds on it (modes 1-5: inertia, gravload, itorque, coriolis, accel),
@@ -1285,6 +1463,15 @@ extern "C" int b2k_tree_codegen(b2k_tree_t t, int op, int grav_mask, char *src, 
 extern "C" int b2k_tree_info(b2k_tree_t t, int op, int dtype, const double *grav, char *buf, int64_t cap)
 {
     if (!t || !buf || cap < 1) { b2k_set_error("b2k_tree_info: bad arguments"); return B2K_ERR_INVALID; }
+    if (op == 300 + B2K_GEN_ACCEL || op == 300 + B2K_GEN_ACCEL_DERIV) { // the rollout kernels (b2k_tree_rollout)
+        const int gm = grav_mask_of(grav);
+        Program *p = get_program(static_cast<SpecCache *>(t->spec), tree_gen(t, op - 300, gm), t->n, Key(op, dtype, gm, 0));
+        if (!p || !p->ok) snprintf(buf, (size_t)cap, "unavailable (%s)", p ? p->why.c_str() : "no cache");
+        else
+            snprintf(buf, (size_t)cap, "k_rollout<%s,tree n=%d,mode=%d>: %d mul + %d fma + %d add per stage, %d constants, %d regs",
+                     dtype == B2K_F64 ? "double" : "float", t->n, op, p->n_mul, p->n_fma, p->n_add, p->nc, p->regs);
+        return B2K_OK;
+    }
     if (op < B2K_GEN_RNE || (op > B2K_GEN_ACCEL_DERIV && op != B2K_GEN_TREE_REGRESSOR) || op == B2K_GEN_RNE_WRENCH) {
         b2k_set_error("b2k_tree_info: operation %d is not one of B2K_DYN_*", op);
         return B2K_ERR_INVALID;
@@ -1395,4 +1582,88 @@ extern "C" int b2k_tree_fdyn(b2k_tree_t t, int dtype, const void *q0, const void
     return fdyn_run("b2k_tree_fdyn", static_cast<SpecCache *>(t->spec), gen, t->n, nullptr, dtype, q0, qd0, ntraj, T, grav, torque_mode,
                     tau, tau_rows, kp, kd, qstar, rtol, atol, max_step, first_step, dt, grid, M, out_t, out_q, out_qd, out_count,
                     out_status, stream);
+}
+
+// ------------------------------------------------------------------ C ABI: fixed-step rollouts with sensitivities
+// gen(mode) runs the code generator of the robot for B2K_GEN_ACCEL (states only) or B2K_GEN_ACCEL_DERIV (sensitivities).
+static int rollout_run(const char *fn, SpecCache *cache, const std::function<GenFn(int)> &gen, int n, const double *offset,
+                       int dtype, const void *q0, const void *qd0, int64_t N, int32_t K, double dt, const double *grav,
+                       const void *tau, int64_t tau_stride, void *q, void *qd, void *A, void *B, void *stream)
+{
+    if (dtype != B2K_F32 && dtype != B2K_F64) { b2k_set_error("%s: dtype must be B2K_F32 or B2K_F64", fn); return B2K_ERR_INVALID; }
+    if (N < 0) { b2k_set_error("%s: N is negative", fn); return B2K_ERR_INVALID; }
+    if (K < 1) { b2k_set_error("%s: K = %d must be at least 1", fn, (int)K); return B2K_ERR_INVALID; }
+    if (!(std::isfinite(dt) && dt > 0)) { b2k_set_error("%s: dt = %g must be finite and positive", fn, dt); return B2K_ERR_INVALID; }
+    if (!grav) { b2k_set_error("%s: grav is NULL (pass MINUS the robot's gravity, as for accel)", fn); return B2K_ERR_INVALID; }
+    if (tau_stride != 0 && tau_stride != (int64_t)K * n) {
+        b2k_set_error("%s: tau_stride = %lld must be 0 (one sequence) or K n = %lld (one per trajectory)", fn, (long long)tau_stride,
+                      (long long)K * n);
+        return B2K_ERR_INVALID;
+    }
+    if (!A != !B) { b2k_set_error("%s: A and B must both be NULL (states only) or both be given (sensitivities)", fn); return B2K_ERR_INVALID; }
+    const int es = dtype == B2K_F64 ? 8 : 4;
+    int rc;
+    if ((rc = b2k_check_array(fn, "q0", q0, N, es)) || (rc = b2k_check_array(fn, "tau", tau, N, es)) ||
+        (rc = b2k_check_array(fn, "q", q, N, es)) || (rc = b2k_check_array(fn, "qd", qd, N, es)))
+        return rc;
+    if (qd0 && (rc = b2k_check_array(fn, "qd0", qd0, N, es))) return rc;
+    const bool sens = A != nullptr;
+    if (sens && ((rc = b2k_check_array(fn, "A", A, N, es)) || (rc = b2k_check_array(fn, "B", B, N, es)))) return rc;
+    if (N == 0) return B2K_OK;
+    const int mode = sens ? B2K_GEN_ACCEL_DERIV : B2K_GEN_ACCEL;
+    Program *p = get_program(cache, gen(mode), n, Key(300 + mode, dtype, grav_mask_of(grav), 0));
+    if (!p || !p->ok) { b2k_set_error("%s: the rollout kernel could not be built (%s)", fn, p ? p->why.c_str() : "no cache"); return B2K_ERR_INVALID; }
+    B2K_ON_DEVICE_OF(q0);
+    CUfunction f;
+    {
+        std::lock_guard<std::mutex> lk(cache->mu);
+        if (get_function(p, &f)) { b2k_set_error("%s: %s", fn, p->why.c_str()); return B2K_ERR_CUDA; }
+    }
+    std::vector<unsigned char> pb = spec_params(p, n, dtype, offset, grav, nullptr);
+    // RollP { real h2, h, h6; int K; long long tau_stride; }
+    std::vector<unsigned char> rb(3 * es + 4 + 8 + 8, 0);
+    const double hv[3] = {dt / 2, dt, dt / 6};
+    for (int k = 0; k < 3; k++) {
+        if (es == 8) memcpy(&rb[8 * k], &hv[k], 8);
+        else { const float v = (float)hv[k]; memcpy(&rb[4 * k], &v, 4); }
+    }
+    const size_t ko = 3 * es, so = (ko + 4 + 7) & ~(size_t)7;
+    memcpy(&rb[ko], &K, 4);
+    memcpy(&rb[so], &tau_stride, 8);
+    long long nt = N;
+    void *args[11] = {pb.data(), rb.data(), (void *)&q0, (void *)&qd0, (void *)&tau, (void *)&q, (void *)&qd, (void *)&A, (void *)&B, (void *)&nt, nullptr};
+    const unsigned grid = (unsigned)((N + 63) / 64);
+    CUresult cr = driver()->LaunchKernel(f, grid, 1, 1, 64, 1, 1, 0, (CUstream)stream, args, nullptr);
+    if (cr != CUDA_SUCCESS) {
+        const char *es2 = nullptr;
+        driver()->GetErrorString(cr, &es2);
+        b2k_set_error("cuLaunchKernel(k_rollout): %s", es2 ? es2 : "?");
+        return B2K_ERR_CUDA;
+    }
+    b2k_count_launch();
+    return B2K_OK;
+}
+
+extern "C" int b2k_rne_rollout(b2k_rne_t r, int dtype, const void *q0, const void *qd0, int64_t N, int32_t K, double dt,
+                               const double *grav, const void *tau, int64_t tau_stride, void *q, void *qd, void *A, void *B, void *stream)
+{
+    const char *fn = "b2k_rne_rollout";
+    if (!r) { b2k_set_error("%s: rne handle is NULL", fn); return B2K_ERR_INVALID; }
+    for (int j = 0; j < r->n; j++)
+        if ((int)r->L[j][4] != 0) { b2k_set_error("%s: joint %d is prismatic; rollouts serve all-revolute arms", fn, j); return B2K_ERR_INVALID; }
+    double offset[B2K_MAX_JOINTS];
+    for (int j = 0; j < r->n; j++) offset[j] = r->L[j][5];
+    const int gm = grav_mask_of(grav);
+    return rollout_run(fn, static_cast<SpecCache *>(r->spec), [r, dtype, gm](int mode) { return dh_gen(r, Key(mode, dtype, gm, 0)); },
+                       r->n, offset, dtype, q0, qd0, N, K, dt, grav, tau, tau_stride, q, qd, A, B, stream);
+}
+
+extern "C" int b2k_tree_rollout(b2k_tree_t t, int dtype, const void *q0, const void *qd0, int64_t N, int32_t K, double dt,
+                                const double *grav, const void *tau, int64_t tau_stride, void *q, void *qd, void *A, void *B, void *stream)
+{
+    const char *fn = "b2k_tree_rollout";
+    if (!t) { b2k_set_error("%s: tree handle is NULL", fn); return B2K_ERR_INVALID; }
+    const int gm = grav_mask_of(grav);
+    return rollout_run(fn, static_cast<SpecCache *>(t->spec), [t, gm](int mode) { return tree_gen(t, mode, gm); }, t->n, nullptr,
+                       dtype, q0, qd0, N, K, dt, grav, tau, tau_stride, q, qd, A, B, stream);
 }

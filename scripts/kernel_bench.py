@@ -1011,3 +1011,103 @@ if any(want(c) for c in TREG_CASES):
                 report(c_gram, ms, N, 4 * n * es, dict(card, fp64_tflops=round(flops / (ms * 1e-3) / 1e12, 2),
                                                       frac_of_34TFLOPs=round(flops / (ms * 1e-3) / 34e12, 4)))
             del q0, qd0, qdd0, tau0
+
+# Fixed-step RK4 rollouts with discrete-time sensitivities (DHRobot.rollout / Robot.rollout: b2k_rne_rollout,
+# b2k_tree_rollout): Puma560 and PandaMDH (DH) and the UR10 assembled as an ETS robot (tree), N = 16384 trajectories of
+# K = 64 steps, one shared torque sequence.  Bytes per trajectory = what the kernel must write: q and qd, 2n (K + 1) reals,
+# plus K 6 n^2 reals of A_k | B_k with sensitivities; reported against 3.35 TB/s.  step_route is what a user has without
+# the kernel, timed in the same call with both routes alternated: per step four accel and four accel_derivatives launches
+# and the torch composition of the RK4 stages.  The card's name and power limit are read in the same run.
+ROLL_CASES = [f"rollout_{r}_{t}_{s}" for r in ("puma", "pandamdh", "ur10tree") for t in ("f64", "f32") for s in ("states", "sens")]
+if any(want(c) for c in ROLL_CASES):
+    import subprocess
+
+    try:
+        plim = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True,
+                              text=True, timeout=30).stdout.strip()
+    except Exception as e:  # the figure is context, the timing does not depend on it
+        plim = f"unavailable ({type(e).__name__})"
+    card = {"gpu": torch.cuda.get_device_name(0), "power_limit": plim}
+    from oracle import chains as ch  # noqa: E402
+
+    def dh_as_tree(dh):
+        """A standard-DH link table as an ETS robot: point masses at the links' centres of mass (Robot.rne's model)."""
+        links, prev = [], rtb.ETS()
+        for j, l in enumerate(dh):
+            post = rtb.ETS()
+            for kind, v in (("tz", l["d"]), ("tx", l["a"]), ("Rx", l["alpha"])):
+                if v != 0:
+                    post = post * getattr(rtb.ET, kind)(v)
+            Tpost = np.eye(4)
+            for et in post:
+                Tpost = Tpost @ et.A()
+            r_in = Tpost[:3, :3] @ np.asarray(l["r"], dtype=float) + Tpost[:3, 3]
+            links.append(rtb.Link(prev * rtb.ET.Rz(), name=f"l{j}", parent=links[-1] if links else None, m=l["m"], r=r_in))
+            prev = post
+        links.append(rtb.Link(prev, name="tool", parent=links[-1]))
+        return rtb.Robot(links)
+
+    def step_route(rob, q0, qd0, tau, h, sens):
+        """RK4 with chained sensitivities from the public accel / accel_derivatives, composed with torch."""
+        n = rob.n
+        x = torch.cat([q0, qd0], 1)
+        N = x.shape[0]
+        I = torch.eye(2 * n, dtype=x.dtype, device=x.device)
+        qs, As, Bs = [x], [], []
+        for k in range(tau.shape[0]):
+            t = tau[k].expand(N, n).contiguous()
+            ks, dxs, dus = [], [], []
+            for c in (0.0, 0.5, 0.5, 1.0):
+                xs = x if not ks else x + (c * h) * ks[-1]
+                q, qd = xs[:, :n].contiguous(), xs[:, n:].contiguous()
+                ks.append(torch.cat([qd, rob.accel(q, qd, t)], 1))
+                if sens:
+                    aq, aqd, at = rob.accel_derivatives(q, qd, t)
+                    J = torch.zeros((N, 2 * n, 2 * n), dtype=x.dtype, device=x.device)
+                    J[:, :n, n:] = torch.eye(n, dtype=x.dtype, device=x.device)
+                    J[:, n:, :n], J[:, n:, n:] = aq, aqd
+                    dxs.append(J if not dxs else J @ (I + (c * h) * dxs[-1]))
+                    Mt = torch.cat([torch.zeros_like(at), at], 1)
+                    dus.append(Mt if not dus else J @ ((c * h) * dus[-1]) + Mt)
+            x = x + (h / 6) * (ks[0] + 2 * ks[1] + 2 * ks[2] + ks[3])
+            qs.append(x)
+            if sens:
+                As.append(I + (h / 6) * (dxs[0] + 2 * dxs[1] + 2 * dxs[2] + dxs[3]))
+                Bs.append((h / 6) * (dus[0] + 2 * dus[1] + 2 * dus[2] + dus[3]))
+        return qs, As, Bs
+
+    NR, KR, HR = 16384, 64, 0.005
+    rngr = np.random.default_rng(19)
+    robots = (("puma", rtb.models.Puma560()), ("pandamdh", rtb.models.PandaMDH()), ("ur10tree", dh_as_tree(ch.ur10_links())))
+    for rname, rob in robots:
+        n = rob.n
+        for dt in (np.float64, np.float32):
+            tag = "f64" if dt == np.float64 else "f32"
+            es = np.dtype(dt).itemsize
+            q0 = torch.from_numpy(rngr.uniform(-1.5, 1.5, (NR, n)).astype(dt)).to(dev)
+            qd0 = torch.from_numpy(rngr.uniform(-1, 1, (NR, n)).astype(dt)).to(dev)
+            tau = torch.from_numpy(rngr.normal(size=(KR, n)).astype(dt)).to(dev)
+            for sname, sens in (("states", False), ("sens", True)):
+                case = f"rollout_{rname}_{tag}_{sname}"
+                if not want(case):
+                    continue
+                # device memory the first call takes beyond torch's allocator: the module and the local memory the
+                # driver reserves for the kernel's per-thread stack (a fresh program per case: dtype / sensitivities)
+                torch.cuda.synchronize()
+                free0, res0 = torch.cuda.mem_get_info()[0], torch.cuda.memory_reserved()
+                rob.rollout(q0, tau, HR, qd0=qd0, sensitivities=sens)
+                torch.cuda.synchronize()
+                driver_mb = ((free0 - torch.cuda.mem_get_info()[0]) - (torch.cuda.memory_reserved() - res0)) / 2**20
+                ms_k, ms_r = [], []
+                for _ in range(2):  # alternate the two routes, so that both see the same clocks
+                    ms_k.append(timeit(lambda i: rob.rollout(q0, tau, HR, qd0=qd0, sensitivities=sens), 1))
+                    ms_r.append(timeit(lambda i: step_route(rob, q0, qd0, tau, HR, sens), 1))
+                ms_k, ms_r = min(ms_k), min(ms_r)
+                bpt = (2 * n * (KR + 1) + (KR * 6 * n * n if sens else 0)) * es
+                report(case, ms_k, NR, bpt, dict(card, steps=KR, bytes_written_per_s=round(bpt * NR / (ms_k * 1e-3), 0),
+                                                 frac_of_3p35TBps=round(bpt * NR / (ms_k * 1e-3) / 3.35e12, 4),
+                                                 step_route_ms=round(ms_r, 3), step_route_launches=KR * (8 if sens else 4),
+                                                 speedup_vs_step_route=round(ms_r / ms_k, 2),
+                                                 driver_reserved_MB_first_call=round(driver_mb, 1),
+                                                 kernel=rob.rne_kernel_info(dtype=dt, op="rollout").split("\n")[int(sens)]))
+            del q0, qd0, tau
